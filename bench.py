@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- K-FAC hot path on ResNet-50 (ImageNet-shaped synthetic data).
 
-    python bench.py --gpus N --steps K --warmup W            (own arm, B200)
+    python bench.py --gpus N --steps K --warmup W            (own arm, H100)
+    python bench.py ... --dump-outputs DIR                    (also write the last timed step's outputs as .npy)
     python bench.py --impl reference --gpus N --steps K ...   (CPU reference arm)
 
 A "step" is one full training iteration of the data-parallel K-FAC hot path:
@@ -54,6 +55,9 @@ def parse():
     ap.add_argument('--no-parity', action='store_true', help='skip the untimed parity step after the timed region')
     ap.add_argument('--no-stationary', action='store_true', help='skip the extra stationary-input timing')
     ap.add_argument('--budget-s', type=float, default=240.0, help='reference arm wall-clock budget')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write what the last timed step computed (loss, a seeded sample of the preconditioned '
+                         'gradients and of the updated parameters) as DIR/<name>.npy')
     return ap.parse_args()
 
 
@@ -165,8 +169,8 @@ def algorithmic_work(pre):
 
 
 def tc_gemm_microbench(lib, dev, n=4096, iters=10):
-    """Isolated timing of the tcgen05 GEMM engine (the kernel under K3/K5/K8):
-    D = A B^T, n^3 problem, fp32 operands (3 x 64 MB > 126 MB L2), CUDA events."""
+    """Isolated timing of the wgmma GEMM engine (the kernel under K3/K5/K8):
+    D = A B^T, n^3 problem, fp32 operands (3 x 64 MB > 50 MB L2), CUDA events."""
     A = torch.randn(n, n, device=dev)
     B = torch.randn(n, n, device=dev)
     D = torch.empty(n, n, device=dev)
@@ -189,6 +193,30 @@ def tc_gemm_microbench(lib, dev, n=4096, iters=10):
 
 
 # ------------------------------------------------------------------ own arm
+DUMP_SAMPLE = 1 << 22      # entries kept of each long output vector (16 MB as float32)
+
+
+def snapshot_outputs(model, loss):
+    """What a caller of the timed path holds after its last step: the loss, the preconditioned gradients and the
+    parameters after the SGD update.  The two vectors (25.6 M entries each for ResNet-50) are sampled at DUMP_SAMPLE
+    fixed positions drawn from a seeded generator, so that two runs can be compared entry for entry."""
+    params = list(model.parameters())
+    g = torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).detach().reshape(-1) for p in params])
+    w = torch.cat([p.detach().reshape(-1) for p in params])
+    if g.numel() > DUMP_SAMPLE:
+        idx = torch.randperm(g.numel(), generator=torch.Generator().manual_seed(1234))[:DUMP_SAMPLE].sort().values
+        idx = idx.to(g.device)
+        g, w = g[idx], w[idx]
+    return {'loss': loss.detach().double().reshape(1).cpu(), 'precond_grads': g.float().cpu(), 'params': w.float().cpu()}
+
+
+def write_outputs(outputs, out_dir):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in outputs.items():
+        np.save(os.path.join(out_dir, name + '.npy'), t.numpy())
+
+
 def parity_step(pre, model, world, rank, dev, hp):
     """One UNTIMED step after the timed region, checked against the CPU oracle (test infrastructure used as
     the checker only; nothing here is timed or shipped).  ResNets hold BatchNorm, so the concatenated-batch
@@ -297,6 +325,7 @@ def run_b200(args):
     copy_stream = torch.cuda.Stream(device=dev)
     h2d_bytes = host[0][0].numel() * 4 + host[0][1].numel() * 8
     counter = {'i': 0}
+    last = {}
 
     def stage(i):
         """Issue the H2D copy of batch i on the copy stream (double-buffered prefetch, like a data loader
@@ -327,6 +356,7 @@ def run_b200(args):
         loss.backward()
         pre.step()
         opt.step()
+        last['loss'] = loss
         if e2e:
             loss_host.copy_(loss.detach().reshape(1), non_blocking=True)
         return nxt
@@ -361,6 +391,8 @@ def run_b200(args):
     timer.enabled = True
     ms_dev, launches = timed_loop(args.steps, False)
     timer.enabled = False
+    # outputs of the last timed step, taken before any later (extra) step changes the model
+    outputs = snapshot_outputs(model, last['loss']) if args.dump_outputs and rank == 0 else None
     phase_ms = timer.totals_ms()
     ms_e2e, _ = timed_loop(args.steps, True)
     clocks = sampler.stop()
@@ -426,8 +458,9 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:  # noqa: BLE001
         pass
-    tensor_peak = float(peaks.get('bf16_tflops_sustained', 1400.0))
-    peak_src = 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)' if peaks else 'fallback'
+    # without a measured peak of this card: the H100 SXM data sheet (dense BF16, 700 W); the card may be set lower
+    tensor_peak = float(peaks.get('bf16_tflops_sustained', 989.0))
+    peak_src = 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)' if peaks else 'H100 SXM data sheet, dense bf16'
     # dominant phase: the batched eigensolver; at N>1 each rank solves only its
     # KAISA share, the roofline line is reported for rank 0's local phase time.
     inv_ms = phase_ms.get('compute_inverses', 0.0) / K
@@ -443,27 +476,7 @@ def run_b200(args):
             my_bytes += 12.0 * l.g_dim ** 2
     achieved = (my_eig / (inv_ms / 1e3) / 1e12) if inv_ms > 0 else 0.0
     gemm_tf, gemm_ms = tc_gemm_microbench(lib, dev) if rank == 0 else (0.0, 0.0)
-    burst_peak = float(peaks.get('bf16_tflops', 1590.0))
-    traffic = None
-    try:   # dram bytes per kfac_eigh_batched call, from the committed ncu capture of this command (N = 1)
-        tr = json.load(open(os.path.join(ROOT, 'profiles', 'eigh_traffic.json')))
-        if world == 1 and tr.get('model') == args.model:
-            traffic = tr.get('dram_bytes_per_call')
-    except Exception:  # noqa: BLE001
-        pass
-    # the same launch seen from the memory side: the tridiagonalisation streams the trailing matrices once per column,
-    # so the MEASURED DRAM bytes of the call (not the 12 n^2 algorithmic ones) over its time, against the measured copy
-    # bandwidth, say how far the dominant kernel is from the HBM bound
-    hbm_view = None
-    try:
-        if traffic and inv_ms > 0:
-            hbm_peak = float(peaks.get('hbm_gbs', 7700.0))
-            gbs = float(traffic) / (inv_ms / 1e3) / 1e9
-            hbm_view = {'bound': 'hbm', 'achieved': gbs, 'peak': hbm_peak, 'unit': 'GB/s', 'frac': gbs / hbm_peak,
-                        'note': 'measured dram bytes of one kfac_eigh_batched call (profiles/eigh_traffic.json) / its '
-                                'CUDA-event time; 90 % of the bytes belong to sytrd_kernel (profiles/r02_launches_eigh_batch.md)'}
-    except Exception:  # noqa: BLE001
-        hbm_view = None
+    burst_peak = float(peaks.get('bf16_tflops', 989.0))
     out = {
         'metric': metric_name(args.model), 'value': value, 'unit': 'images/s', 'n_gpus': world, 'steps': K,
         'warmup': W, 'ms_per_step': ms_dev / K, 'higher_is_better': True,
@@ -471,7 +484,7 @@ def run_b200(args):
         'data': 'synthetic',
         'config': {'workload': wl, 'global_batch': B * world, 'grad_worker_fraction': frac,
                    'parallelism': f'dp{world}', 'distinct_batches': NB,
-                   'l2': 'inputs+factors >> 126 MB L2 (activations 1.4 GB, factors 615 MB)'},
+                   'l2': 'inputs+factors >> 50 MB L2 (activations 1.4 GB, factors 615 MB)'},
         'clocks': clocks,
         'e2e': {'value': e2e_value, 'unit': 'images/s', 'ms_per_step': ms_e2e / K,
                 'h2d_bytes_per_step': h2d_bytes, 'd2h_bytes_per_step': 4,
@@ -493,23 +506,22 @@ def run_b200(args):
         'roofline': {'kernel': 'kfac_eigh_batched: one call per step over all factors of this rank '
                                + EIGH_KERNEL_NOTE,
                      'bound': 'tensor', 'achieved': achieved, 'peak': tensor_peak, 'unit': 'TFLOP/s',
-                     'frac': achieved / tensor_peak if tensor_peak else None, 'traffic': traffic,
+                     'frac': achieved / tensor_peak if tensor_peak else None, 'traffic': None,
                      'algorithmic_bytes': my_bytes,
                      'ms_per_launch': inv_ms,
                      'convention': 'algorithmic 9 n^3 flop per eigendecomposition (SURVEY.md 8d) summed over the '
-                                   "rank's factors / CUDA-event time of the call; algorithmic bytes 3*4*n^2 per factor; "
-                                   'traffic = dram__bytes_read+write of all kernels of one call (profiles/eigh_traffic.json)',
+                                   "rank's factors / CUDA-event time of the call; algorithmic bytes 3*4*n^2 per factor",
                      'peak_source': peak_src},
-        'roofline_hbm_view': hbm_view,
         # the GEMM engine all tensor-core kernels instantiate, timed alone on a 4096^3 problem
-        'roofline_engine': {'kernel': 'tc::pipeline_kernel<GemmPolicy> (tcgen05 3xTF32 GEMM engine), 4096^3, isolated',
+        'roofline_engine': {'kernel': 'tc::pipeline_kernel<GemmPolicy> (wgmma 3xTF32 GEMM engine), 4096^3, isolated',
                             'bound': 'tensor', 'achieved': gemm_tf, 'peak': burst_peak, 'unit': 'TFLOP/s',
                             'frac': gemm_tf / burst_peak if burst_peak else None, 'traffic': None,
                             'ms_per_launch': gemm_ms,
                             'convention': 'algorithmic fp32 flops 2*M*N*K per launch / CUDA-event time; every product is '
                                           'issued as 3 TF32 MMAs, so the tensor pipe executes 3x these flops at the TF32 '
                                           'rate (= half the bf16 rate the peak was measured with)',
-                            'peak_source': 'measured (MEASURED_PEAKS.json bf16_tflops, burst)' if peaks else 'fallback 1590'},
+                            'peak_source': 'measured (MEASURED_PEAKS.json bf16_tflops, burst)' if peaks else
+                                           'H100 SXM data sheet, dense bf16'},
         'algorithmic_flops_per_step': {'eigh_9n3': eig_flops, 'precondition_4ga(g+a)': prec_flops},
     }
     if not args.no_parity:
@@ -522,6 +534,8 @@ def run_b200(args):
         pre.overlap_factor_allreduce = True
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         out['cpu_baseline'] = cpu_baseline(args, steps=2, warmup=1, budget=150.0)
+    if outputs is not None:
+        write_outputs(outputs, args.dump_outputs)
     if rank == 0:
         print(json.dumps(out))
     if world > 1:
@@ -560,7 +574,7 @@ REF_DIR = os.path.join(ROOT, 'oracle', '_ref')
 
 def reference_kind():
     """'reference' when the unmodified reference package was installed into oracle/_ref by
-    oracle/build_ref.sh (it travels to the GPU box with the snapshot), else 'port' (the oracle)."""
+    oracle/build_ref.sh, else 'port' (the oracle)."""
     return 'reference' if os.path.isdir(os.path.join(REF_DIR, 'kfac')) else 'port'
 
 

@@ -1,5 +1,5 @@
 /*
- * kfac_b200.h -- C ABI of the B200-native K-FAC hot path (libkfac_b200.so).
+ * kfac_b200.h -- C ABI of the H100-native (sm_90a) K-FAC hot path (libkfac_b200.so).
  *
  * The reference (gpauloski/kfac-pytorch v0.4.2) has no FFI: its hot path is a
  * chain of torch calls inside Python classes.  This header is the boundary a
@@ -58,8 +58,10 @@ long long kfac_launch_count(void);
  * (kfac/layers/modules.py:123-141) + append_bias_ones (utils.py:8-15):
  * x is (rows, features) row-major; d = features + append_ones. */
 /* ws may be NULL (SIMT kernel).  With a workspace of kfac_factor_linear_workspace_bytes()
- * (non-zero for tall inputs: rows >= 512, features >= 128) the activations are transposed
- * once into a feature-major matrix and the SYRK runs on the tcgen05 engine. */
+ * tall inputs (rows >= 512, features >= 128) are transposed once into a feature-major matrix
+ * and the SYRK runs on the wgmma engine; the workspace also holds the per-split partials of a
+ * reduction split over the SMs.  Every factor call is deterministic (partials are added in a
+ * fixed order; without a workspace the reduction runs unsplit). */
 size_t kfac_factor_linear_workspace_bytes(int64_t rows, int features, int append_ones);
 int kfac_factor_linear(const void* x, int dtype, int64_t rows, int features,
                        int append_ones, float scale, float* acc, void* ws,
@@ -110,7 +112,7 @@ int kfac_factor_ema(const kfac_ema_item* items, int count, float alpha,
  *   n <= 128  two-sided Jacobi, the whole matrix in the shared memory of one CTA;
  *   n  > 128  Householder tridiagonalisation (one persistent kernel for the batch, CTA groups per
  *             matrix) -> divide and conquer on the tridiagonal matrix -> block-reflector
- *             back-transformation (grouped tcgen05 GEMMs) -- the stages of LAPACK's ssyevd. */
+ *             back-transformation (grouped wgmma GEMMs) -- the stages of LAPACK's ssyevd. */
 typedef struct kfac_eigh_item {
   const float* F; /* n x n dense (ld = n) */
   float* Q;       /* n x n, leading dimension ldq */
@@ -232,7 +234,7 @@ int kfac_gemm_f32(const float* A, int64_t sa_m, int64_t sa_k, const float* B,
                   int64_t sb_k, int64_t sb_n, float* C, int64_t ldc, int M,
                   int N, int K, float alpha, float beta, void* stream);
 
-/* Tensor-core engine (tcgen05 / TMA, 3xTF32 split, fp32 accumulate in TMEM):
+/* Tensor-core engine (wgmma / TMA, 3xTF32 split, fp32 accumulate in registers):
  * D (+)= alpha * A B^T with A (M x K) and B (N x K) row-major fp32, lda/ldb
  * multiples of 4 and 16-byte aligned bases.  atomic != 0: accumulate into D
  * with split-K (`splits` <= 0: automatic).  Exposed for tests / profiling. */

@@ -1,7 +1,7 @@
 """ctypes binding of libkfac_b200.so (C ABI declared in include/kfac_b200.h).
 
 There is NO CPU fallback: if the shared library is missing this module raises
-at import of the symbols, and every compute entry point raises if no sm_100
+at import of the symbols, and every compute entry point raises if no sm_90
 device is current.
 """
 from __future__ import annotations
@@ -100,7 +100,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise KFACNativeError(
             f'{LIB_PATH} not found: build it with `python -c "import __graft_entry__ as g; g.build()"` '
-            '(nvcc, sm_100a). kfac_b200 has no CPU / PyTorch fallback.')
+            '(nvcc, sm_90a). kfac_b200 has no CPU / PyTorch fallback.')
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing
@@ -139,5 +139,5 @@ def stream_ptr() -> int:
 def require_device(t: torch.Tensor) -> None:
     if not t.is_cuda:
         raise KFACNativeError(
-            'kfac_b200 runs on CUDA (sm_100a) tensors only; got a tensor on '
+            'kfac_b200 runs on CUDA (sm_90a) tensors only; got a tensor on '
             f'{t.device}. There is no CPU fallback.')

@@ -1,4 +1,4 @@
-"""Step orchestrator of the B200-native K-FAC preconditioner.
+"""Step orchestrator of the H100-native K-FAC preconditioner.
 
 Mirrors `BaseKFACPreconditioner` (kfac/base_preconditioner.py:22-479): same
 constructor keywords, properties, hooks, `step()`, `state_dict()`,
@@ -6,7 +6,7 @@ constructor keywords, properties, hooks, `step()`, `state_dict()`,
 same externally visible schedule (`steps % factor_update_steps`,
 `steps % inv_update_steps`, micro-batch accumulation).
 
-What is different underneath (B200-first):
+What is different underneath (H100-first):
   * all per-layer tensors are views into a few contiguous HBM arenas
     (factors | micro-batch sums | second-order data | preconditioned grads);
   * every phase of `step()` is ONE call into libkfac_b200.so over all layers
@@ -50,7 +50,7 @@ class _Scratch:
 
 def _storage_numel(shape: tuple[int, ...]) -> int:
     """Floats reserved for one arena entry; always a multiple of 4 so that every
-    entry starts 16-byte aligned (TMA / tcgen05 GEMM operands)."""
+    entry starts 16-byte aligned (TMA / wgmma GEMM operands)."""
     if len(shape) == 2:
         return shape[0] * _cabi.ld4(shape[1])
     return _cabi.ld4(shape[0])
@@ -145,7 +145,7 @@ def _release_peer_memory(peer_bases: list[int], own_ptr: int) -> None:
 
 
 class BaseKFACPreconditioner:
-    """K-FAC distributed gradient preconditioner (native sm_100a hot path)."""
+    """K-FAC distributed gradient preconditioner (native sm_90a hot path)."""
 
     def __init__(
         self,
@@ -270,7 +270,7 @@ class BaseKFACPreconditioner:
             device = next(iter(self._layers.values()))[1].module.device if self._layers else torch.device('cuda')
         if device.type != 'cuda':
             raise _cabi.KFACNativeError(
-                f'kfac_b200 needs the model on a CUDA (sm_100a) device, found {device}; '
+                f'kfac_b200 needs the model on a CUDA (sm_90a) device, found {device}; '
                 'there is no CPU fallback')
         _cabi.load()
         self._device = device

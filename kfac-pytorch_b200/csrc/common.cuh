@@ -1,4 +1,4 @@
-// Shared helpers for the K-FAC B200 kernels.
+// Shared helpers for the K-FAC kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -88,7 +88,7 @@ struct GemmArgs {
 
 int launch_gemm(const GemmArgs& g, cudaStream_t stream);
 
-// tcgen05 engine (gemm_tc.cu); returns KFAC_ERR_UNSUPPORTED when the shape /
+// wgmma engine (gemm_tc.cu); returns KFAC_ERR_UNSUPPORTED when the shape /
 // alignment is outside what the tensor-core kernel handles.
 struct TcGemmArgs {
   const float* A; int64_t lda;     // M x K row-major (K-major operand), lda % 4 == 0
@@ -107,6 +107,12 @@ struct TcGemmArgs {
   float* peerD[7]; int npeer;      // fused broadcast: the epilogue also stores the tile into these peer copies of D
 };
 bool tc_gemm_supported(const TcGemmArgs& a);
+// the split count launch_tc_gemm runs for a request of `splits` over kb_total k-blocks (every split non-empty)
+inline int tc_normalize_splits(int splits, int kb_total) {
+  splits = splits < 1 ? 1 : (splits > kb_total ? kb_total : splits);
+  const int per = (kb_total + splits - 1) / splits;
+  return (kb_total + per - 1) / per;
+}
 int launch_tc_gemm(const TcGemmArgs& a, cudaStream_t stream);
 int tc_num_sms();
 

@@ -1,6 +1,6 @@
 // Direct symmetric eigensolver for the large K-FAC factors (replaces torch.linalg.eigh of
 // kfac/layers/eigen.py:310,331 for n > 128):  F = H T H^T (sytrd.cu), T = Z L Z^T (stedc.cu),
-// Q = H Z by compact-WY block reflectors of 128 Householder vectors (this file; tcgen05 GEMMs).
+// Q = H Z by compact-WY block reflectors of 128 Householder vectors (this file; wgmma GEMMs).
 // Host side: workspace layout, the CTA-group schedule of the tridiagonalisation kernel, and the
 // enqueue of all stages on ONE stream without host synchronisation.
 #include "eigh_direct.cuh"
@@ -192,12 +192,13 @@ void make_layout(const int* n, int count, Layout& L) {
 }
 
 // ---- CTA-group schedule of the tridiagonalisation kernel --------------------------------------
-// Time model of one matrix on a group of C CTAs, fitted (least squares on the relative error, worst 6 %) to the sweep
-// tests/sytrd_sweep.py over n = 256 .. 4608, C = 1 .. 148 on a B200 (profiles/r02_sytrd_sweep.md): per column
+// Time model of one matrix on a group of C CTAs, fitted (least squares on the relative error, worst 6.6 %, mean 1.9 %)
+// to the sweep tests/sytrd_sweep.py over n = 256 .. 4608, C = 1 .. 132 on an H100 SXM 80 GB at a 400 W power limit
+// (points below the smallest group a matrix can use left out): per column
 //   T0 + T1 n            barriers, dependent cross-CTA loads, the serial vector phases
 //   (B n^2 + GA n) / C   tile products of the trailing matrix (averaged over its shrinking size) + row work
 //   DE log2 C            barrier and cross-CTA reduction cost growing with the group
-constexpr double T0 = 7.78e-6, T1 = 4.7e-11, BETA = 1.144e-11, GAMMA = 2.06e-8, DELTA = 2.03e-7, EPS = -2.62e-6;
+constexpr double T0 = 6.92e-6, T1 = 2.82e-10, BETA = 1.24e-11, GAMMA = 1.6e-8, DELTA = 2.72e-7, EPS = -1.23e-6;
 double job_time(int n, int C) {
   return (double)n * (T0 + T1 * n + (BETA * (double)n * n + GAMMA * n + EPS) / C + DELTA * std::log2((double)C));
 }

@@ -2,8 +2,8 @@
 //   1. sytrd.cu   Householder tridiagonalisation  F = H T H^T   (persistent multi-CTA kernel, fp32 SIMT,
 //                 lower-triangle 64x64 tiles resident in L2, two group barriers per column)
 //   2. stedc.cu   divide and conquer on T (Cuppen / Gu-Eisenstat): leaf solves in shared memory,
-//                 rank-one merges = deflation + secular equation + one tcgen05 GEMM per merge
-//   3. eigh_direct.cu  back-transformation Q = H Z with compact-WY block reflectors (tcgen05 GEMMs)
+//                 rank-one merges = deflation + secular equation + one wgmma GEMM per merge
+//   3. eigh_direct.cu  back-transformation Q = H Z with compact-WY block reflectors (wgmma GEMMs)
 // Replaces torch.linalg.eigh of kfac/layers/eigen.py:310,331 (LAPACK ssyevd = the same three stages).
 #pragma once
 #include "common.cuh"
@@ -63,7 +63,7 @@ size_t stedc_plan_bytes(const int* n, int count);   // includes the grouped-GEMM
 int launch_stedc(DcMat* h_mats, DcMat* d_mats, int count, void* plan_ws, size_t plan_bytes, int* status, cudaStream_t s,
                  bool q_zeroed = false);
 
-// plain fp32 TN GEMM on the tcgen05 engine: D = alpha * A B^T (+ D when accumulate)
+// plain fp32 TN GEMM on the wgmma engine: D = alpha * A B^T (+ D when accumulate)
 int gemm_tn_plain(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M, int N,
                   int K, cudaStream_t s);
 // a few side streams for independent small launches (per-merge / per-matrix GEMM chains)

@@ -6,6 +6,8 @@
 // are read in their native NCHW / (rows, features) layout.
 #include "common.cuh"
 
+#include <algorithm>
+
 namespace kfac {
 
 constexpr int CT = 64;   // covariance output tile
@@ -19,13 +21,15 @@ struct CovArgs {
   int batch;
   int feat;            // real features (without the ones column)
   int ones;            // append a constant-one feature
-  int splits;          // row splits per batch entry
+  int splits;          // splits of the sample range (all batch entries, flattened)
   float scale;
   float* acc;          // d x d, d = feat + ones
+  float* slab;         // splits x d x d partials (upper tiles), required when splits > 1
 };
 
-// acc += scale * X^T X over upper-triangular 64x64 tiles (mirrored), reduction
-// over samples split across CTAs with atomics.
+// acc += scale * X^T X over upper-triangular 64x64 tiles (mirrored).  The reduction over the samples of all batch
+// entries is split across CTAs; split sp stores its partial tile into slab sp and cov_reduce_kernel adds the slabs
+// in a fixed order (every run gives the same bits).  With one split the CTA is the only writer of its tile.
 template <typename T, bool FEATURE_MAJOR>
 __global__ void __launch_bounds__(256) cov_kernel(CovArgs a) {
   __shared__ __align__(16) float As[CK][CT + 4];
@@ -36,11 +40,12 @@ __global__ void __launch_bounds__(256) cov_kernel(CovArgs a) {
   int t = blockIdx.x, tm = 0;
   while (t >= nt - tm) { t -= nt - tm; ++tm; }
   const int tn = tm + t;
-  const int b = blockIdx.y / a.splits, sp = blockIdx.y % a.splits;
-  int chunk = (a.rows + a.splits - 1) / a.splits;
+  const int sp = blockIdx.y;
+  const int64_t total = (int64_t)a.rows * a.batch;
+  int64_t chunk = (total + a.splits - 1) / a.splits;
   chunk = (chunk + CK - 1) / CK * CK;
-  const int r_begin = sp * chunk, r_end = min(a.rows, r_begin + chunk);
-  const T* __restrict__ x = reinterpret_cast<const T*>(a.x) + (int64_t)b * a.batch_stride;
+  const int64_t r_begin = sp * chunk, r_end = min(total, r_begin + chunk);
+  const T* __restrict__ xb = reinterpret_cast<const T*>(a.x);
   const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
   const int m0 = tm * CT, n0 = tn * CT;
   float acc[4][4];
@@ -49,7 +54,7 @@ __global__ void __launch_bounds__(256) cov_kernel(CovArgs a) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
 
-  for (int r0 = r_begin; r0 < r_end; r0 += CK) {
+  for (int64_t r0 = r_begin; r0 < r_end; r0 += CK) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       int f, r;
@@ -59,14 +64,19 @@ __global__ void __launch_bounds__(256) cov_kernel(CovArgs a) {
       float va = 0.f, vb = 0.f;
       const int fa = m0 + f, fb = n0 + f;
       if (rv) {
+        // flattened sample index -> (batch entry, row)
+        const int64_t q = r0 + r;
+        const int b = a.batch > 1 ? (int)(q / a.rows) : 0;
+        const int64_t rr = q - (int64_t)b * a.rows;
+        const T* __restrict__ x = xb + (int64_t)b * a.batch_stride;
         if (fa < a.feat)
-          va = to_float<T>(FEATURE_MAJOR ? x[(int64_t)fa * a.ld + (r0 + r)]
-                                         : x[(int64_t)(r0 + r) * a.ld + fa]);
+          va = to_float<T>(FEATURE_MAJOR ? x[(int64_t)fa * a.ld + rr]
+                                         : x[rr * a.ld + fa]);
         else if (fa < d) va = 1.f;
         if (tn != tm) {
           if (fb < a.feat)
-            vb = to_float<T>(FEATURE_MAJOR ? x[(int64_t)fb * a.ld + (r0 + r)]
-                                           : x[(int64_t)(r0 + r) * a.ld + fb]);
+            vb = to_float<T>(FEATURE_MAJOR ? x[(int64_t)fb * a.ld + rr]
+                                           : x[rr * a.ld + fb]);
           else if (fb < d) vb = 1.f;
         }
       }
@@ -97,39 +107,88 @@ __global__ void __launch_bounds__(256) cov_kernel(CovArgs a) {
       const int n = n0 + tx * 4 + j;
       if (n >= d) continue;
       const float v = a.scale * acc[i][j];
-      atomicAdd(&a.acc[(int64_t)m * d + n], v);
-      if (tn != tm) atomicAdd(&a.acc[(int64_t)n * d + m], v);
+      if (a.splits > 1) {
+        a.slab[(int64_t)sp * d * d + (int64_t)m * d + n] = v;
+      } else {
+        a.acc[(int64_t)m * d + n] += v;
+        if (tn != tm) a.acc[(int64_t)n * d + m] += v;
+      }
     }
   }
 }
 
+// acc[i][j] += sum_sp slab[sp][min(i,j)][max(i,j)], splits added in a fixed order
+__global__ void cov_reduce_kernel(const float* __restrict__ slab, int splits, int d, float* acc) {
+  const int64_t dd = (int64_t)d * d;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < dd; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int i = (int)(idx / d), j = (int)(idx - (int64_t)i * d);
+    const int64_t src = i <= j ? idx : (int64_t)j * d + i;
+    float t = slab[src];
+    for (int sp = 1; sp < splits; ++sp) t += slab[sp * dd + src];
+    acc[idx] += t;
+  }
+}
+
+// split plans of the two covariance paths (shared by the launches and the workspace sizes)
+static int cov_tc_splits(int d, int64_t rows, int batch) {
+  const int nt = ceil_div(d, 128), ntiles = nt * (nt + 1) / 2;
+  const int kb_total = ceil_div(rows, 32) * batch;
+  const int num_sms = tc_num_sms();
+  int splits = 1;
+  if (ntiles < num_sms) splits = std::max(1, std::min(num_sms / ntiles, kb_total / 8));
+  return tc_normalize_splits(splits, kb_total);
+}
+static int cov_simt_splits(int d, int64_t rows, int batch) {
+  const int nt = ceil_div(d, CT), tiles = nt * (nt + 1) / 2;
+  const int64_t total = rows * batch;
+  int splits = ceil_div((int64_t)tc_num_sms() * 3, tiles);
+  return (int)std::max<int64_t>(1, std::min<int64_t>(splits, ceil_div(total, 4 * CK)));
+}
+// bytes of the split partials: the larger of the two paths (the tensor-core path also depends on alignment)
+static size_t cov_slab_bytes(int d, int64_t rows, int batch) {
+  const int s = std::max(cov_tc_splits(d, rows, batch), cov_simt_splits(d, rows, batch));
+  return s > 1 ? (size_t)s * d * d * sizeof(float) : 0;
+}
+
+static int cov_reduce(const CovArgs& a, int d, int splits, cudaStream_t s) {
+  const int blocks = (int)std::min<int64_t>(ceil_div((int64_t)d * d, 256), (int64_t)tc_num_sms() * 16);
+  cov_reduce_kernel<<<blocks, 256, 0, s>>>(a.slab, splits, d, a.acc);
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
+// a.slab (cov_slab_bytes) lets long reductions be split over the SMs; without it they run as one split
 template <bool FEATURE_MAJOR>
 static int launch_cov(CovArgs a, int dtype, cudaStream_t s) {
   const int d = a.feat + a.ones;
   if (d <= 0 || a.rows <= 0 || a.batch <= 0) return KFAC_OK;
   if (FEATURE_MAJOR && dtype == KFAC_F32 && a.ones == 0 && d >= 64 && (int64_t)a.rows * a.batch >= 256) {
-    // tcgen05 SYRK: X (features x samples) is a K-major operand as it lies in HBM;
-    // upper-triangular tiles only, split over the samples, partial tiles added with atomics.
+    // tensor-core SYRK: X (features x samples) is a K-major operand as it lies in HBM;
+    // upper-triangular tiles only, split over the samples into per-split partials.
     TcGemmArgs t{};
     t.A = (const float*)a.x; t.lda = a.ld; t.B = t.A; t.ldb = a.ld;
     t.D = a.acc; t.ldd = d; t.M = d; t.N = d; t.K = a.rows;
     t.kbatch = a.batch; t.a_kb_stride = a.batch_stride; t.b_kb_stride = a.batch_stride;
-    t.upper_only = 1; t.atomic = 1; t.splits = 0; t.alpha = a.scale;
-    if (tc_gemm_supported(t)) return launch_tc_gemm(t, s);
+    t.upper_only = 1; t.alpha = a.scale;
+    if (tc_gemm_supported(t)) {
+      const int splits = a.slab ? cov_tc_splits(d, a.rows, a.batch) : 1;
+      if (splits > 1) { t.slab = a.slab; t.slab_stride = (int64_t)d * d; t.splits = splits; }
+      else { t.accumulate = 1; t.splits = 1; }
+      const int rc = launch_tc_gemm(t, s);
+      if (rc || splits == 1) return rc;
+      return cov_reduce(a, d, splits, s);
+    }
   }
   const int nt = ceil_div(d, CT);
   const int tiles = nt * (nt + 1) / 2;
-  int splits = ceil_div(148 * 3, (int64_t)tiles * a.batch);
-  splits = max(1, min(splits, ceil_div(a.rows, 4 * CK)));
-  a.splits = splits;
-  dim3 grid(tiles, a.batch * splits);
-  if (grid.y > 65535) { set_error("cov: too many batch*splits"); return KFAC_ERR_BAD_ARG; }
+  a.splits = a.slab ? cov_simt_splits(d, a.rows, a.batch) : 1;
+  dim3 grid(tiles, a.splits);
   if (dtype == KFAC_F32) cov_kernel<float, FEATURE_MAJOR><<<grid, 256, 0, s>>>(a);
   else if (dtype == KFAC_F16) cov_kernel<__half, FEATURE_MAJOR><<<grid, 256, 0, s>>>(a);
   else if (dtype == KFAC_BF16) cov_kernel<__nv_bfloat16, FEATURE_MAJOR><<<grid, 256, 0, s>>>(a);
   else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   KFAC_LAUNCH_CHECK();
-  return KFAC_OK;
+  return a.splits > 1 ? cov_reduce(a, d, a.splits, s) : KFAC_OK;
 }
 
 // im2col into a FEATURE-major fp32 matrix: out[(c,i,j)][(n,ho,wo)]
@@ -288,17 +347,35 @@ __global__ void scale_kernel(float* buf, int64_t count, float s) {
 
 static inline int grid_for(int64_t total, int threads = 256) {
   int64_t b = (total + threads - 1) / threads;
-  return (int)max((int64_t)1, min(b, (int64_t)148 * 16));
+  return (int)max((int64_t)1, min(b, (int64_t)tc_num_sms() * 16));
 }
+
+// Workspace of a factor call: [packed feature-major matrix (pack bytes, may be 0)] [split partials of the SYRK].
+// Without the partials region the reduction runs as one split (deterministic as well, less parallel).
+struct CovWs {
+  size_t pack, slab_off, total;
+  CovWs(size_t pack_bytes, int d, int64_t rows, int batch) : pack(pack_bytes) {
+    slab_off = pack ? align_up(pack, 256) : 0;
+    const size_t slab = cov_slab_bytes(d, rows, batch);
+    total = slab ? slab_off + slab : pack;
+  }
+  float* slab(void* ws, size_t ws_bytes) const {
+    return (ws && total > slab_off && ws_bytes >= total) ? (float*)((char*)ws + slab_off) : nullptr;
+  }
+};
 
 }  // namespace kfac
 
 using namespace kfac;
 
-extern "C" size_t kfac_factor_linear_workspace_bytes(int64_t rows, int features, int append_ones) {
+static size_t linear_pack_bytes(int64_t rows, int features, int append_ones) {
   if (rows < 512 || features < 128) return 0;   // small problems stay on the SIMT kernel
   const int64_t ld = (rows + 3) / 4 * 4;
   return (size_t)ld * (size_t)(features + (append_ones ? 1 : 0)) * sizeof(float);
+}
+
+extern "C" size_t kfac_factor_linear_workspace_bytes(int64_t rows, int features, int append_ones) {
+  return CovWs(linear_pack_bytes(rows, features, append_ones), features + (append_ones ? 1 : 0), rows, 1).total;
 }
 
 extern "C" int kfac_factor_linear(const void* x, int dtype, int64_t rows, int features,
@@ -306,10 +383,10 @@ extern "C" int kfac_factor_linear(const void* x, int dtype, int64_t rows, int fe
                                   void* stream) {
   KFAC_CHECK_ARG(x && acc, "null pointer");
   KFAC_CHECK_ARG(rows >= 0 && rows < (1ll << 31) && features > 0, "dims");
-  const size_t need = kfac_factor_linear_workspace_bytes(rows, features, append_ones);
-  if (need > 0 && ws && ws_bytes >= need) {
+  const CovWs w(linear_pack_bytes(rows, features, append_ones), features + (append_ones ? 1 : 0), rows, 1);
+  if (w.pack > 0 && ws && ws_bytes >= w.pack) {
     // tall activations (tokens x hidden): transpose once into a feature-major matrix
-    // (ones row materialised) and run the tcgen05 SYRK on it
+    // (ones row materialised) and run the tensor-core SYRK on it
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t ld = (rows + 3) / 4 * 4;
     const int ones = append_ones ? 1 : 0;
@@ -321,24 +398,37 @@ extern "C" int kfac_factor_linear(const void* x, int dtype, int64_t rows, int fe
     KFAC_LAUNCH_CHECK();
     CovArgs a{};
     a.x = ws; a.ld = ld; a.batch_stride = 0; a.rows = (int)rows; a.batch = 1;
-    a.feat = features + ones; a.ones = 0; a.scale = scale; a.acc = acc;
+    a.feat = features + ones; a.ones = 0; a.scale = scale; a.acc = acc; a.slab = w.slab(ws, ws_bytes);
     return launch_cov<true>(a, KFAC_F32, st);
   }
   CovArgs a{};
   a.x = x; a.ld = features; a.batch_stride = 0; a.rows = (int)rows; a.batch = 1;
-  a.feat = features; a.ones = append_ones ? 1 : 0; a.scale = scale; a.acc = acc;
+  a.feat = features; a.ones = append_ones ? 1 : 0; a.scale = scale; a.acc = acc; a.slab = w.slab(ws, ws_bytes);
   return launch_cov<false>(a, dtype, (cudaStream_t)stream);
+}
+
+static bool conv_in_place(int C, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw) {
+  // 1x1 / stride 1 reads the NCHW input in place -- unless its rows (H*W floats) are not 16-byte multiples
+  // (7 x 7 maps): TMA cannot address those, so they are packed like an im2col matrix
+  return kh == 1 && kw == 1 && sh == 1 && sw == 1 && ph == 0 && pw == 0 && (((int64_t)H * W) % 4 == 0 || C < 64);
+}
+
+static CovWs conv_input_ws(int batch, int C, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw,
+                           int append_ones) {
+  const int ones = append_ones ? 1 : 0;
+  if (conv_in_place(C, H, W, kh, kw, sh, sw, ph, pw)) return CovWs(0, C + ones, (int64_t)H * W, batch);
+  const int64_t Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
+  const int64_t rows = (int64_t)batch * Ho * Wo, ld = (rows + 3) / 4 * 4;
+  const int d = C * kh * kw + ones;
+  return CovWs((size_t)ld * d * sizeof(float), d, rows, 1);
 }
 
 extern "C" size_t kfac_factor_conv2d_input_workspace_bytes(int batch, int C, int H, int W, int kh,
                                                            int kw, int sh, int sw, int ph, int pw,
                                                            int append_ones) {
-  // 1x1 / stride 1 reads the NCHW input in place -- unless its rows (H*W floats) are not 16-byte multiples
-  // (7 x 7 maps): TMA cannot address those, so they are packed like an im2col matrix
-  if (kh == 1 && kw == 1 && sh == 1 && sw == 1 && ph == 0 && pw == 0 && (((int64_t)H * W) % 4 == 0 || C < 64)) return 0;
-  const int64_t Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
-  const int64_t ld = ((int64_t)batch * Ho * Wo + 3) / 4 * 4;
-  return (size_t)ld * ((size_t)C * kh * kw + (append_ones ? 1 : 0)) * sizeof(float);
+  if (batch <= 0 || C <= 0 || H <= 0 || W <= 0 || kh <= 0 || kw <= 0 || sh <= 0 || sw <= 0 || ph < 0 || pw < 0) return 0;
+  if ((H + 2 * ph - kh) / sh + 1 <= 0 || (W + 2 * pw - kw) / sw + 1 <= 0) return 0;
+  return conv_input_ws(batch, C, H, W, kh, kw, sh, sw, ph, pw, append_ones).total;
 }
 
 extern "C" int kfac_factor_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W,
@@ -351,17 +441,17 @@ extern "C" int kfac_factor_conv2d_input(const void* x, int dtype, int batch, int
   cudaStream_t s = (cudaStream_t)stream;
   const int Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
   KFAC_CHECK_ARG(Ho > 0 && Wo > 0, "empty output");
+  const CovWs w = conv_input_ws(batch, C, H, W, kh, kw, sh, sw, ph, pw, append_ones);
   CovArgs a{};
-  a.ones = append_ones ? 1 : 0; a.scale = scale; a.acc = acc;
-  if (kh == 1 && kw == 1 && sh == 1 && sw == 1 && ph == 0 && pw == 0 && (((int64_t)H * W) % 4 == 0 || C < 64)) {
+  a.ones = append_ones ? 1 : 0; a.scale = scale; a.acc = acc; a.slab = w.slab(ws, ws_bytes);
+  if (conv_in_place(C, H, W, kh, kw, sh, sw, ph, pw)) {
     // 1x1 / stride 1: the NCHW input already is a feature-major (C x HW) matrix per image
     a.x = x; a.ld = (int64_t)H * W; a.batch_stride = (int64_t)C * H * W;
     a.rows = H * W; a.batch = batch; a.feat = C;
     return launch_cov<true>(a, dtype, s);
   }
-  const size_t need = kfac_factor_conv2d_input_workspace_bytes(batch, C, H, W, kh, kw, sh, sw, ph, pw, append_ones);
-  if (!ws || ws_bytes < need) {
-    set_error("conv2d_input: workspace too small (%zu < %zu)", ws_bytes, need);
+  if (!ws || ws_bytes < w.pack) {
+    set_error("conv2d_input: workspace too small (%zu < %zu)", ws_bytes, w.pack);
     return KFAC_ERR_WORKSPACE;
   }
   const int64_t rows = (int64_t)batch * Ho * Wo;
@@ -381,20 +471,25 @@ extern "C" int kfac_factor_conv2d_input(const void* x, int dtype, int batch, int
   return launch_cov<true>(a, KFAC_F32, s);
 }
 
-extern "C" size_t kfac_factor_conv2d_gradout_workspace_bytes(int batch, int C, int Ho, int Wo) {
+static CovWs gradout_ws(int batch, int C, int Ho, int Wo) {
   // maps whose rows (Ho*Wo floats) are not 16-byte multiples (7 x 7) are packed into an aligned feature-major
-  // matrix for the tcgen05 SYRK; everything else is read in place
-  if (((int64_t)Ho * Wo) % 4 == 0 || C < 64) return 0;
-  const int64_t ld = ((int64_t)batch * Ho * Wo + 3) / 4 * 4;
-  return (size_t)ld * (size_t)C * sizeof(float);
+  // matrix for the tensor-core SYRK; everything else is read in place
+  if (((int64_t)Ho * Wo) % 4 == 0 || C < 64) return CovWs(0, C, (int64_t)Ho * Wo, batch);
+  const int64_t rows = (int64_t)batch * Ho * Wo, ld = (rows + 3) / 4 * 4;
+  return CovWs((size_t)ld * (size_t)C * sizeof(float), C, rows, 1);
+}
+
+extern "C" size_t kfac_factor_conv2d_gradout_workspace_bytes(int batch, int C, int Ho, int Wo) {
+  if (batch <= 0 || C <= 0 || Ho <= 0 || Wo <= 0) return 0;
+  return gradout_ws(batch, C, Ho, Wo).total;
 }
 
 extern "C" int kfac_factor_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo,
                                           float scale, float* acc, void* ws, size_t ws_bytes, void* stream) {
   KFAC_CHECK_ARG(g && acc, "null pointer");
   KFAC_CHECK_ARG(batch > 0 && C > 0 && Ho > 0 && Wo > 0, "geometry");
-  const size_t need = kfac_factor_conv2d_gradout_workspace_bytes(batch, C, Ho, Wo);
-  if (need > 0 && ws && ws_bytes >= need) {
+  const CovWs w = gradout_ws(batch, C, Ho, Wo);
+  if (w.pack > 0 && ws && ws_bytes >= w.pack) {
     cudaStream_t s = (cudaStream_t)stream;
     const int64_t rows = (int64_t)batch * Ho * Wo;
     KFAC_CHECK_ARG(rows < (1ll << 31), "rows overflow");
@@ -409,12 +504,12 @@ extern "C" int kfac_factor_conv2d_gradout(const void* g, int dtype, int batch, i
     KFAC_LAUNCH_CHECK();
     CovArgs a{};
     a.x = ws; a.ld = ld; a.batch_stride = 0; a.rows = (int)rows; a.batch = 1; a.feat = C; a.ones = 0;
-    a.scale = scale; a.acc = acc;
+    a.scale = scale; a.acc = acc; a.slab = w.slab(ws, ws_bytes);
     return launch_cov<true>(a, KFAC_F32, s);
   }
   CovArgs a{};
   a.x = g; a.ld = (int64_t)Ho * Wo; a.batch_stride = (int64_t)C * Ho * Wo;
-  a.rows = Ho * Wo; a.batch = batch; a.feat = C; a.ones = 0; a.scale = scale; a.acc = acc;
+  a.rows = Ho * Wo; a.batch = batch; a.feat = C; a.ones = 0; a.scale = scale; a.acc = acc; a.slab = w.slab(ws, ws_bytes);
   return launch_cov<true>(a, dtype, (cudaStream_t)stream);
 }
 

@@ -1,4 +1,4 @@
-// Grouped tcgen05 GEMM: ONE launch runs a whole list of independent problems
+// Grouped wgmma GEMM: ONE launch runs a whole list of independent problems
 //     D_i = epilogue_i(alpha_i * A_i B_i^T)        (A_i: M x K, B_i: N x K, row-major fp32, 3xTF32 split)
 // through the persistent pipeline of tc_pipeline.cuh.  Work items are (problem, 128 x 128 tile, K split);
 // the per-problem TMA descriptors live in a device table (the kernel walks it by binary search), so the
@@ -38,10 +38,7 @@ struct GroupedParams { const GProb* probs; int nprobs; };
 struct GroupedPolicy {
   using Params = GroupedParams;
   struct Item { const GProb* pr; int m0, n0, kb0, kb1, sp, idx; };
-  static constexpr int BN = GBN;
-  static constexpr bool B_IS_A = false;
   static constexpr uint32_t TX_BYTES = 2 * tc::PTILE;
-  static constexpr bool MN_MAJOR = false;
   static constexpr int CHUNK = 1;
   __device__ static void reset(Item& it) { it.idx = 0; it.pr = nullptr; }
   __device__ static int total_work(const Params&, int t) { return t; }
@@ -70,13 +67,13 @@ struct GroupedPolicy {
     tc::tma_load_3d(a, &it.pr->tmA, bar, kc, it.m0, 0);
     tc::tma_load_3d(b, &it.pr->tmB, bar, kc, it.n0, 0);
   }
-  __device__ static void store(const Params&, const Item& it, int row, int col0, float (&v)[32]) {
+  __device__ static void store(const Params&, const Item& it, int row, int col, float (&v)[2]) {
     const GProb& p = *it.pr;
-    const int m = it.m0 + row, nb = it.n0 + col0;
+    const int m = it.m0 + row, nb = it.n0 + col;
     if (m >= p.M || nb >= p.N) return;
     float* drow = p.D + (int64_t)it.sp * p.slab_stride + (int64_t)m * p.ldd + nb;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
+    for (int j = 0; j < 2; ++j) {
       float x = p.alpha * v[j];
       if (nb + j < p.N) {
         if (p.epi == EPI_MUL) x *= p.E[(int64_t)m * p.lde + nb + j];
@@ -86,31 +83,22 @@ struct GroupedPolicy {
     }
     if (p.mode == 2) {
 #pragma unroll
-      for (int j = 0; j < 32; ++j)
+      for (int j = 0; j < 2; ++j)
         if (nb + j < p.N) atomicAdd(drow + j, v[j]);
       return;
     }
-    if ((p.ldd & 3) == 0 && nb + 32 <= p.N) {
+    if (((uintptr_t)drow & 7) == 0 && (p.ldd & 1) == 0 && nb + 2 <= p.N) {
       if (p.mode == 1) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const float4 o = *reinterpret_cast<const float4*>(drow + j);
-          v[j] += o.x; v[j + 1] += o.y; v[j + 2] += o.z; v[j + 3] += o.w;
-        }
+        const float2 o = *reinterpret_cast<const float2*>(drow);
+        v[0] += o.x; v[1] += o.y;
       }
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<float4*>(drow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+      *reinterpret_cast<float2*>(drow) = make_float2(v[0], v[1]);
       // fused compute + broadcast: the same tile goes straight to the peers' copies of D (P2P over NVLink)
-      for (int q = 0; q < p.npeer; ++q) {
-        float* prow = p.peerD[q] + (int64_t)m * p.ldd + nb;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(prow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-      }
+      for (int q = 0; q < p.npeer; ++q)
+        *reinterpret_cast<float2*>(p.peerD[q] + (int64_t)m * p.ldd + nb) = make_float2(v[0], v[1]);
     } else {
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
+      for (int j = 0; j < 2; ++j) {
         if (nb + j >= p.N) continue;
         drow[j] = (p.mode == 1) ? drow[j] + v[j] : v[j];
         for (int q = 0; q < p.npeer; ++q) p.peerD[q][(int64_t)m * p.ldd + nb + j] = v[j];

@@ -1,4 +1,4 @@
-// Grouped tcgen05 GEMM (gemm_grouped.cu): one launch for a list of independent D_i = epi_i(alpha_i A_i B_i^T).
+// Grouped wgmma GEMM (gemm_grouped.cu): one launch for a list of independent D_i = epi_i(alpha_i A_i B_i^T).
 #pragma once
 #include "common.cuh"
 

@@ -1,6 +1,6 @@
 // fp32 SIMT GEMM engine: the size-class for small / oddly shaped operands
 // (factor dims < 128, ragged tails, strided transposes).  Large aligned tiles
-// go to the tcgen05 engine in gemm_tc.cu.
+// go to the wgmma engine in gemm_tc.cu.
 #include "common.cuh"
 
 namespace kfac {

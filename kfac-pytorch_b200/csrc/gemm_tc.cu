@@ -1,15 +1,14 @@
-// tcgen05 GEMM engine: D = epilogue(alpha * A B^T), A (M x K) and B (N x K)
+// wgmma GEMM engine: D = epilogue(alpha * A B^T), A (M x K) and B (N x K)
 // row-major fp32 ("TN", both operands K-major), fp32-equivalent accuracy from a
-// 3xTF32 split:  a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi  with fp32 TMEM
+// 3xTF32 split:  a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi  with fp32 register
 // accumulation (single-pass TF32 fails the 1e-3 parity bar, SURVEY.md 7.3 H1).
 //
-// One persistent CTA per SM, warp-specialised:
+// One persistent CTA per SM, warp-specialised (tc_pipeline.cuh):
 //   warp 0      TMA producer   (cp.async.bulk.tensor 3-D tiles, SWIZZLE_128B)
-//   warp 1      MMA issuer     (one lane: 12 x tcgen05.mma 128x128x8 per k-block)
-//   warps 2-5   splitter       (smem -> smem: lo = x - trunc_tf32(x))
-//   warps 6-9   epilogue       (tcgen05.ld TMEM -> regs -> fused epilogue -> HBM)
-// 3 smem stages x {A_hi, B_hi, A_lo, B_lo} x 16 KB = 192 KB; 2 TMEM accumulators
-// (2 x 128 columns) so the epilogue of tile i overlaps the MMAs of tile i+1.
+//   warps 1-3   splitter       (smem -> smem: lo = x - trunc_tf32(x))
+//   warps 4-11  two consumer warpgroups (12 x wgmma m64n128k8 per k-block each, then the
+//               fused epilogue from the accumulator registers -> HBM)
+// 3 smem stages x {A_hi, B_hi, A_lo, B_lo} x 16 KB = 192 KB.
 #include "common.cuh"
 #include "tc_pipeline.cuh"
 
@@ -31,10 +30,7 @@ struct TcParams {
 struct GemmPolicy {
   using Params = TcParams;
   struct Item { int m0, n0, kb0, kb1, diag, sp; };
-  static constexpr int BN = TBN;
-  static constexpr bool B_IS_A = false;
   static constexpr uint32_t TX_BYTES = 2 * tc::PTILE;
-  static constexpr bool MN_MAJOR = false;
   static constexpr int CHUNK = 1;
   __device__ static void reset(Item&) {}
   __device__ static int total_work(const Params&, int t) { return t; }
@@ -61,13 +57,13 @@ struct GemmPolicy {
     tc::tma_load_3d(a, &p.tmA, bar, kc, it.m0, bt);
     tc::tma_load_3d(b, &p.tmB, bar, kc, it.n0, bt);
   }
-  __device__ static void store(const Params& p, const Item& it, int row, int col0, float (&v)[32]) {
-    const int m = it.m0 + row, nb = it.n0 + col0;
+  __device__ static void store(const Params& p, const Item& it, int row, int col, float (&v)[2]) {
+    const int m = it.m0 + row, nb = it.n0 + col;
     if (m >= p.M || nb >= p.N) return;
-    const bool mirror = p.upper_only && !it.diag;
+    const bool mirror = p.upper_only && !it.diag && p.slab_stride == 0;   // split partials hold the upper tiles only
     float* drow = p.D + (int64_t)it.sp * p.slab_stride + (int64_t)m * p.ldd + nb;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
+    for (int j = 0; j < 2; ++j) {
       float x = p.alpha * v[j];
       if (nb + j < p.N) {
         if (p.epi == EPI_MUL) x *= p.E[(int64_t)m * p.lde + nb + j];
@@ -75,35 +71,29 @@ struct GemmPolicy {
       }
       v[j] = x;
     }
-    if (!p.atomic && !mirror && (p.ldd & 3) == 0 && nb + 32 <= p.N) {
+    if (!p.atomic && !mirror && ((uintptr_t)drow & 7) == 0 && (p.ldd & 1) == 0 && nb + 2 <= p.N) {
       if (p.accum) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const float4 o = *reinterpret_cast<const float4*>(drow + j);
-          v[j] += o.x; v[j + 1] += o.y; v[j + 2] += o.z; v[j + 3] += o.w;
-        }
+        const float2 o = *reinterpret_cast<const float2*>(drow);
+        v[0] += o.x; v[1] += o.y;
       }
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<float4*>(drow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+      *reinterpret_cast<float2*>(drow) = make_float2(v[0], v[1]);
       // fused compute + broadcast: the same tile goes straight to the peers' copies of D
       // (P2P stores over NVLink, overlapped with the MMAs of the next tile)
-      for (int q = 0; q < p.npeer; ++q) {
-        float* prow = p.peerD[q] + (int64_t)m * p.ldd + nb;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(prow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-      }
+      for (int q = 0; q < p.npeer; ++q)
+        *reinterpret_cast<float2*>(p.peerD[q] + (int64_t)m * p.ldd + nb) = make_float2(v[0], v[1]);
     } else {
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
+      for (int j = 0; j < 2; ++j) {
         if (nb + j >= p.N) continue;
         if (p.atomic) {
           atomicAdd(drow + j, v[j]);
           if (mirror) atomicAdd(p.D + (int64_t)(nb + j) * p.ldd + m, v[j]);
         } else {
           drow[j] = p.accum ? drow[j] + v[j] : v[j];
-          if (mirror) p.D[(int64_t)(nb + j) * p.ldd + m] = v[j];
+          if (mirror) {
+            float* t = p.D + (int64_t)(nb + j) * p.ldd + m;
+            *t = p.accum ? *t + v[j] : v[j];
+          }
           for (int q = 0; q < p.npeer; ++q) p.peerD[q][(int64_t)m * p.ldd + nb + j] = v[j];
         }
       }
@@ -165,7 +155,7 @@ int tc_num_sms() {
   if (!n) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-      n = 148;
+      n = 132;
   }
   return n;
 }
@@ -199,7 +189,7 @@ int launch_tc_gemm(const TcGemmArgs& a, cudaStream_t stream) {
   p.D = a.D; p.ldd = a.ldd; p.M = a.M; p.N = a.N; p.K = a.K; p.kbatch = kbatch;
   p.tiles_m = ceil_div(a.M, TBM); p.tiles_n = ceil_div(a.N, TBN);
   p.upper_only = a.upper_only; p.atomic = a.atomic; p.alpha = a.alpha; p.accum = a.accumulate;
-  if (a.accumulate && (a.atomic || a.upper_only || a.npeer > 0 || a.splits > 1)) { set_error("tc_gemm: accumulate needs the plain single-split epilogue"); return KFAC_ERR_BAD_ARG; }
+  if (a.accumulate && (a.atomic || a.npeer > 0 || a.splits > 1)) { set_error("tc_gemm: accumulate needs the plain single-split epilogue"); return KFAC_ERR_BAD_ARG; }
   p.epi = a.epi; p.E = a.E; p.lde = a.lde; p.dg = a.dg; p.da = a.da; p.damping = a.damping;
   p.npeer = a.npeer;
   for (int q = 0; q < a.npeer && q < 7; ++q) p.peerD[q] = a.peerD[q];
@@ -211,12 +201,9 @@ int launch_tc_gemm(const TcGemmArgs& a, cudaStream_t stream) {
     splits = 1;
     if (a.atomic && ntiles < num_sms) splits = std::max(1, std::min(num_sms / ntiles, kb_total / 8));
   }
-  splits = std::max(1, std::min(splits, kb_total));
+  splits = tc_normalize_splits(splits, kb_total);
   if (splits > 1 && !a.atomic && !a.slab) { set_error("tc_gemm: split-K needs atomic accumulation or a slab workspace"); return KFAC_ERR_BAD_ARG; }
-  if (a.slab && (a.atomic || a.upper_only || a.npeer > 0 || a.epi != EPI_NONE || a.accumulate)) { set_error("tc_gemm: slab split-K needs the plain epilogue"); return KFAC_ERR_BAD_ARG; }
-  // make every split non-empty
-  const int per = ceil_div(kb_total, splits);
-  splits = ceil_div(kb_total, per);
+  if (a.slab && (a.atomic || a.npeer > 0 || a.epi != EPI_NONE || a.accumulate)) { set_error("tc_gemm: slab split-K needs the plain epilogue"); return KFAC_ERR_BAD_ARG; }
   p.splits = splits;
   if (a.slab) { p.D = a.slab; p.slab_stride = a.slab_stride; }
   const int total = ntiles * splits;

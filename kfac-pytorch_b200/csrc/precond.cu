@@ -132,7 +132,7 @@ __global__ void transpose_kernel(const float* src, int lds, float* dst, int ldd,
 
 static inline int grid_for(int64_t total) {
   int64_t b = (total + 255) / 256;
-  return (int)max((int64_t)1, min(b, (int64_t)148 * 8));
+  return (int)max((int64_t)1, min(b, (int64_t)tc_num_sms() * 8));
 }
 
 struct Epi { int kind = EPI_NONE; const float* E = nullptr; int64_t lde = 0;

@@ -10,7 +10,7 @@
 //       secular  (one warp per root: bracketing bisection on |mu| with geometric steps, pole-shifted origin)
 //       zhat     (one warp per entry: Loewner product)
 //       rank + build (final order; rows of U~^T: new eigenvectors in the basis of the old columns)
-//       GEMM     Q_new = Q_old U~ on the tcgen05 engine, ONE grouped launch per level.  Merges of more than
+//       GEMM     Q_new = Q_old U~ on the wgmma engine, ONE grouped launch per level.  Merges of more than
 //                DENSE_MAX rows use the structure LAPACK's slaed2/slaed3 use: only the k non-deflated columns of
 //                Q_old enter the product (packed as [upper-only | mixed | lower-only] into P), the upper and lower
 //                row halves are two problems over the column ranges they can see, and the deflated eigenvectors
@@ -600,8 +600,9 @@ int launch_stedc(DcMat* h_mats, DcMat* d_mats, int count, void* plan_ws, size_t 
     KFAC_LAUNCH_CHECK();
     dc_copy_d_kernel<<<dim3(ceil_div(mmax, 256), nm), 256, 0, s>>>(d_mats, d_levels[l]);
     KFAC_LAUNCH_CHECK();
-    // Q_new = Q_old U~ for every merge of the level: ONE grouped tcgen05 launch.  Long reductions are split into
-    // chains of <= 512 (the tensor-core accumulator truncates) and added atomically into the zeroed target block.
+    // Q_new = Q_old U~ for every merge of the level: ONE grouped wgmma launch.  Every output tile is computed by one
+    // CTA over the whole reduction (its k range is read on the device) and added once into the zeroed target block,
+    // so the result is the same in every run.
     std::vector<GroupedGemm> gg;
     for (auto& mg : lv) {
       const DcMat& mt = h_mats[mg.mat];
@@ -614,7 +615,7 @@ int launch_stedc(DcMat* h_mats, DcMat* d_mats, int count, void* plan_ws, size_t 
         // structured: packed non-deflated columns, upper and lower row halves over the k-block ranges written by the
         // deflation kernel (I_KR); deflated eigenvectors are copied afterwards
         KFAC_CUDA(cudaMemset2DAsync(mt.Q[mg.src ^ 1] + o, (size_t)mt.ld * 4, 0, (size_t)m * 4, (size_t)m, s));
-        g.splits = ceil_div(m, 512); g.mode = 2;
+        g.mode = 2;
         const int* kr = mt.iscr + (int64_t)I_KR * mt.n + mg.lo;
         g.A = mt.P + o; g.D = mt.Q[mg.src ^ 1] + o; g.M = n1; g.krange = kr;
         gg.push_back(g);

@@ -13,7 +13,7 @@
 //             effective column x' = A[:, s+1] - V W[s+1,:]^T - W V[s+1,:]^T and |x'|^2 partials -> barrier 2
 // After TRD_NB columns the lower tiles get the rank-2*NB update A -= V W^T + W V^T (fp32 SIMT: the
 // tensor core's 3xTF32 accumulate would cost the tridiagonal ~1e-5 of accuracy) -> one more barrier.
-// The matrix (<= 42 MB of lower tiles at n = 4608) stays resident in the 126 MB L2; algorithmic traffic
+// The matrix (<= 42 MB of lower tiles at n = 4608) fits the 50 MB L2 of an H100; algorithmic traffic
 // is 2/3 n^3 * 4 bytes of L2 reads for the products.  Everything is deterministic (no atomics on data).
 #include "eigh_direct.cuh"
 
@@ -112,20 +112,13 @@ __device__ __forceinline__ float reduce8h(float (&r)[8], int lane) {
   return r[0];
 }
 
-// packed fp32 pairs (FFMA2 / FMUL2 of sm_100): one issue slot for two fused multiply-adds
+// fp32 pairs: sm_90 has no packed fp32 instruction, so each pair is two round-to-nearest FFMA / FMUL
+// (the same rounding per element as a packed pair)
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra, rb, rc, rd;
-  memcpy(&ra, &a, 8); memcpy(&rb, &b, 8); memcpy(&rc, &c, 8);
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d; memcpy(&d, &rd, 8);
-  return d;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 __device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  unsigned long long ra, rb, rd;
-  memcpy(&ra, &a, 8); memcpy(&rb, &b, 8);
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  float2 d; memcpy(&d, &rd, 8);
-  return d;
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
 
 // sums of 16 per-lane values over the warp with 16 shuffles: afterwards every lane holds the complete sum of value
@@ -283,7 +276,7 @@ __device__ void tridiagonalise(const TrdMat& mt, int cta, int ncta, float* smem)
         }
         sub_sync(sg);
         const int tx = st_tid & 15, ty = st_tid >> 4;
-        float2 acc[4][2];                              // 4 x 4 outputs as packed pairs (FFMA2)
+        float2 acc[4][2];                              // 4 x 4 outputs as fp32 pairs
 #pragma unroll
         for (int i = 0; i < 4; ++i) { acc[i][0] = make_float2(0.f, 0.f); acc[i][1] = make_float2(0.f, 0.f); }
 #pragma unroll 8
@@ -333,7 +326,7 @@ __device__ void tridiagonalise(const TrdMat& mt, int cta, int ncta, float* smem)
     }
     // symmetric product with the lower tiles of this sub-group (128 threads: a warp takes 16 rows of the tile; its lower
     // half-warp rows 0..7, the upper one rows 8..15; a lane holds 4 adjacent columns of 8 rows).  The phase is bound by
-    // issue slots, not by bandwidth: 128-bit loads, packed fp32 pairs and half-warp reductions keep the count down.
+    // issue slots, not by bandwidth: 128-bit loads, fp32 pairs and half-warp reductions keep the count down.
     float vav = 0.f;
     {
       float* cs = stage + sg8 * (4 * T);             // column partial sums: [4 warps][64]

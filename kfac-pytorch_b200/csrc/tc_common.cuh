@@ -1,5 +1,5 @@
-// sm_100a building blocks: mbarrier, TMA (cp.async.bulk.tensor), TMEM
-// allocation, tcgen05.mma / tcgen05.ld / tcgen05.commit -- raw inline PTX.
+// sm_90a building blocks: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA
+// (wgmma.mma_async, kind tf32) and its shared-memory descriptors -- raw inline PTX.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -47,9 +47,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ------------------------------------------------------------------ TMA
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0,
                                             int c1, int c2) {
   asm volatile(
@@ -58,87 +55,47 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// ------------------------------------------------------------------ TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32 (fp32 containers, 10-bit mantissa used)
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// ------------------------------------------------------------------ wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, tf32 operands (fp32 containers, 10-bit mantissa used), fp32
+// accumulators in registers; both operands K-major in shared memory.  scale_d == 0: D = A B^T.
+// Accumulator layout (per warpgroup): warp w, lane l, d[4 j + 2 h + i] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + i].
+__device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], uint64_t a_desc, uint64_t b_desc, int scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+      "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
+      "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d)
       : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 // --------------------------------------------------------------- descriptors
-// K-major operand tile, rows of 128 B (32 fp32), SWIZZLE_128B, 8-row groups 1024 B
-// apart (cute::UMMA::SmemDescriptor: start>>4 | LBO<<16 | SBO<<32 | version=1<<46 | layout<<61).
+// K-major operand tile, rows of 128 B (32 fp32), SWIZZLE_128B as written by TMA, 8-row groups 1024 B apart
+// (sm_90 wgmma matrix descriptor: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 | layout << 62, SWIZZLE_128B = 1).
+// The tile base must be 1024-byte aligned; the next 8 reduction indices start 32 B further along the row.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;            // LBO (unused for swizzled K-major) = 1
   d |= (uint64_t)(1024 >> 4) << 32;  // SBO = 1024 B
-  d |= (uint64_t)1 << 46;            // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;            // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;            // SWIZZLE_128B
   return d;
-}
-// MN-major operand tile (the reduction index K runs over smem ROWS): 32-element (128 B)
-// MN atoms x 8 K rows, SWIZZLE_128B.  A {32 (MN), 32 (K)} TMA box lands as 4 such atoms
-// stacked along K (1024 B apart = SBO); boxes for successive MN ranges are 4096 B apart
-// (= LBO).  (cute canonical layout ((T,8,m),(8,k)):((1,T,LBO),(8T,SBO)).)
-__device__ __forceinline__ uint64_t make_mnmajor_sw128_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)(4096 >> 4) << 16;  // LBO: next 32-wide MN atom
-  d |= (uint64_t)(1024 >> 4) << 32;  // SBO: next group of 8 K rows
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// cute::UMMA::InstrDescriptor for kind::tf32, fp32 accumulate; mn_major: both operands MN-major
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, bool mn_major = false) {
-  return (1u << 4)                      // c_format = F32
-         | (2u << 7) | (2u << 10)       // a_format = b_format = TF32
-         | (mn_major ? ((1u << 15) | (1u << 16)) : 0u)   // a_major, b_major
-         | ((uint32_t)(N >> 3) << 17)   // n_dim
-         | ((uint32_t)(M >> 4) << 24);  // m_dim
 }
 
 }  // namespace tc

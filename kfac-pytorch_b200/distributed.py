@@ -1,5 +1,5 @@
 """Communication of the K-FAC hot path over torch.distributed (NCCL on the
-B200 box, gloo in the CPU tests).
+GPU, gloo in the CPU tests).
 
 Replaces kfac/distributed.py:124-385 (`TorchDistributedCommunicator`): instead
 of one async collective per tensor plus flatten/unflatten bucket copies, the

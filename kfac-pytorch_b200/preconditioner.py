@@ -32,7 +32,7 @@ def _mock_new_group(x: list[int]) -> None:
 
 
 class KFACPreconditioner(BaseKFACPreconditioner):
-    """K-FAC gradient preconditioner with KAISA placement on B200 (sm_100a)."""
+    """K-FAC gradient preconditioner with KAISA placement on H100 (sm_90a)."""
 
     def __init__(
         self,

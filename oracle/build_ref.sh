@@ -1,8 +1,8 @@
 #!/bin/bash
 # TEST INFRASTRUCTURE ONLY.  Installs the UNMODIFIED reference (gpauloski/kfac-pytorch, a pure
-# Python package) from /root/reference into oracle/_ref/ so that `bench.py --impl reference`
-# and the cpu_baseline leg can drive the real kfac.preconditioner.KFACPreconditioner on the
-# GPU box's host cores (oracle/_ref is git-ignored but travels with the gpurun snapshot).
+# Python package) from a reference checkout ($REFERENCE_ROOT) into oracle/_ref/ so that
+# `bench.py --impl reference` and the cpu_baseline leg can drive the real
+# kfac.preconditioner.KFACPreconditioner on the host cores (oracle/_ref is git-ignored).
 # No reference source is copied into the repository history.
 set -e
 HERE="$(cd "$(dirname "$0")" && pwd)"

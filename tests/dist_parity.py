@@ -91,7 +91,7 @@ def main():
                 print(f'rank {rank}: {pre._tdc.calls["allreduce"]} factor all-reduces, expected {want_calls}', flush=True)
                 ok = False
     # wide layers (a = 833 / 769, g = 768): the large-matrix eigensolver class, an eigenbasis broadcast
-    # segment of several MB (C2) and a multi-tile (6 x 7 tiles of 128 x 128) tcgen05 precondition epilogue
+    # segment of several MB (C2) and a multi-tile (6 x 7 tiles of 128 x 128) wgmma precondition epilogue
     # that stores straight into the peers' arenas (fused compute + broadcast, C3)
     class Wide(torch.nn.Module):
         def __init__(self):

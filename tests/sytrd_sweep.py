@@ -1,5 +1,5 @@
 """Diagnostic: tridiagonalisation time over (n, CTA group size), the data the schedule model of eigh_direct.cu is fitted to.
-python tests/sytrd_sweep.py > gpurun_out/sytrd_sweep.csv"""
+python tests/sytrd_sweep.py > sytrd_sweep.csv"""
 import ctypes as C
 import os
 import sys
@@ -24,7 +24,7 @@ for n in (256, 512, 576, 1024, 1152, 2048, 2304, 4608):
     d, e, tau = torch.zeros(n, device=dev), torch.zeros(n, device=dev), torch.zeros(n, device=dev)
     need = lib.kfac_stage_direct_workspace_bytes(n)
     ws = torch.empty(need, dtype=torch.uint8, device=dev)
-    for ncta in (1, 2, 3, 4, 6, 8, 12, 16, 24, 36, 48, 72, 100, 148):
+    for ncta in (1, 2, 3, 4, 6, 8, 12, 16, 24, 36, 48, 72, 100, 132):
         best = 1e9
         ok = True
         for it in range(3):

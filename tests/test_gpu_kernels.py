@@ -30,8 +30,8 @@ def S():
     return torch.cuda.current_stream().cuda_stream
 
 
-def test_device_is_blackwell(lib):
-    assert lib.kfac_device_arch() >= 100
+def test_device_is_hopper(lib):
+    assert lib.kfac_device_arch() == 90
 
 
 @pytest.mark.parametrize('M,N,K', [(1, 1, 1), (7, 5, 3), (64, 64, 64), (100, 130, 257), (20, 577, 64), (300, 33, 1000)])
@@ -66,11 +66,16 @@ def test_factor_linear(lib, dev, rows, feat, ones, dtype):
     assert lib.kfac_factor_linear(xd.data_ptr(), {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}[dtype],
                                   rows, feat, ones, 1.0 / rows, acc.data_ptr(), ws.data_ptr() if need else None, need,
                                   S()) == 0
+    acc2 = torch.zeros_like(acc)
+    assert lib.kfac_factor_linear(xd.data_ptr(), {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}[dtype],
+                                  rows, feat, ones, 1.0 / rows, acc2.data_ptr(), ws.data_ptr() if need else None, need,
+                                  S()) == 0
     torch.cuda.synchronize()
     ref = O.linear_a_factor(x.float(), bool(ones))
     got = 0.5 * (acc + acc.t())
     assert rel_fro(got, ref) < 2e-5
     assert torch.equal(acc, acc.t()) or rel_fro(acc, acc.t()) < 1e-6
+    assert torch.equal(acc, acc2)        # the same bits in every call
 
 
 def test_get_cov_reference_vector_on_gpu(lib, dev):
@@ -130,12 +135,18 @@ def test_factor_conv2d_gradout(lib, dev, B, Cc, Ho, Wo, with_ws):
     gd = g.to(dev)
     scale = 1.0 / (B * float(Ho * Wo) ** 3)
     need = lib.kfac_factor_conv2d_gradout_workspace_bytes(B, Cc, Ho, Wo) if with_ws else 0
-    assert (need > 0) == (with_ws and (Ho * Wo) % 4 != 0 and Cc >= 64)
+    # maps whose rows are not 16-byte multiples are packed (feature-major, rows padded to 4); the workspace also
+    # holds the split partials of the SYRK
+    packed = (B * Ho * Wo + 3) // 4 * 4 * Cc * 4 if (Ho * Wo) % 4 != 0 and Cc >= 64 else 0
+    assert not with_ws or need >= packed
     ws = torch.empty(max(need, 1), dtype=torch.uint8, device=dev)
-    assert lib.kfac_factor_conv2d_gradout(gd.data_ptr(), 0, B, Cc, Ho, Wo, scale, acc.data_ptr(),
-                                          ws.data_ptr() if need else None, need, S()) == 0
+    acc2 = torch.zeros_like(acc)
+    for out in (acc, acc2):
+        assert lib.kfac_factor_conv2d_gradout(gd.data_ptr(), 0, B, Cc, Ho, Wo, scale, out.data_ptr(),
+                                              ws.data_ptr() if need else None, need, S()) == 0
     torch.cuda.synchronize()
     assert rel_fro(0.5 * (acc + acc.t()), ref) < 2e-5
+    assert torch.equal(acc, acc2)        # the same bits in every call
 
 
 def test_factor_ema(lib, dev):

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM engine (3xTF32 split, TMA-fed, TMEM accumulators) vs fp64."""
+"""wgmma GEMM engine (3xTF32 split, TMA-fed, register accumulators) vs fp64."""
 import pytest
 import torch
 
@@ -34,8 +34,8 @@ def test_tc_gemm_matches_fp64(lib, M, N, K):
     torch.cuda.synchronize()
     ref = 0.5 * (A[:, :K].double() @ B[:, :K].double().t())
     e = rel_fro(D, ref)
-    # single-pass TF32 gives ~5e-4 here; the 3-term split is fp32-class.  The TMEM
-    # accumulator truncates (one truncating add per k-step of 8): allow ~4e-9 * K.
+    # single-pass TF32 gives ~5e-4 here; the 3-term split is fp32-class.  The tensor-core
+    # accumulator may truncate (one add per k-step of 8): allow ~4e-9 * K.
     assert e < 3e-6 + 4e-9 * K, (M, N, K, e)
     e_max = ((D.double() - ref).abs().max() / ref.abs().max()).item()
     assert e_max < 2e-5 + 1e-8 * K, e_max

@@ -209,7 +209,7 @@ def test_arena_entries_are_16_byte_aligned():
 
 
 def test_bench_reference_arm_contract():
-    """`bench.py --impl reference` (the CPU arm the driver runs beside the B200 arm) prints ONE JSON
+    """`bench.py --impl reference` (the CPU arm run beside the GPU arm) prints ONE JSON
     line with the contract keys; exercised on the small workload so it stays in the CPU budget."""
     import json
     import subprocess
