@@ -150,8 +150,11 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
                                    (int)tc::PSMEM));
     attr = true;
   }
+  // the arguments of every problem are checked (and every tensor map encoded) before anything is launched: a
+  // rejected call leaves all outputs untouched
   std::vector<GProb> tab;
   std::vector<RProb> red;
+  std::vector<int> simt;
   long long red_total = 0;
   int work = 0;
   for (int i = 0; i < count; ++i) {
@@ -167,21 +170,7 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
       set_error("grouped gemm: a device-side k range needs the atomic mode on the tensor-core path");
       return KFAC_ERR_BAD_ARG;
     }
-    if (!grouped_gemm_tc_ok(g)) {
-      // small / unaligned problems: one SIMT launch each (fp32, no split needed)
-      GemmArgs a{};
-      a.A = g.A; a.sa_m = g.lda; a.sa_k = 1; a.B = g.B; a.sb_k = 1; a.sb_n = g.ldb;
-      a.C = g.D; a.ldc = g.ldd; a.M = g.M; a.N = g.N; a.K = g.K; a.batch = 1; a.splitk = 1;
-      a.alpha = g.alpha; a.beta = g.mode == 0 ? 0.f : 1.f; a.epi = g.epi; a.E = g.E; a.lde = g.lde; a.dg = g.dg; a.da = g.da; a.damping = g.damping;
-      int rc = launch_gemm(a, s);
-      if (rc) return rc;
-      if (g.npeer > 0) {
-        for (int q = 0; q < g.npeer; ++q)
-          KFAC_CUDA(cudaMemcpy2DAsync(g.peerD[q], (size_t)g.ldd * 4, g.D, (size_t)g.ldd * 4, (size_t)g.N * 4, g.M,
-                                      cudaMemcpyDeviceToDevice, s));
-      }
-      continue;
-    }
+    if (!grouped_gemm_tc_ok(g)) { simt.push_back(i); continue; }
     GProb p{};
     int rc;
     if ((rc = make_tmap_3d(&p.tmA, g.A, (uint64_t)g.K, (uint64_t)g.M, 1, (uint64_t)g.lda * 4, (uint64_t)g.lda * 4 * g.M, GBM))) return rc;
@@ -209,6 +198,21 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
     work += tiles * p.splits;
     tab.push_back(p);
   }
+  for (const int i : simt) {
+    // small / unaligned problems: one SIMT launch each (fp32, no split needed)
+    const GroupedGemm& g = probs[i];
+    GemmArgs a{};
+    a.A = g.A; a.sa_m = g.lda; a.sa_k = 1; a.B = g.B; a.sb_k = 1; a.sb_n = g.ldb;
+    a.C = g.D; a.ldc = g.ldd; a.M = g.M; a.N = g.N; a.K = g.K; a.batch = 1; a.splitk = 1;
+    a.alpha = g.alpha; a.beta = g.mode == 0 ? 0.f : 1.f; a.epi = g.epi; a.E = g.E; a.lde = g.lde; a.dg = g.dg; a.da = g.da; a.damping = g.damping;
+    int rc = launch_gemm(a, s);
+    if (rc) return rc;
+    if (g.npeer > 0) {
+      for (int q = 0; q < g.npeer; ++q)
+        KFAC_CUDA(cudaMemcpy2DAsync(g.peerD[q], (size_t)g.ldd * 4, g.D, (size_t)g.ldd * 4, (size_t)g.N * 4, g.M,
+                                    cudaMemcpyDeviceToDevice, s));
+    }
+  }
   if (tab.empty()) return KFAC_OK;
   GProb* d_tab = (GProb*)ws;
   RProb* d_red = (RProb*)((char*)ws + align_up(sizeof(GProb) * (size_t)std::max(1, count), 256));
@@ -227,3 +231,36 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
 }
 
 }  // namespace kfac
+
+// test entry (not in the public header): the grouped engine on a list of problems, without peer stores.
+// Mirrors GroupedGemm minus the peer fields.
+struct kfac_stage_gemm {
+  const float* A; int64_t lda;
+  const float* B; int64_t ldb;
+  float* D; int64_t ldd;
+  int M, N, K;
+  float alpha;
+  int epi; const float* E; int64_t lde; const float* dg; const float* da; float damping;
+  int splits; float* slab; int64_t slab_stride;
+  int mode; const int* krange;
+};
+
+extern "C" size_t kfac_stage_grouped_gemm_ws_bytes(int count) { return kfac::grouped_gemm_ws_bytes(count); }
+
+extern "C" int kfac_stage_grouped_gemm(const kfac_stage_gemm* probs, int count, void* ws, size_t ws_bytes,
+                                       void* stream) {
+  using namespace kfac;
+  KFAC_CHECK_ARG(count >= 0 && (probs || count == 0), "grouped gemm test args");
+  std::vector<GroupedGemm> g(count);
+  for (int i = 0; i < count; ++i) {
+    const kfac_stage_gemm& p = probs[i];
+    GroupedGemm q{};
+    q.A = p.A; q.lda = p.lda; q.B = p.B; q.ldb = p.ldb; q.D = p.D; q.ldd = p.ldd;
+    q.M = p.M; q.N = p.N; q.K = p.K; q.alpha = p.alpha;
+    q.epi = p.epi; q.E = p.E; q.lde = p.lde; q.dg = p.dg; q.da = p.da; q.damping = p.damping;
+    q.splits = p.splits; q.slab = p.slab; q.slab_stride = p.slab_stride;
+    q.mode = p.mode; q.krange = p.krange;
+    g[i] = q;
+  }
+  return launch_grouped_gemm(g.data(), count, ws, ws_bytes, (cudaStream_t)stream);
+}

@@ -383,6 +383,117 @@ def test_precondition_and_update(lib, dev, g, a, bias, method):
     assert rel_fro(new, ref_scale * ref) < 2e-4
 
 
+def bits(x):
+    """Bit pattern of a float tensor, for bitwise comparisons."""
+    return x.contiguous().view(torch.int32 if x.element_size() == 4 else torch.int16)
+
+
+def test_precondition_many_layers_half_precision(lib, dev):
+    """One precondition call over several layers, as the product makes it: split stages (a, g > 1024; a not a
+    multiple of 4), layers small enough for the SIMT fallback, fp32 / fp16 / bf16 gradients, and dgda (EPI_MUL)
+    next to da/dg (EPI_DIV_OUTER) layers in the same grouped launch; then the inverse method over the same list,
+    the kl-clip scale and the write-back, each against fp64 on the gradient values as stored."""
+    from kfac_b200 import _cabi
+    from oracle import kfac_oracle as O
+    damping = float(torch.tensor(0.003, dtype=torch.float32))
+    layers = [(1030, 1153, 1, torch.bfloat16, 'dgda'),   # g, a, bias, gradient dtype, eigen epilogue
+              (48, 200, 0, torch.float16, 'dadg'),
+              (10, 21, 1, torch.bfloat16, 'dgda'),
+              (512, 2049, 0, torch.float32, 'dadg'),
+              (200, 300, 1, torch.float16, 'dgda')]
+    gen = torch.Generator(device=dev).manual_seed(11)
+    nan = float('nan')
+
+    def stored(x):   # (rows, cols) fp32 in storage with ld4(cols) and NaN padding columns
+        out = torch.full((x.shape[0], _cabi.ld4(x.shape[1])), nan, device=dev)
+        out[:, :x.shape[1]] = x
+        return out
+
+    def basis(n):    # orthogonal eigenbasis and a spread of non-negative eigenvalues, fp32 as stored
+        q, _ = torch.linalg.qr(torch.randn(n, n, dtype=torch.float64, device=dev, generator=gen))
+        return q.float(), (torch.rand(n, dtype=torch.float64, device=dev, generator=gen) ** 4).float()
+
+    L = []
+    for g, a, bias, dtype, epi in layers:
+        qa, da = basis(a)
+        qg, dg = basis(g)
+        w = torch.randn(g, a - bias, device=dev, generator=gen).to(dtype)
+        b = torch.randn(g, device=dev, generator=gen).to(dtype) if bias else None
+        grad = O.grad_matrix(w.double(), b.double() if bias else None)
+        dgda = O.eigen_dgda(dg.double(), da.double(), damping).float()
+        a_inv = ((qa.double() / (da.double() + damping)) @ qa.double().t()).float()
+        g_inv = ((qg.double() / (dg.double() + damping)) @ qg.double().t()).float()
+        if epi == 'dgda':
+            ref_e = O.precondition_eigen(grad, qa.double(), qg.double(), dgda=dgda.double())
+        else:
+            ref_e = O.precondition_eigen(grad, qa.double(), qg.double(), da=da.double(), dg=dg.double(), damping=damping)
+        ref_i = O.precondition_inverse(grad, a_inv.double(), g_inv.double())
+        L.append(dict(g=g, a=a, bias=bias, dtype=dtype, epi=epi, w=w, b=b, grad=grad, ref_e=ref_e, ref_i=ref_i,
+                      qa=stored(qa), qaT=stored(qa.t()), qg=stored(qg), qgT=stored(qg.t()), dgda=stored(dgda),
+                      da=da, dg=dg, a_inv=stored(a_inv), g_inv=stored(g_inv)))
+
+    def precondition(method):
+        """kfac_precondition over all layers into fresh NaN-filled P buffers and a NaN-filled workspace."""
+        items = (_cabi.PrecondItem * len(L))()
+        Ps = []
+        for i, l in enumerate(L):
+            g, a = l['g'], l['a']
+            lda_, ldg_ = _cabi.ld4(a), _cabi.ld4(g)
+            P = torch.full((g, lda_), nan, device=dev)
+            Ps.append(P)
+            e = method == _cabi.KFAC_EIGEN
+            p = lambda k, use: l[k].data_ptr() if use else None  # noqa: E731
+            items[i] = _cabi.PrecondItem(l['w'].data_ptr(), l['b'].data_ptr() if l['bias'] else None,
+                                         _cabi.DTYPE_CODE[l['dtype']], g, a,
+                                         p('qa', e), p('qaT', e), p('qg', e), p('qgT', e), p('dgda', e and l['epi'] == 'dgda'),
+                                         p('da', e and l['epi'] == 'dadg'), p('dg', e and l['epi'] == 'dadg'),
+                                         p('a_inv', not e), p('g_inv', not e), lda_, ldg_, lda_, P.data_ptr(), lda_)
+        need = lib.kfac_precondition_workspace_bytes(items, len(L))
+        ws = torch.full((need,), 255, dtype=torch.uint8, device=dev)     # all-ones bytes: NaN floats
+        rc = lib.kfac_precondition(items, len(L), method, damping, ws.data_ptr(), need, S())
+        assert rc == 0, lib.kfac_last_error()
+        torch.cuda.synchronize()
+        return [P[:, :l['a']] for P, l in zip(Ps, L)]
+
+    out = {}
+    for method, key in ((_cabi.KFAC_EIGEN, 'ref_e'), (_cabi.KFAC_INVERSE, 'ref_i')):
+        P1 = out[method] = precondition(method)
+        for P, l in zip(P1, L):
+            assert rel_fro(P, l[key]) < 1e-4, (method, l['g'], l['a'], rel_fro(P, l[key]))
+        P2 = precondition(method)
+        for p1, p2, l in zip(P1, P2, L):     # the same bits in every call
+            assert torch.equal(bits(p1), bits(p2)), (method, l['g'], l['a'])
+    Pe = out[_cabi.KFAC_EIGEN]
+
+    # kl-clip scale: nu = min(1, sqrt(kl_clip / |lr^2 sum P * grad|)), kl_clip chosen so that nu ~ 0.5
+    gi = (_cabi.GradItem * len(L))()
+    for i, (P, l) in enumerate(zip(Pe, L)):
+        gi[i] = _cabi.GradItem(P.data_ptr(), l['w'].data_ptr(), l['b'].data_ptr() if l['bias'] else None,
+                               _cabi.DTYPE_CODE[l['dtype']], l['g'], l['a'], _cabi.ld4(l['a']))
+    vg = sum(float((P.double() * l['grad']).sum()) for P, l in zip(Pe, L))
+    lr = float(torch.tensor(0.1, dtype=torch.float32))
+    kl_clip = float(torch.tensor(0.25 * abs(vg) * lr * lr, dtype=torch.float32))
+    nu_ref = min(1.0, (kl_clip / abs(vg * lr * lr)) ** 0.5)
+    gneed = lib.kfac_grad_workspace_bytes(len(L))
+    gws = torch.full((gneed,), 255, dtype=torch.uint8, device=dev)
+    nu = torch.zeros(1, device=dev)
+    assert lib.kfac_grad_scale(gi, len(L), kl_clip, lr, gws.data_ptr(), gneed, nu.data_ptr(), S()) == 0
+    torch.cuda.synchronize()
+    assert nu_ref < 1.0 and abs(float(nu) - nu_ref) <= 1e-6 * nu_ref, (float(nu), nu_ref)
+
+    # write-back: fp32 multiply, then round to nearest even into the gradient dtype -- bit for bit
+    for scale in (nu, None):
+        assert lib.kfac_grad_update(gi, len(L), scale.data_ptr() if scale is not None else None, gws.data_ptr(),
+                                    gneed, S()) == 0
+        torch.cuda.synchronize()
+        for P, l in zip(Pe, L):
+            want = (scale * P if scale is not None else P).to(l['dtype'])
+            aw = l['a'] - l['bias']
+            assert torch.equal(bits(l['w']), bits(want[:, :aw])), (l['g'], l['a'], l['dtype'], scale is None)
+            if l['bias']:
+                assert torch.equal(bits(l['b']), bits(want[:, aw])), (l['g'], l['a'], l['dtype'], scale is None)
+
+
 def test_not_ready_maps_to_runtime_error(lib, dev):
     from kfac_b200 import _cabi
     w = torch.randn(4, 4, device=dev)
