@@ -102,6 +102,21 @@ typedef struct kfac_ema_item {
 int kfac_factor_ema(const kfac_ema_item* items, int count, float alpha,
                     void* stream);
 
+/* Guarded EMA for mixed-precision training with a dynamic loss scale (replaces the
+ * division of the grad-outputs by grad_scaler() in layers/base.py:365-366).
+ * loss_scale: HOST array of `count` DEVICE pointers to one float each (NULL array or
+ * NULL entry = 1); the window of item i is multiplied by u = (1 / *loss_scale[i])^2 as it
+ * is read.  A window with an entry whose unscaled value is not finite or exceeds 1e15 in
+ * magnitude (the bound kfac_eigh_batched rejects) is DROPPED: its factor keeps its value
+ * (becomes exactly I when `first` = 1), its batch is zeroed and *skipped (device counter,
+ * may be NULL) is incremented.  Every other item gets the bits kfac_factor_ema gives on
+ * batch * u (on batch itself for a NULL scale).  ws: kfac_factor_ema_guarded_workspace_bytes(count)
+ * bytes of device memory (one drop flag per item).  Two launches per 40 items (scan, EMA). */
+size_t kfac_factor_ema_guarded_workspace_bytes(int count);
+int kfac_factor_ema_guarded(const kfac_ema_item* items, int count, float alpha,
+                            const float* const* loss_scale, unsigned long long* skipped,
+                            void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------- eigendecomposition
  * K5: replaces torch.linalg.eigh + clamp(min=0) in
  * KFACEigenLayer.compute_{a,g}_inv (kfac/layers/eigen.py:295-344).

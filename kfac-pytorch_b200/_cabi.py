@@ -61,6 +61,9 @@ SIGNATURES = {
     'kfac_factor_conv2d_gradout_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
     'kfac_factor_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     'kfac_factor_ema': (c_int, [C.POINTER(EmaItem), c_int, c_float, c_void_p]),
+    'kfac_factor_ema_guarded_workspace_bytes': (c_size_t, [c_int]),
+    'kfac_factor_ema_guarded': (c_int, [C.POINTER(EmaItem), c_int, c_float, C.POINTER(c_void_p), c_void_p,
+                                        c_void_p, c_size_t, c_void_p]),
     'kfac_eigh_workspace_bytes': (c_size_t, [C.POINTER(c_int), c_int]),
     'kfac_eigh_batched': (c_int, [C.POINTER(EighItem), c_int, c_void_p, c_size_t, c_int, c_float, c_void_p]),
     'kfac_eigh_status': (c_int, [c_void_p, c_void_p, c_void_p]),

@@ -14,6 +14,26 @@ What is different underneath (H100-first):
     scale stays on the device);
   * each communication phase is one collective per (source, group) on an
     arena slice instead of 1-3 collectives per layer.
+
+Mixed precision with a loss scale (`grad_scaler=`): every factor update then
+runs through the guarded EMA, which drops a window whose statistics are not
+finite (an fp16 overflow step) instead of carrying it into the running factor.
+With a `torch.amp.GradScaler` the scale is never read on the host: each G hook
+copies the scaler's current scale into a per-layer device slot, the G
+statistics are formed unscaled, and the EMA multiplies the window by 1/s^2
+from that slot.  This relies on the order of the usual AMP loop:
+
+    scaler.scale(loss).backward()   # G hooks snapshot the scale
+    scaler.unscale_(optimizer)
+    preconditioner.step()           # every closed window is consumed here
+    scaler.step(optimizer)
+    scaler.update()                 # the scale changes only here
+
+so all micro-batches of a window share one scale.  A window that stays open
+across step() (step() called before `accumulation_steps` micro-batches have
+run) can span an update() and so two scales; the last snapshot is applied to
+the whole window.  Under data parallelism every rank must use the same scale,
+as GradScaler does when it unscales gradients that DDP has already averaged.
 """
 from __future__ import annotations
 
@@ -209,6 +229,10 @@ class BaseKFACPreconditioner:
         self._gemm_scratch = _Scratch()     # precondition / inverse temporaries
         self._grad_scratch = _Scratch()     # kl-clip / write-back item table + partial sums
         self._pending_alpha: dict[float, list[tuple[KFACLayer, str]]] = {}
+        # with a loss scale every factor goes through the guarded EMA (non-finite windows are dropped and counted)
+        self._guard_factors = any(l.grad_scaler is not None for _, l in self._layers.values())
+        self._ema_scratch = _Scratch()        # drop flags of the guarded EMA
+        self._skipped: torch.Tensor | None = None   # device counter of dropped windows
         # C1: the batch statistics (not the factors) are averaged over the ranks BEFORE the EMA -- the same factors by
         # linearity -- so that the A block can be reduced while backward still runs (base_preconditioner.py:452-457)
         self.overlap_factor_allreduce = True
@@ -258,6 +282,12 @@ class BaseKFACPreconditioner:
     @property
     def steps(self) -> int:
         return self._steps
+
+    @property
+    def skipped_factor_updates(self) -> int:
+        """Number of factor windows the guarded EMA has dropped because their statistics were not finite (or
+        exceeded 1e15 in magnitude).  Only counted with a `grad_scaler`; reading it synchronises the device."""
+        return int(self._skipped.item()) if self._skipped is not None else 0
 
     # ------------------------------------------------------------ arenas
     def _layer_list(self) -> list[tuple[str, KFACLayer]]:
@@ -339,6 +369,11 @@ class BaseKFACPreconditioner:
             l._inv[key] = _bind(self._local_arena, off, shape)
             l._inv_cols[key] = shape[-1]
             off += _storage_numel(shape)
+        if self._guard_factors:
+            self._skipped = torch.zeros(1, dtype=torch.int64, device=device)
+            self._g_scales = torch.ones(len(ll), dtype=torch.float32, device=device)
+            for i, (_, l) in enumerate(ll):
+                l._g_scale_slot = self._g_scales.narrow(0, i, 1)
         self._vg = torch.zeros(1, dtype=torch.float64, device=device)
         self._nu = torch.ones(1, dtype=torch.float32, device=device)
         self._arenas_ready = True
@@ -469,7 +504,20 @@ class BaseKFACPreconditioner:
 
     # ------------------------------------------------------------ hooks
     def _grad_scale_value(self, layer: KFACLayer) -> float:
-        return float(layer.grad_scaler()) if layer.grad_scaler is not None else 1.0
+        """Loss scale folded into the G statistics on the host (1 when the guarded EMA applies it on the device)."""
+        if layer.grad_scaler is None or layer.device_grad_scaler:
+            return 1.0
+        return float(layer.grad_scaler())
+
+    @staticmethod
+    def _snapshot_loss_scale(layer: KFACLayer) -> None:
+        """Stream-ordered copy of the GradScaler's current scale into the layer's device slot (no host sync)."""
+        scaler = layer.grad_scaler
+        scale = scaler._get_scale_async() if scaler.is_enabled() else None
+        if scale is not None:
+            layer._g_scale_slot.copy_(scale)
+        else:
+            layer._g_scale_slot.fill_(scaler._init_scale if scaler.is_enabled() else 1.0)
 
     @torch.no_grad()
     def _save_input(self, module: torch.nn.Module, input_: tuple[torch.Tensor, ...]) -> None:
@@ -509,6 +557,8 @@ class BaseKFACPreconditioner:
             self._flush_factor_updates()
         if self._update_factors_in_hook and self._mini_steps[name] % self._accumulation_steps == 0:
             self._launch_a_block_reduction()     # first backward hook of the window: every A statistic is complete
+        if layer.device_grad_scaler:
+            self._snapshot_loss_scale(layer)
         # the backward hook runs on the autograd thread: it gets its own scratch buffer
         layer.module.accumulate_g(cast_for_factor(g, layer.factor_dtype), layer._g_batch_view,
                                   self._grad_scale_value(layer), self._scratch_bwd)
@@ -593,8 +643,10 @@ class BaseKFACPreconditioner:
             return
         self._reduce_batches()
         lib = _cabi.load()
+        stream = _cabi.stream_ptr()
         for alpha, todo in self._pending_alpha.items():
             items = (_cabi.EmaItem * len(todo))()
+            scales = (C.c_void_p * len(todo))()      # guarded EMA: loss-scale slot of a G item, NULL otherwise
             for i, (layer, which) in enumerate(todo):
                 if which == 'a':
                     items[i] = _cabi.EmaItem(layer._a_view.data_ptr(), layer._a_batch_view.data_ptr(),
@@ -603,8 +655,17 @@ class BaseKFACPreconditioner:
                 else:
                     items[i] = _cabi.EmaItem(layer._g_view.data_ptr(), layer._g_batch_view.data_ptr(),
                                              layer.g_dim, int(not layer._has_g), 1.0 / layer._g_count)
+                    if layer.device_grad_scaler:
+                        scales[i] = layer._g_scale_slot.data_ptr()
                     layer._has_g, layer._g_count, layer._g_pending = True, 0, False
-            _cabi.check(lib.kfac_factor_ema(items, len(todo), alpha, _cabi.stream_ptr()), 'kfac_factor_ema')
+            if not self._guard_factors:
+                _cabi.check(lib.kfac_factor_ema(items, len(todo), alpha, stream), 'kfac_factor_ema')
+                continue
+            # decided after C1, so every rank drops the same windows
+            need = lib.kfac_factor_ema_guarded_workspace_bytes(len(todo))
+            ws = self._ema_scratch.get(need, self._device)
+            _cabi.check(lib.kfac_factor_ema_guarded(items, len(todo), alpha, scales, self._skipped.data_ptr(),
+                                                    ws.data_ptr(), need, stream), 'kfac_factor_ema_guarded')
         self._pending_alpha = {}
 
     # ------------------------------------------------------------ step

@@ -263,8 +263,30 @@ struct EmaBatch {
   int first_block[41];   // prefix sums of the number of tile pairs T (T + 1) / 2 per item
   int count;
   float alpha;
+  // guarded EMA only: per-item loss scale (NULL = 1), drop flags set by window_scan_kernel, drop counter
+  const float* scale[40];
+  const int* dropped;
+  unsigned long long* skipped;
 };
 
+// 1/s^2 of a loss scale, formed as (1/s)^2: exact for the powers of two a GradScaler uses, and still normal for
+// scales up to 2^63 (s * s would overflow first).  A non-finite or zero scale gives a non-finite or zero factor,
+// which makes every non-zero window entry non-finite, so the window is dropped.
+__device__ __forceinline__ float window_unscale(const float* s) {
+  if (s == nullptr) return 1.f;
+  const float r = 1.f / *s;
+  return r * r;
+}
+
+// alpha * f + beta * (x + y), rounded as fma(beta, x + y, alpha * f).  Spelled out so that the compiler cannot contract
+// it differently in the two instantiations of ema_kernel: the guarded EMA must give the bits of the unguarded one.
+__device__ __forceinline__ float ema_update(float alpha, float f, float beta, float x, float y) {
+  return __fmaf_rn(beta, __fadd_rn(x, y), __fmul_rn(alpha, f));
+}
+
+// GUARD = false: kfac_factor_ema.  GUARD = true: the window is multiplied by window_unscale() as it is read, and a
+// window flagged by window_scan_kernel is dropped (factor unchanged, or I when it is the first window; batch = 0).
+template <bool GUARD>
 __global__ void __launch_bounds__(256) ema_kernel(const __grid_constant__ EmaBatch eb) {
   __shared__ float A[32][33], B[32][33];
   int item = 0;
@@ -279,12 +301,22 @@ __global__ void __launch_bounds__(256) ema_kernel(const __grid_constant__ EmaBat
   const int d = it.d, tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const float alpha = eb.alpha, beta = (1.f - eb.alpha) * it.inv_count * 0.5f;
   const int i0 = ti * 32, j0 = tj * 32;
+  bool drop = false;
+  float u = 1.f;
+  if (GUARD) {
+    drop = eb.dropped[item] != 0;
+    u = window_unscale(eb.scale[item]);
+    if (drop && p == 0 && threadIdx.x == 0 && eb.skipped) atomicAdd(eb.skipped, 1ull);
+  }
 #pragma unroll
   for (int r = ty; r < 32; r += 8) {
     const int iu = i0 + r, ju = j0 + tx;   // upper tile (ti, tj)
-    A[r][tx] = (iu < d && ju < d) ? it.batch[(int64_t)iu * d + ju] : 0.f;
+    float va = (iu < d && ju < d) ? it.batch[(int64_t)iu * d + ju] : 0.f;
     const int il = j0 + r, jl = i0 + tx;   // mirror tile (tj, ti)
-    B[r][tx] = (il < d && jl < d) ? it.batch[(int64_t)il * d + jl] : 0.f;
+    float vb = (il < d && jl < d) ? it.batch[(int64_t)il * d + jl] : 0.f;
+    if (GUARD) { va *= u; vb *= u; }
+    A[r][tx] = va;
+    B[r][tx] = vb;
   }
   __syncthreads();
 #pragma unroll
@@ -293,9 +325,12 @@ __global__ void __launch_bounds__(256) ema_kernel(const __grid_constant__ EmaBat
       const int i = i0 + r, j = j0 + tx;
       if (i < d && j < d) {
         const int64_t idx = (int64_t)i * d + j;
-        const float s = beta * (A[r][tx] + B[tx][r]);
-        const float f = it.first ? (i == j ? 1.f : 0.f) : it.factor[idx];
-        it.factor[idx] = alpha * f + s;
+        if (!drop) {
+          const float f = it.first ? (i == j ? 1.f : 0.f) : it.factor[idx];
+          it.factor[idx] = ema_update(alpha, f, beta, A[r][tx], B[tx][r]);
+        } else if (it.first) {
+          it.factor[idx] = i == j ? 1.f : 0.f;
+        }
         it.batch[idx] = 0.f;
       }
     }
@@ -303,13 +338,53 @@ __global__ void __launch_bounds__(256) ema_kernel(const __grid_constant__ EmaBat
       const int i = j0 + r, j = i0 + tx;
       if (i < d && j < d) {
         const int64_t idx = (int64_t)i * d + j;
-        const float s = beta * (A[tx][r] + B[r][tx]);
-        const float f = it.first ? 0.f : it.factor[idx];
-        it.factor[idx] = alpha * f + s;
+        if (!drop) {
+          const float f = it.first ? 0.f : it.factor[idx];
+          it.factor[idx] = ema_update(alpha, f, beta, A[tx][r], B[r][tx]);
+        } else if (it.first) {
+          it.factor[idx] = 0.f;
+        }
         it.batch[idx] = 0.f;
       }
     }
   }
+}
+
+// Drop flags of the guarded EMA: dropped[i] = 1 if an entry of window i, unscaled, is not finite or exceeds 1e15 in
+// magnitude (the bound the eigensolver rejects).  Every block of an item strides over its d x d window (16-byte
+// loads where the window is 16-byte aligned); the flag is raised with an integer atomic, so the result does not
+// depend on the order of the blocks.
+struct ScanBatch {
+  const float* batch[40];
+  const float* scale[40];
+  int64_t n[40];         // d * d
+  int first_block[41];   // prefix sums of the blocks per item
+  int count;
+  int* dropped;
+};
+
+__device__ __forceinline__ bool window_entry_bad(float v, float u) { return !(fabsf(v * u) <= 1e15f); }
+
+__global__ void __launch_bounds__(256) window_scan_kernel(const __grid_constant__ ScanBatch sb) {
+  int item = 0;
+  while (item + 1 < sb.count && (int)blockIdx.x >= sb.first_block[item + 1]) ++item;
+  const float* __restrict__ x = sb.batch[item];
+  const int64_t n = sb.n[item];
+  const float u = window_unscale(sb.scale[item]);
+  const int64_t tid = (int64_t)(blockIdx.x - sb.first_block[item]) * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)(sb.first_block[item + 1] - sb.first_block[item]) * blockDim.x;
+  bool bad = false;
+  int64_t done = 0;
+  if ((reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+    const float4* __restrict__ x4 = reinterpret_cast<const float4*>(x);
+    for (int64_t i = tid; i < n / 4; i += stride) {
+      const float4 v = x4[i];
+      bad |= window_entry_bad(v.x, u) | window_entry_bad(v.y, u) | window_entry_bad(v.z, u) | window_entry_bad(v.w, u);
+    }
+    done = n / 4 * 4;
+  }
+  for (int64_t i = done + tid; i < n; i += stride) bad |= window_entry_bad(x[i], u);
+  if (__syncthreads_or(bad) && threadIdx.x == 0) atomicOr(sb.dropped + item, 1);
 }
 
 __global__ void dgda_kernel(const float* dg, const float* da, int g, int a, float damping, float* out, int ldo) {
@@ -513,9 +588,10 @@ extern "C" int kfac_factor_conv2d_gradout(const void* g, int dtype, int batch, i
   return launch_cov<true>(a, dtype, (cudaStream_t)stream);
 }
 
-extern "C" int kfac_factor_ema(const kfac_ema_item* items, int count, float alpha, void* stream) {
-  KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "items");
-  cudaStream_t s = (cudaStream_t)stream;
+// EMA over up to 40 items per launch.  guard: `dropped` (one int per item, zeroed) receives the drop flags of a scan
+// launch that precedes each EMA launch.
+static int launch_ema(const kfac_ema_item* items, int count, float alpha, const float* const* loss_scale,
+                      int* dropped, unsigned long long* skipped, cudaStream_t s) {
   for (int base = 0; base < count; base += 40) {
     EmaBatch eb{};
     eb.count = min(40, count - base);
@@ -529,10 +605,57 @@ extern "C" int kfac_factor_ema(const kfac_ema_item* items, int count, float alph
       blocks += T * (T + 1) / 2;
     }
     eb.first_block[eb.count] = blocks;
-    ema_kernel<<<blocks, 256, 0, s>>>(eb);
+    if (!dropped) {
+      ema_kernel<false><<<blocks, 256, 0, s>>>(eb);
+      KFAC_LAUNCH_CHECK();
+      continue;
+    }
+    ScanBatch sb{};
+    sb.count = eb.count;
+    sb.dropped = dropped + base;
+    int scan_blocks = 0;
+    for (int i = 0; i < eb.count; ++i) {
+      eb.scale[i] = sb.scale[i] = loss_scale ? loss_scale[base + i] : nullptr;
+      sb.batch[i] = eb.it[i].batch;
+      sb.n[i] = (int64_t)eb.it[i].d * eb.it[i].d;
+      sb.first_block[i] = scan_blocks;
+      scan_blocks += (int)std::min<int64_t>(ceil_div(sb.n[i], 256 * 4 * 8), 1024);   // ~32 floats per thread
+    }
+    sb.first_block[eb.count] = scan_blocks;
+    window_scan_kernel<<<scan_blocks, 256, 0, s>>>(sb);
+    KFAC_LAUNCH_CHECK();
+    eb.dropped = dropped + base;
+    eb.skipped = skipped;
+    ema_kernel<true><<<blocks, 256, 0, s>>>(eb);
     KFAC_LAUNCH_CHECK();
   }
   return KFAC_OK;
+}
+
+extern "C" int kfac_factor_ema(const kfac_ema_item* items, int count, float alpha, void* stream) {
+  KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "items");
+  return launch_ema(items, count, alpha, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" size_t kfac_factor_ema_guarded_workspace_bytes(int count) {
+  return count > 0 ? align_up((size_t)count * sizeof(int), 256) : 0;
+}
+
+extern "C" int kfac_factor_ema_guarded(const kfac_ema_item* items, int count, float alpha,
+                                       const float* const* loss_scale, unsigned long long* skipped, void* ws,
+                                       size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "items");
+  if (count == 0) return KFAC_OK;
+  for (int i = 0; i < count; ++i)   // every item is checked before anything is launched
+    KFAC_CHECK_ARG(items[i].factor && items[i].batch && items[i].d > 0, "ema item");
+  const size_t need = kfac_factor_ema_guarded_workspace_bytes(count);
+  if (!ws || ws_bytes < need) {
+    set_error("factor_ema_guarded: workspace too small (%zu < %zu)", ws_bytes, need);
+    return KFAC_ERR_WORKSPACE;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  KFAC_CUDA(cudaMemsetAsync(ws, 0, (size_t)count * sizeof(int), s));
+  return launch_ema(items, count, alpha, loss_scale, (int*)ws, skipped, s);
 }
 
 extern "C" int kfac_dgda(const float* dg, const float* da, int g, int a, float damping, float* out,

@@ -215,9 +215,14 @@ class KFACLayer:
         self.module = module
         self.method = method
         self.prediv_eigenvalues = prediv_eigenvalues
-        if grad_scaler is not None and hasattr(grad_scaler, 'get_scale'):
+        # a torch.amp.GradScaler (torch.cuda.amp.GradScaler is a subclass) is kept as is: the G hook snapshots its
+        # scale on the device into `_g_scale_slot` (no host sync).  Other objects with get_scale() and plain callables
+        # are called on the host in every G hook.
+        if (grad_scaler is not None and not isinstance(grad_scaler, torch.amp.GradScaler)
+                and hasattr(grad_scaler, 'get_scale')):
             grad_scaler = grad_scaler.get_scale
         self.grad_scaler = grad_scaler
+        self._g_scale_slot = None               # device float: loss scale of the open G window (bound by the preconditioner)
         self.factor_dtype = factor_dtype
         self.inv_dtype = inv_dtype
         self.symmetry_aware = symmetry_aware
@@ -240,6 +245,11 @@ class KFACLayer:
 
     def __repr__(self) -> str:
         return f'{self.__class__.__name__}({repr(self.module)})'
+
+    @property
+    def device_grad_scaler(self) -> bool:
+        """True when the loss scale is read on the device (a torch.amp.GradScaler)."""
+        return isinstance(self.grad_scaler, torch.amp.GradScaler)
 
     # -------- reference-compatible read accessors (views into the arenas)
     def _as_factor_dtype(self, t):
