@@ -224,6 +224,75 @@ int kfac_grad_scale(const kfac_grad_item* items, int count, float kl_clip,
 int kfac_grad_update(const kfac_grad_item* items, int count, const float* scale,
                      void* ws, size_t ws_bytes, void* stream);
 
+/* ----------------------------------------------------------------- EKFAC
+ * Eigenvalue-corrected K-FAC (George et al., 2018): the Kronecker product dg x da of the
+ * eigenvalues is replaced by second moments S measured in the eigenbasis,
+ *   S_batch = (1/N) sum_r (Qg^T g_r)^2 (Qa^T x_r)^2^T          (g x a, element-wise squares),
+ * and the eigen precondition runs with dgda = 1 / (S + damping).
+ *
+ * Row writers: the rows x_r / g_r of one layer, SAMPLE-major fp32 (N x ld_out, ld_out a multiple
+ * of 4 and >= d; columns [d, ld_out) are written as 0).  Every value is multiplied by
+ * scale / *loss_scale (loss_scale: optional DEVICE float, the AMP loss scale; NULL = 1).
+ * The feature order is that of the factor calls above.  No workspace. */
+int kfac_rows_linear(const void* x, int dtype, int64_t rows, int features, int append_ones,
+                     float scale, const float* loss_scale, float* out, int ld_out, void* stream);
+int kfac_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W, int kh,
+                           int kw, int sh, int sw, int ph, int pw, int append_ones, float scale,
+                           float* out, int ld_out, void* stream);
+/* g (batch, C, Ho, Wo) -> rows (batch*Ho*Wo, C) */
+int kfac_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo,
+                             float scale, const float* loss_scale, float* out, int ld_out,
+                             void* stream);
+
+/* S_batch of every item, for all items together; no floating-point atomics, the same bits on
+ * every run.  Launches: one grouped wgmma launch of the projections (x^2 epilogue), the K = N
+ * product as one grouped launch, and the fixed-order sum of its split partials.  Extra launches:
+ *   - a projection with K = a or g > 1024 is accumulated in place over chunks of <= 512 columns,
+ *     one grouped launch per chunk round (up to 16 at K = 8192), then one squaring launch;
+ *   - the grouped engine runs each problem that is too small or narrow for the tensor cores
+ *     (M or N < 64) as its own SIMT launch: the projections of a layer with a or g < 64 (or with
+ *     fewer than 64 rows), and its S_batch product (g or a < 64) once per 4096 rows, followed by
+ *     one summing launch per such layer. */
+typedef struct kfac_ekfac_stat_item {
+  const float* X;   /* N x ldx: rows x_r (kfac_rows_*) */
+  const float* G;   /* N x ldg: rows g_r */
+  const float* qaT; /* a x a (ld = ldqa): rows are the eigenvectors of A (kfac_eigh_item.QT) */
+  const float* qgT; /* g x g (ld = ldqg) */
+  float* S_batch;   /* out: g x a (ld = lds); the padding columns [a, lds) are unspecified */
+  int64_t N;        /* rows, < 2^31 */
+  int a, g;
+  int ldx, ldg, ldqa, ldqg, lds;   /* ldx, ldg, lds multiples of 4 */
+} kfac_ekfac_stat_item;
+size_t kfac_ekfac_statistics_workspace_bytes(const kfac_ekfac_stat_item* items, int count);
+int kfac_ekfac_statistics(const kfac_ekfac_stat_item* items, int count, void* ws,
+                          size_t ws_bytes, void* stream);
+
+/* Schedule of S, one mode per call, then dgda = 1 / (S + damping) (padding columns 0):
+ *   KEEP  S unchanged (the per-step damping refresh)
+ *   EMA   S = alpha*S + (1-alpha)*S_batch
+ *   RESET S = S_batch                     (a window measured in a new basis)
+ *   SEED  S = dg x da                     (a new basis without a window: the K-FAC eigen method)
+ * EMA and RESET drop the window of an item whose S_batch holds an entry that is not finite or
+ * exceeds 1e15 in magnitude, or whose drop_a / drop_g flag (the drop flags kfac_factor_ema_guarded
+ * leaves in its workspace) is set: EMA then keeps S, RESET falls back to SEED.  A window dropped
+ * for its S_batch alone (neither flag set) increments *skipped (device counter, may be NULL); the
+ * guarded EMA has counted the others.  One launch (two with the scan of S_batch in EMA / RESET). */
+enum kfac_ekfac_mode { KFAC_EKFAC_KEEP = 0, KFAC_EKFAC_EMA = 1, KFAC_EKFAC_RESET = 2, KFAC_EKFAC_SEED = 3 };
+typedef struct kfac_ekfac_update_item {
+  float* S;             /* g x a running second moments (ld) */
+  const float* S_batch; /* g x a (ld); EMA / RESET only */
+  const float* dg;      /* eigenvalues of G (g) and A (a); SEED / RESET only */
+  const float* da;
+  float* dgda;          /* out: g x a (ld) */
+  int g, a, ld;
+  const int* drop_a;    /* optional DEVICE flags: non-zero drops the window */
+  const int* drop_g;
+} kfac_ekfac_update_item;
+size_t kfac_ekfac_update_workspace_bytes(int count);
+int kfac_ekfac_update(const kfac_ekfac_update_item* items, int count, float alpha, int mode,
+                      float damping, unsigned long long* skipped, void* ws, size_t ws_bytes,
+                      void* stream);
+
 /* ---------------------------------------------------------- peer memory
  * Buffers that other ranks of the node write into directly (CUDA IPC over NVLink).
  * kfac_peer_alloc: cudaMalloc + zero + export a 64-byte IPC handle (caller-owned: free with

@@ -19,6 +19,7 @@ c_void_p, c_int, c_float, c_size_t, c_int64 = C.c_void_p, C.c_int, C.c_float, C.
 KFAC_OK, KFAC_ERR_BAD_ARG, KFAC_ERR_NOT_READY, KFAC_ERR_CUDA = 0, -1, -2, -3
 KFAC_ERR_WORKSPACE, KFAC_ERR_NO_CONVERGE, KFAC_ERR_UNSUPPORTED = -4, -5, -6
 KFAC_EIGEN, KFAC_INVERSE = 1, 2
+KFAC_EKFAC_KEEP, KFAC_EKFAC_EMA, KFAC_EKFAC_RESET, KFAC_EKFAC_SEED = 0, 1, 2, 3
 
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
@@ -48,6 +49,17 @@ class GradItem(C.Structure):
                 ('grad_dtype', c_int), ('g', c_int), ('a', c_int), ('ldp', c_int)]
 
 
+class EkfacStatItem(C.Structure):
+    _fields_ = [('X', c_void_p), ('G', c_void_p), ('qaT', c_void_p), ('qgT', c_void_p), ('S_batch', c_void_p),
+                ('N', c_int64), ('a', c_int), ('g', c_int),
+                ('ldx', c_int), ('ldg', c_int), ('ldqa', c_int), ('ldqg', c_int), ('lds', c_int)]
+
+
+class EkfacUpdateItem(C.Structure):
+    _fields_ = [('S', c_void_p), ('S_batch', c_void_p), ('dg', c_void_p), ('da', c_void_p), ('dgda', c_void_p),
+                ('g', c_int), ('a', c_int), ('ld', c_int), ('drop_a', c_void_p), ('drop_g', c_void_p)]
+
+
 # name -> (restype, argtypes); must list EVERY symbol of include/kfac_b200.h
 SIGNATURES = {
     'kfac_version': (c_int, []),
@@ -75,6 +87,15 @@ SIGNATURES = {
     'kfac_grad_workspace_bytes': (c_size_t, [c_int]),
     'kfac_grad_scale': (c_int, [C.POINTER(GradItem), c_int, c_float, c_float, c_void_p, c_size_t, c_void_p, c_void_p]),
     'kfac_grad_update': (c_int, [C.POINTER(GradItem), c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'kfac_rows_linear': (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p]),
+    'kfac_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
+    'kfac_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
+                                         c_void_p]),
+    'kfac_ekfac_statistics_workspace_bytes': (c_size_t, [C.POINTER(EkfacStatItem), c_int]),
+    'kfac_ekfac_statistics': (c_int, [C.POINTER(EkfacStatItem), c_int, c_void_p, c_size_t, c_void_p]),
+    'kfac_ekfac_update_workspace_bytes': (c_size_t, [c_int]),
+    'kfac_ekfac_update': (c_int, [C.POINTER(EkfacUpdateItem), c_int, c_float, c_int, c_float, c_void_p, c_void_p,
+                                  c_size_t, c_void_p]),
     'kfac_peer_alloc': (c_int, [c_size_t, C.POINTER(c_void_p), c_void_p]),
     'kfac_peer_open': (c_int, [c_void_p, C.POINTER(c_void_p)]),
     'kfac_peer_close': (c_int, [c_void_p]),

@@ -34,6 +34,16 @@ across step() (step() called before `accumulation_steps` micro-batches have
 run) can span an update() and so two scales; the last snapshot is applied to
 the whole window.  Under data parallelism every rank must use the same scale,
 as GradScaler does when it unscales gradients that DDP has already averaged.
+
+EKFAC (`compute_method='ekfac'`): the hooks also keep the rows of the window
+(sample-major fp32 row buffers, one forward and one backward per window), and
+step() measures their second moments S_batch in the eigenbasis, after the
+factor EMA and after the eigendecompositions of an inverse step:
+    factor step, no new basis     S <- factor_decay * S + (1 - factor_decay) * S_batch
+    factor step, new basis        S <- S_batch
+    new basis without a window    S <- dg x da       (also after load_state_dict)
+    every step                    dgda <- 1 / (S + damping)
+and the eigen precondition runs with that dgda.  S is not part of state_dict().
 """
 from __future__ import annotations
 
@@ -134,6 +144,13 @@ def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignm
                 sa.add(layer, 'da', (a,))
                 sg.add(layer, 'qg', (g, g))
                 sg.add(layer, 'dg', (g,))
+        elif layer.method == ComputeMethod.EKFAC:
+            # eigenvalues too: every rank seeds S with dg x da for a basis no window has been measured in
+            sa, sg = seg(src_a), seg(src_g)
+            sa.add(layer, 'qa', (a, a))
+            sa.add(layer, 'da', (a,))
+            sg.add(layer, 'qg', (g, g))
+            sg.add(layer, 'dg', (g,))
         else:
             seg(src_a).add(layer, 'a_inv', (a, a))
             seg(src_g).add(layer, 'g_inv', (g, g))
@@ -233,6 +250,7 @@ class BaseKFACPreconditioner:
         self._guard_factors = any(l.grad_scaler is not None for _, l in self._layers.values())
         self._ema_scratch = _Scratch()        # drop flags of the guarded EMA
         self._skipped: torch.Tensor | None = None   # device counter of dropped windows
+        self._ekfac_scratch = _Scratch()      # EKFAC projections + split partials, and the update's item table
         # C1: the batch statistics (not the factors) are averaged over the ranks BEFORE the EMA -- the same factors by
         # linearity -- so that the A block can be reduced while backward still runs (base_preconditioner.py:452-457)
         self.overlap_factor_allreduce = True
@@ -285,8 +303,9 @@ class BaseKFACPreconditioner:
 
     @property
     def skipped_factor_updates(self) -> int:
-        """Number of factor windows the guarded EMA has dropped because their statistics were not finite (or
-        exceeded 1e15 in magnitude).  Only counted with a `grad_scaler`; reading it synchronises the device."""
+        """Number of factor windows dropped because their statistics were not finite (or exceeded 1e15 in
+        magnitude): by the guarded EMA, only with a `grad_scaler`; with EKFAC also the windows whose factors were kept
+        but whose S_batch was dropped (with or without a `grad_scaler`).  Reading it synchronises the device."""
         return int(self._skipped.item()) if self._skipped is not None else 0
 
     # ------------------------------------------------------------ arenas
@@ -356,6 +375,9 @@ class BaseKFACPreconditioner:
                         plan.append((l, '_da', (l.a_dim,)))
                     if mine_g:
                         plan.append((l, '_dg', (l.g_dim,)))
+            elif l.method == ComputeMethod.EKFAC:
+                # every rank forms its own dgda from S (never communicated)
+                plan += [(l, '_qaT', (l.a_dim, l.a_dim)), (l, '_qgT', (l.g_dim, l.g_dim)), (l, 'dgda', (l.g_dim, l.a_dim))]
             else:
                 if mine_a:
                     plan += [(l, '_qa', (l.a_dim, l.a_dim)), (l, '_da', (l.a_dim,))]
@@ -369,8 +391,19 @@ class BaseKFACPreconditioner:
             l._inv[key] = _bind(self._local_arena, off, shape)
             l._inv_cols[key] = shape[-1]
             off += _storage_numel(shape)
-        if self._guard_factors:
+        ek = [l for _, l in ll if l.method == ComputeMethod.EKFAC]
+        if ek:
+            total = sum(l.g_dim * _cabi.ld4(l.a_dim) for l in ek)
+            self._s_arena = torch.zeros(total, dtype=torch.float32, device=device)
+            self._s_batch_arena = torch.zeros(total, dtype=torch.float32, device=device)
+            off = 0
+            for l in ek:
+                l._S = _bind(self._s_arena, off, (l.g_dim, l.a_dim))
+                l._S_batch = _bind(self._s_batch_arena, off, (l.g_dim, l.a_dim))
+                off += _storage_numel((l.g_dim, l.a_dim))
+        if self._guard_factors or ek:
             self._skipped = torch.zeros(1, dtype=torch.int64, device=device)
+        if self._guard_factors:
             self._g_scales = torch.ones(len(ll), dtype=torch.float32, device=device)
             for i, (_, l) in enumerate(ll):
                 l._g_scale_slot = self._g_scales.narrow(0, i, 1)
@@ -501,6 +534,11 @@ class BaseKFACPreconditioner:
             compute_inverses = False
         if compute_inverses:
             self._compute_inverses()
+            # S <- dg x da: no window has been measured in these bases; rows kept before the load are discarded
+            for _, layer in self._layers.values():
+                if layer.method == ComputeMethod.EKFAC:
+                    layer._rows_n_a = layer._rows_n_g = 0
+            self._ekfac_update(new_basis=True)
 
     # ------------------------------------------------------------ hooks
     def _grad_scale_value(self, layer: KFACLayer) -> float:
@@ -529,6 +567,9 @@ class BaseKFACPreconditioner:
         name, layer = self._layers[module]
         x = input_[0]
         self._ensure_arenas(x.device)
+        if layer.method == ComputeMethod.EKFAC and layer._rows_n_a:
+            raise RuntimeError(f'EKFAC: {name} was called a second time in one factor window (one forward and one '
+                               'backward pass per layer between step() calls; weight-shared modules are not supported)')
         if layer._a_pending:       # a completed accumulation window is still queued
             self._flush_factor_updates()
         if self._a_reduce_work is not None:
@@ -537,7 +578,13 @@ class BaseKFACPreconditioner:
             self._a_reduce_work.wait()
             self._a_reduce_work = None
             self._a_block_reduced = False
-        layer.module.accumulate_a(cast_for_factor(x, layer.factor_dtype), layer._a_batch_view, self._scratch)
+        x = cast_for_factor(x, layer.factor_dtype)
+        layer.module.accumulate_a(x, layer._a_batch_view, self._scratch)
+        if layer.method == ComputeMethod.EKFAC:
+            n = layer.module.num_rows_a(x)
+            layer._rows_x = self._row_buffer(layer._rows_x, n * _cabi.ld4(layer.a_dim))
+            layer.module.write_rows_a(x, layer._rows_x)
+            layer._rows_n_a = n
         layer._a_count += 1
         self._mini_steps[name] += 1
         if self._update_factors_in_hook and self._mini_steps[name] % self._accumulation_steps == 0:
@@ -553,6 +600,9 @@ class BaseKFACPreconditioner:
         name, layer = self._layers[module]
         g = grad_output if isinstance(grad_output, torch.Tensor) else grad_output[0]
         self._ensure_arenas(g.device)
+        if layer.method == ComputeMethod.EKFAC and layer._rows_n_g:
+            raise RuntimeError(f'EKFAC: {name} was called a second time in one factor window (one forward and one '
+                               'backward pass per layer between step() calls; weight-shared modules are not supported)')
         if layer._g_pending:
             self._flush_factor_updates()
         if self._update_factors_in_hook and self._mini_steps[name] % self._accumulation_steps == 0:
@@ -560,11 +610,24 @@ class BaseKFACPreconditioner:
         if layer.device_grad_scaler:
             self._snapshot_loss_scale(layer)
         # the backward hook runs on the autograd thread: it gets its own scratch buffer
-        layer.module.accumulate_g(cast_for_factor(g, layer.factor_dtype), layer._g_batch_view,
-                                  self._grad_scale_value(layer), self._scratch_bwd)
+        g = cast_for_factor(g, layer.factor_dtype)
+        grad_scale = self._grad_scale_value(layer)
+        layer.module.accumulate_g(g, layer._g_batch_view, grad_scale, self._scratch_bwd)
+        if layer.method == ComputeMethod.EKFAC:
+            n = layer.module.num_rows_g(g)
+            layer._rows_g = self._row_buffer(layer._rows_g, n * _cabi.ld4(layer.g_dim))
+            layer.module.write_rows_g(g, layer._rows_g, grad_scale,
+                                      layer._g_scale_slot.data_ptr() if layer.device_grad_scaler else None)
+            layer._rows_n_g = n
         layer._g_count += 1
         if self._update_factors_in_hook and self._mini_steps[name] % self._accumulation_steps == 0:
             self._mark_pending(layer, 'g')
+
+    def _row_buffer(self, buf: torch.Tensor | None, numel: int) -> torch.Tensor:
+        """Grow-only fp32 row buffer of one layer and side (EKFAC)."""
+        if buf is None or buf.numel() < numel:
+            buf = torch.empty(numel, dtype=torch.float32, device=self._device)
+        return buf
 
     def _mark_pending(self, layer: KFACLayer, which: str) -> None:
         """Queue the EMA update of one factor (layers/base.py:375-405); it is
@@ -644,6 +707,12 @@ class BaseKFACPreconditioner:
         self._reduce_batches()
         lib = _cabi.load()
         stream = _cabi.stream_ptr()
+        flags = None
+        if self._guard_factors:
+            # one drop-flag region per call, kept until step() has read the flags of its EKFAC layers
+            sizes = [lib.kfac_factor_ema_guarded_workspace_bytes(len(todo)) for todo in self._pending_alpha.values()]
+            flags = self._ema_scratch.get(sum(sizes), self._device)
+            flag_off = 0
         for alpha, todo in self._pending_alpha.items():
             items = (_cabi.EmaItem * len(todo))()
             scales = (C.c_void_p * len(todo))()      # guarded EMA: loss-scale slot of a G item, NULL otherwise
@@ -663,9 +732,12 @@ class BaseKFACPreconditioner:
                 continue
             # decided after C1, so every rank drops the same windows
             need = lib.kfac_factor_ema_guarded_workspace_bytes(len(todo))
-            ws = self._ema_scratch.get(need, self._device)
+            ws = flags.data_ptr() + flag_off
+            flag_off += need
             _cabi.check(lib.kfac_factor_ema_guarded(items, len(todo), alpha, scales, self._skipped.data_ptr(),
-                                                    ws.data_ptr(), need, stream), 'kfac_factor_ema_guarded')
+                                                    ws, need, stream), 'kfac_factor_ema_guarded')
+            for i, (layer, which) in enumerate(todo):
+                setattr(layer, '_drop_' + which, ws + 4 * i)
         self._pending_alpha = {}
 
     # ------------------------------------------------------------ step
@@ -684,8 +756,10 @@ class BaseKFACPreconditioner:
                 self._mark_pending(layer, 'g')
         self._flush_factor_updates()      # C1 (average of the batch statistics) + EMA
 
-        if self.steps % self.inv_update_steps == 0:
+        new_basis = self.steps % self.inv_update_steps == 0
+        if new_basis:
             self._compute_inverses()
+        self._ekfac_update(new_basis)
 
         self._precondition()
         self._scale_and_write_back()
@@ -738,6 +812,11 @@ class BaseKFACPreconditioner:
                         eig.append((layer._a_view, I['qa'], I['_qaT'], I['da'], layer.a_dim))
                     if mine_g:
                         eig.append((layer._g_view, I['qg'], I['_qgT'], I['dg'], layer.g_dim))
+            elif layer.method == ComputeMethod.EKFAC:
+                if mine_a:
+                    eig.append((layer._a_view, I['qa'], I['_qaT'], I['da'], layer.a_dim))
+                if mine_g:
+                    eig.append((layer._g_view, I['qg'], I['_qgT'], I['dg'], layer.g_dim))
             else:
                 if mine_a:
                     eig.append((layer._a_view, I['_qa'], None, I['_da'], layer.a_dim))
@@ -794,6 +873,57 @@ class BaseKFACPreconditioner:
                                                    layer._inv['_' + key + 'T'].data_ptr(), ld, n, n, stream),
                                 'kfac_transpose')
 
+    # EKFAC ----------------------------------------------------------------
+    def _ekfac_update(self, new_basis: bool) -> None:
+        """S and dgda of every EKFAC layer (the schedule of the module docstring).  A layer takes part once its bases
+        and eigenvalues are available; its window (the rows of this step's forward and backward) is consumed."""
+        ek = [l for _, l in reversed(self._layer_list()) if l.method == ComputeMethod.EKFAC]
+        if not ek:
+            return
+        lib = _cabi.load()
+        stream = _cabi.stream_ptr()
+        ready = [l for l in ek if {'qa', 'qg', 'da', 'dg'} <= l._inv_ready]
+        windows = [l for l in ready if l._rows_n_a and l._rows_n_g]
+        for l in windows:
+            if l._rows_n_a != l._rows_n_g:
+                raise RuntimeError(f'EKFAC: {l._rows_n_a} rows on the A side and {l._rows_n_g} on the G side')
+        if windows:
+            items = (_cabi.EkfacStatItem * len(windows))()
+            for i, l in enumerate(windows):
+                a, g = l.a_dim, l.g_dim
+                items[i] = _cabi.EkfacStatItem(l._rows_x.data_ptr(), l._rows_g.data_ptr(), l._inv['_qaT'].data_ptr(),
+                                               l._inv['_qgT'].data_ptr(), l._S_batch.data_ptr(), l._rows_n_a, a, g,
+                                               _cabi.ld4(a), _cabi.ld4(g), _cabi.ld4(a), _cabi.ld4(g), _cabi.ld4(a))
+            need = lib.kfac_ekfac_statistics_workspace_bytes(items, len(windows))
+            ws = self._ekfac_scratch.get(need, self._device)
+            _cabi.check(lib.kfac_ekfac_statistics(items, len(windows), ws.data_ptr(), need, stream),
+                        'kfac_ekfac_statistics')
+            # C1 for S_batch: one average over the world (linear in the rows, like the factors)
+            self._tdc.allreduce_average(self._s_batch_arena, group=None)
+        in_window = set(map(id, windows))
+        rest = [l for l in ready if id(l) not in in_window]
+        damping = float(self.damping)
+        alpha = float(self.factor_decay)
+        for todo, mode in ((windows, _cabi.KFAC_EKFAC_RESET if new_basis else _cabi.KFAC_EKFAC_EMA),
+                           (rest, _cabi.KFAC_EKFAC_SEED if new_basis else _cabi.KFAC_EKFAC_KEEP)):
+            if not todo:
+                continue
+            items = (_cabi.EkfacUpdateItem * len(todo))()
+            for i, l in enumerate(todo):
+                I = l._inv
+                items[i] = _cabi.EkfacUpdateItem(l._S.data_ptr(), l._S_batch.data_ptr(), I['dg'].data_ptr(),
+                                                 I['da'].data_ptr(), I['dgda'].data_ptr(), l.g_dim, l.a_dim,
+                                                 _cabi.ld4(l.a_dim), l._drop_a, l._drop_g)
+            need = lib.kfac_ekfac_update_workspace_bytes(len(todo))
+            ws = self._ekfac_scratch.get(need, self._device)
+            _cabi.check(lib.kfac_ekfac_update(items, len(todo), alpha, mode, damping, self._skipped.data_ptr(),
+                                              ws.data_ptr(), need, stream), 'kfac_ekfac_update')
+            for l in todo:
+                l._inv_ready.add('dgda')
+        for l in ek:
+            l._rows_n_a = l._rows_n_g = 0
+            l._drop_a = l._drop_g = None
+
     # K8/K9/K10 + C3 -------------------------------------------------------
     def _grad_ptrs(self, layer: KFACLayer):
         m = layer.module
@@ -821,6 +951,11 @@ class BaseKFACPreconditioner:
                 ok = ('qa' in ready and 'qg' in ready and
                       ('dgda' in ready if layer.prediv_eigenvalues else ('da' in ready and 'dg' in ready)))
                 if not ok:
+                    raise RuntimeError('Eigendecompositions for both A and G have not been computed')
+                eigen = True
+            elif layer.method == ComputeMethod.EKFAC:
+                # the eigen precondition with dgda = 1 / (S + damping)
+                if not ('qa' in ready and 'qg' in ready and 'dgda' in ready):
                     raise RuntimeError('Eigendecompositions for both A and G have not been computed')
                 eigen = True
             else:
@@ -908,6 +1043,8 @@ class BaseKFACPreconditioner:
         for _, layer in self._layers.values():
             for key, size in layer.memory_usage().items():
                 sizes[key] += size
+        if 'ekfac' in sizes and self._ekfac_scratch.buf is not None:
+            sizes['ekfac'] += self._ekfac_scratch.buf.numel()   # squared projections + split partials of S_batch
         sizes['total'] = sum(sizes.values())
         return sizes
 

@@ -70,7 +70,7 @@ __device__ __forceinline__ void store_from_float(void* p, int dtype, int64_t i, 
 }
 
 // ---------------------------------------------------------------- SIMT GEMM
-enum GemmEpilogue { EPI_NONE = 0, EPI_MUL = 1, EPI_DIV_OUTER = 2 };
+enum GemmEpilogue { EPI_NONE = 0, EPI_MUL = 1, EPI_DIV_OUTER = 2, EPI_SQUARE = 3 };   // EPI_SQUARE: store x^2
 
 struct GemmArgs {
   const float* A; int64_t sa_m, sa_k, sa_b;   // A(m,k) = A[b*sa_b + m*sa_m + k*sa_k]

@@ -78,6 +78,7 @@ struct GroupedPolicy {
       if (nb + j < p.N) {
         if (p.epi == EPI_MUL) x *= p.E[(int64_t)m * p.lde + nb + j];
         else if (p.epi == EPI_DIV_OUTER) x = x / (p.dg[m] * p.da[nb + j] + p.damping);
+        else if (p.epi == EPI_SQUARE) x = x * x;
       }
       v[j] = x;
     }

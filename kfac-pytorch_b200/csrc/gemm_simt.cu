@@ -73,6 +73,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
       float v = g.alpha * acc[i][j];
       if (g.epi == EPI_MUL) v *= g.E[(int64_t)m * g.lde + n];
       else if (g.epi == EPI_DIV_OUTER) v = v / (g.dg[m] * g.da[n] + g.damping);
+      else if (g.epi == EPI_SQUARE) v = v * v;
       float* c = &C[(int64_t)m * g.ldc + n];
       if (g.atomic) atomicAdd(c, v);
       else *c = (g.beta == 0.f) ? v : (v + g.beta * (*c));

@@ -17,9 +17,12 @@ class AssignmentStrategy(Enum):
 
 
 class ComputeMethod(Enum):
-    """EIGEN: (G (x) A + damping I)^-1 ;  INVERSE: (G+damping I)^-1 (x) (A+damping I)^-1."""
+    """EIGEN: (G (x) A + damping I)^-1 ;  INVERSE: (G+damping I)^-1 (x) (A+damping I)^-1 ;
+    EKFAC: the eigenbases of EIGEN with second moments S measured in them in place of dg (x) da
+    (George et al., 2018; an extension beyond the reference)."""
     EIGEN = 1
     INVERSE = 2
+    EKFAC = 3
 
 
 class DistributedStrategy(Enum):

@@ -65,6 +65,21 @@ class ModuleHelper:
     def accumulate_g(self, g: torch.Tensor, acc: torch.Tensor, grad_scale: float, scratch=None) -> None:
         raise NotImplementedError
 
+    # EKFAC row writers: the rows x_r / g_r of one micro-batch (exactly the rows the A / G statistics are formed of),
+    # written sample-major in fp32 into `out`, a buffer of at least num_rows_{a,g} x ld4(d) floats
+    def num_rows_a(self, x: torch.Tensor) -> int:
+        raise NotImplementedError
+
+    def num_rows_g(self, g: torch.Tensor) -> int:
+        raise NotImplementedError
+
+    def write_rows_a(self, x: torch.Tensor, out: torch.Tensor) -> None:
+        raise NotImplementedError
+
+    def write_rows_g(self, g: torch.Tensor, out: torch.Tensor, grad_scale: float, loss_scale: int | None) -> None:
+        """loss_scale: device pointer of a float the rows are divided by (the AMP loss scale), or None."""
+        raise NotImplementedError
+
 
 _NATIVE_INPUT_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
 
@@ -131,6 +146,26 @@ class LinearModuleHelper(ModuleHelper):
                                            ws.data_ptr() if ws is not None else None, need,
                                            _cabi.stream_ptr()), 'kfac_factor_linear')
 
+    def num_rows_a(self, x):
+        return x.numel() // x.size(-1)
+
+    num_rows_g = num_rows_a
+
+    def _write_rows(self, t, out, ones, scale, loss_scale):
+        _cabi.require_device(t)
+        t = t.detach()
+        t = t if t.is_contiguous() else t.contiguous()
+        feat = t.size(-1)
+        _cabi.check(_cabi.load().kfac_rows_linear(t.data_ptr(), _dtype_code(t), t.numel() // feat, feat, ones, scale,
+                                                  loss_scale, out.data_ptr(), _cabi.ld4(feat + ones),
+                                                  _cabi.stream_ptr()), 'kfac_rows_linear')
+
+    def write_rows_a(self, x, out):
+        self._write_rows(x, out, int(self.has_bias()), 1.0, None)
+
+    def write_rows_g(self, g, out, grad_scale, loss_scale):
+        self._write_rows(g, out, 0, 1.0 / grad_scale, loss_scale)
+
 
 class Conv2dModuleHelper(ModuleHelper):
     """torch.nn.Conv2d (modules.py:144-237).  Like the reference, dilation and
@@ -189,6 +224,36 @@ class Conv2dModuleHelper(ModuleHelper):
                                                    _cabi.stream_ptr()),
                     'kfac_factor_conv2d_gradout')
 
+    def num_rows_a(self, x):
+        B, _, H, W, kh, kw, sh, sw, ph, pw = self._geometry(x)
+        return B * ((H + 2 * ph - kh) // sh + 1) * ((W + 2 * pw - kw) // sw + 1)
+
+    def num_rows_g(self, g):
+        return g.size(0) * g.size(2) * g.size(3)
+
+    def write_rows_a(self, x, out):
+        _cabi.require_device(x)
+        x = x.detach()
+        x = x if x.is_contiguous() else x.contiguous()
+        geo = self._geometry(x)
+        B, Cc, H, W, kh, kw, sh, sw, ph, pw = geo
+        S = ((H + 2 * ph - kh) // sh + 1) * ((W + 2 * pw - kw) // sw + 1)
+        ones = int(self.has_bias())
+        # rows scaled by 1/S, the ones column included (modules.py:170-178)
+        _cabi.check(_cabi.load().kfac_rows_conv2d_input(x.data_ptr(), _dtype_code(x), *geo, ones, 1.0 / S, out.data_ptr(),
+                                                        _cabi.ld4(Cc * kh * kw + ones), _cabi.stream_ptr()),
+                    'kfac_rows_conv2d_input')
+
+    def write_rows_g(self, g, out, grad_scale, loss_scale):
+        _cabi.require_device(g)
+        g = g.detach()
+        g = g if g.is_contiguous() else g.contiguous()
+        B, Cc, Ho, Wo = g.shape
+        _cabi.check(_cabi.load().kfac_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, Ho, Wo,
+                                                          1.0 / (float(Ho * Wo) * grad_scale), loss_scale,
+                                                          out.data_ptr(), _cabi.ld4(Cc), _cabi.stream_ptr()),
+                    'kfac_rows_conv2d_gradout')
+
 
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
 CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
@@ -242,6 +307,12 @@ class KFACLayer:
         self._inv_ready = set()
         self._p_view = None
         self._grad_ready = False
+        # EKFAC (bound by the preconditioner): S and S_batch (g x ld4(a) arena views), grow-only row buffers, the
+        # rows written in the open factor window, and the guarded EMA's drop flags of that window (device pointers)
+        self._S = self._S_batch = None
+        self._rows_x = self._rows_g = None
+        self._rows_n_a = self._rows_n_g = 0
+        self._drop_a = self._drop_g = None
 
     def __repr__(self) -> str:
         return f'{self.__class__.__name__}({repr(self.module)})'
@@ -312,6 +383,9 @@ class KFACLayer:
         for k in self._inv_ready:
             bucket = 'a_inverses' if k in ('qa', 'da', 'a_inv') else 'g_inverses'
             out[bucket] += self._inv[k].numel() * b
+        if self._S is not None:
+            out['ekfac'] = sum(t.numel() * b for t in (self._S, self._S_batch, self._rows_x, self._rows_g)
+                               if t is not None)
         return out
 
     def reset_batch(self) -> None:
@@ -320,6 +394,8 @@ class KFACLayer:
             self._g_batch_view.zero_()
         self._a_count = self._g_count = 0
         self._a_pending = self._g_pending = False
+        self._rows_n_a = self._rows_n_g = 0
+        self._drop_a = self._drop_g = None
 
 
 def any_match(query: str, patterns: list[str]) -> bool:

@@ -32,7 +32,14 @@ def _mock_new_group(x: list[int]) -> None:
 
 
 class KFACPreconditioner(BaseKFACPreconditioner):
-    """K-FAC gradient preconditioner with KAISA placement on H100 (sm_90a)."""
+    """K-FAC gradient preconditioner with KAISA placement on H100 (sm_90a).
+
+    `compute_method` takes EIGEN and INVERSE like the reference, and EKFAC: the eigen method with the
+    Kronecker product of the eigenvalues replaced by second moments measured in the eigenbasis at every
+    factor step (George et al., 2018).  EKFAC needs `grad_worker_fraction` to resolve to COMM_OPT,
+    `accumulation_steps=1` and, for integer schedules, `inv_update_steps` a multiple of
+    `factor_update_steps`; `compute_eigenvalue_outer_product` is ignored with it.
+    """
 
     def __init__(
         self,
@@ -105,6 +112,16 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             else:
                 distributed_strategy = DistributedStrategy.HYBRID_OPT
         assert isinstance(grad_worker_fraction, float)
+
+        if compute_method == ComputeMethod.EKFAC:
+            if distributed_strategy != DistributedStrategy.COMM_OPT:
+                raise ValueError('compute_method=EKFAC needs grad_worker_fraction to resolve to COMM_OPT '
+                                 '(every rank holds the eigenbases and measures its rows in them)')
+            if accumulation_steps != 1:
+                raise ValueError('compute_method=EKFAC needs accumulation_steps=1')
+            if (not callable(inv_update_steps) and not callable(factor_update_steps) and factor_update_steps > 0
+                    and inv_update_steps % factor_update_steps != 0):
+                raise ValueError('compute_method=EKFAC needs inv_update_steps to be a multiple of factor_update_steps')
 
         if not colocate_factors and distributed_strategy is DistributedStrategy.MEM_OPT:
             warnings.warn('grad_worker_frac=1/world_size (MEM_OPT) requires '
