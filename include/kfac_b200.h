@@ -117,6 +117,26 @@ int kfac_factor_ema_guarded(const kfac_ema_item* items, int count, float alpha,
                             const float* const* loss_scale, unsigned long long* skipped,
                             void* ws, size_t ws_bytes, void* stream);
 
+/* Embedding layers (an extension beyond the reference, opt-in): an nn.Embedding is a Linear
+ * layer whose input rows are one-hot vectors e_idx, so its A factor is DIAGONAL, the token
+ * frequencies.  It is kept as a vector of V floats and never eigendecomposed.
+ * kfac_factor_embedding: acc[v] += alpha * count(idx == v) over the N indices (alpha = 1/N).
+ * idx: N int32 (index_dtype KFAC_I32) or int64 (KFAC_I64) indices in [0, V); they are trusted
+ * (the embedding's forward pass has already checked them).  Deterministic and without a host
+ * sync: an integer histogram in ws (kfac_factor_embedding_workspace_bytes(V) bytes), then one
+ * fixed-order scale-and-add per entry.  No floating-point atomics. */
+enum kfac_index_dtype { KFAC_I32 = 3, KFAC_I64 = 4 };
+size_t kfac_factor_embedding_workspace_bytes(int V);
+int kfac_factor_embedding(const void* idx, int index_dtype, int64_t N, int V, float alpha,
+                          float* acc, void* ws, size_t ws_bytes, void* stream);
+/* EMA of diagonal factors (vectors of d = V floats), the schedule of kfac_factor_ema on the
+ * diagonal and with the same rounding (the bits kfac_factor_ema gives on diag(batch)):
+ *   factor = alpha*(first ? 1 : factor) + (1-alpha)*inv_count*batch;   batch = 0
+ * There is no guarded variant: a window of token counts is finite whatever the loss scale, so
+ * under a grad_scaler the A side of an embedding is never dropped, and its G side (a dense
+ * d x d factor) goes through kfac_factor_ema_guarded like every other G.  One launch per 40 items. */
+int kfac_factor_ema_diag(const kfac_ema_item* items, int count, float alpha, void* stream);
+
 /* ------------------------------------------------------- eigendecomposition
  * K5: replaces torch.linalg.eigh + clamp(min=0) in
  * KFACEigenLayer.compute_{a,g}_inv (kfac/layers/eigen.py:295-344).
@@ -170,7 +190,15 @@ int kfac_transpose(const float* src, int ld_src, float* dst, int ld_dst, int row
  * inverse.py:215-234).  grad matrix = [wgrad viewed (g, a-1|a), bgrad].
  *   EIGEN  : P = Qg [ (Qg^T grad Qa) * dgda ] Qa^T     (dgda != NULL)
  *            P = Qg [ (Qg^T grad Qa) / (dg x da + damping) ] Qa^T  (else)
- *   INVERSE: P = Ginv grad Ainv */
+ *   INVERSE: P = Ginv grad Ainv
+ * Embedding items (kind = KFAC_ITEM_EMBEDDING): wgrad is the (a = V, g = d) weight gradient,
+ * bgrad NULL, da the diagonal A factor (V floats; its own eigenvalues), and P (V x ldp, ldp >= d)
+ * is written in the weight's layout:
+ *   EIGEN  : P = [(wgrad Qg) / (da x dg + damping)] Qg^T     (qg, qgT, dg; dgda is not used)
+ *   INVERSE: P = diag(1 / (da + damping)) wgrad Ginv          (g_inv)
+ * qa, qaT, a_inv, dgda and ldqa are ignored.  The two (one) GEMMs join the grouped launches of
+ * the dense items; the other items' results do not depend on the embedding items. */
+enum kfac_item_kind { KFAC_ITEM_DENSE = 0, KFAC_ITEM_EMBEDDING = 1 };
 typedef struct kfac_precond_item {
   const void* wgrad; /* (g, a - has_bias) */
   const void* bgrad; /* (g) or NULL */
@@ -194,6 +222,7 @@ typedef struct kfac_precond_item {
    * to P and to all peers (P2P over NVLink).  n_peers = 0: local only. */
   float* const* peer_P;
   int n_peers;
+  int kind; /* kfac_item_kind; 0 (dense) for the positional initialisers written before it */
 } kfac_precond_item;
 size_t kfac_precondition_workspace_bytes(const kfac_precond_item* items, int count);
 int kfac_precondition(const kfac_precond_item* items, int count, int method,

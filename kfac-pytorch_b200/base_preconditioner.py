@@ -132,7 +132,16 @@ def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignm
                 inv[key] = _Segment(src, group)
             return inv[key]
 
-        if layer.method == ComputeMethod.EIGEN:
+        if layer.diag_a:
+            # embedding: the A snapshot (its own eigenvalues) and the data of G; never a V x d dgda
+            seg(src_a).add(layer, 'da', (a,))
+            sg = seg(src_g)
+            if layer.method == ComputeMethod.EIGEN:
+                sg.add(layer, 'qg', (g, g))
+                sg.add(layer, 'dg', (g,))
+            else:
+                sg.add(layer, 'g_inv', (g, g))
+        elif layer.method == ComputeMethod.EIGEN:
             if layer.prediv_eigenvalues:
                 s = seg(src_g)
                 s.add(layer, 'qa', (a, a))
@@ -159,7 +168,7 @@ def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignm
         src = assignment.src_grad_worker(name)
         if src not in grad:
             grad[src] = _Segment(src, assignment.grad_receiver_group(name))
-        grad[src].add(layer, 'P', (layer.g_dim, layer.a_dim))
+        grad[src].add(layer, 'P', layer.p_shape)
     inv_segments = list(inv.values())
     grad_segments = [grad[k] for k in sorted(grad)]
     for segs in (inv_segments, grad_segments):
@@ -262,9 +271,14 @@ class BaseKFACPreconditioner:
         self.fused_grad_broadcast = True
         self._eig_status: torch.Tensor | None = None     # pinned host int: status word of the last eigensolver call
 
-        for module in self._layers:
+        for module, (_, layer) in self._layers.items():
             module.register_forward_pre_hook(self._save_input)
-            module.register_full_backward_hook(self._save_grad_output)
+            if layer.diag_a:
+                # the input of an embedding (the indices) never requires grad: a full backward hook would fire through
+                # the output with a warning on every backward pass, so the output tensor is hooked directly
+                module.register_forward_hook(self._hook_output)
+            else:
+                module.register_full_backward_hook(self._save_grad_output)
 
     # ------------------------------------------------------------ properties
     def __repr__(self) -> str:
@@ -324,8 +338,8 @@ class BaseKFACPreconditioner:
         _cabi.load()
         self._device = device
         ll = self._layer_list()
-        # dense d x d factors, each starting 16-byte aligned
-        total = sum(_cabi.ld4(l.a_dim ** 2) + _cabi.ld4(l.g_dim ** 2) for _, l in ll)
+        # dense d x d factors (a vector of V floats for the diagonal A of an embedding), each starting 16-byte aligned
+        total = sum(_cabi.ld4(l.a_dim if l.diag_a else l.a_dim ** 2) + _cabi.ld4(l.g_dim ** 2) for _, l in ll)
         self._factor_arena = torch.zeros(total, dtype=torch.float32, device=device)
         self._batch_arena = torch.zeros(total, dtype=torch.float32, device=device)
         # layout: all A factors, then all G factors -- the A block is complete after the forward pass and is
@@ -334,9 +348,10 @@ class BaseKFACPreconditioner:
         for which in ('a', 'g'):
             for _, l in ll:
                 dim = l.a_dim if which == 'a' else l.g_dim
-                n = dim * dim
-                setattr(l, f'_{which}_view', self._factor_arena.narrow(0, off, n).view(dim, dim))
-                setattr(l, f'_{which}_batch_view', self._batch_arena.narrow(0, off, n).view(dim, dim))
+                shape = (dim,) if which == 'a' and l.diag_a else (dim, dim)
+                n = dim if len(shape) == 1 else dim * dim
+                setattr(l, f'_{which}_view', self._factor_arena.narrow(0, off, n).view(shape))
+                setattr(l, f'_{which}_batch_view', self._batch_arena.narrow(0, off, n).view(shape))
                 off += _cabi.ld4(n)
             if which == 'a':
                 self._a_block_numel = off
@@ -366,7 +381,14 @@ class BaseKFACPreconditioner:
         for name, l in ll:
             mine_a = rank == self._assignment.inv_worker(name, 'A')
             mine_g = rank == self._assignment.inv_worker(name, 'G')
-            if l.method == ComputeMethod.EIGEN:
+            if l.diag_a:
+                # embedding: only G is decomposed; its K-major basis for the GEMM engine, or the scratch of G_inv
+                if l.method == ComputeMethod.EIGEN:
+                    if self._assignment.is_grad_worker(name):
+                        plan.append((l, '_qgT', (l.g_dim, l.g_dim)))
+                elif mine_g:
+                    plan += [(l, '_qg', (l.g_dim, l.g_dim)), (l, '_dg', (l.g_dim,))]
+            elif l.method == ComputeMethod.EIGEN:
                 if self._assignment.is_grad_worker(name):
                     # K-major (transposed) copies of the eigenbases for the GEMM engine
                     plan += [(l, '_qaT', (l.a_dim, l.a_dim)), (l, '_qgT', (l.g_dim, l.g_dim))]
@@ -578,7 +600,8 @@ class BaseKFACPreconditioner:
             self._a_reduce_work.wait()
             self._a_reduce_work = None
             self._a_block_reduced = False
-        x = cast_for_factor(x, layer.factor_dtype)
+        if not layer.diag_a:        # integer indices are counted as they are
+            x = cast_for_factor(x, layer.factor_dtype)
         layer.module.accumulate_a(x, layer._a_batch_view, self._scratch)
         if layer.method == ComputeMethod.EKFAC:
             n = layer.module.num_rows_a(x)
@@ -589,6 +612,11 @@ class BaseKFACPreconditioner:
         self._mini_steps[name] += 1
         if self._update_factors_in_hook and self._mini_steps[name] % self._accumulation_steps == 0:
             self._mark_pending(layer, 'a')
+
+    def _hook_output(self, module: torch.nn.Module, input_, output: torch.Tensor) -> None:
+        """Forward hook of an embedding: the gradient of its output reaches _save_grad_output through a tensor hook."""
+        if module.training and output.requires_grad:
+            output.register_hook(lambda g: self._save_grad_output(module, None, g))
 
     @torch.no_grad()
     def _save_grad_output(self, module: torch.nn.Module, grad_input, grad_output) -> None:
@@ -678,21 +706,31 @@ class BaseKFACPreconditioner:
             # pack -> one all-reduce of the packed arena -> mirror back
             lib = _cabi.load()
             stream = _cabi.stream_ptr()
+            # (a diagonal A -- a vector -- is passed through as it is)
+            def packed_numel(view, d):
+                return d if view.dim() == 1 else d * (d + 1) // 2
             if getattr(self, '_packed_arena', None) is None:
-                total = sum(l.a_dim * (l.a_dim + 1) // 2 + l.g_dim * (l.g_dim + 1) // 2 for _, l in ll)
+                total = sum(packed_numel(l._a_batch_view, l.a_dim) + packed_numel(l._g_batch_view, l.g_dim)
+                            for _, l in ll)
                 self._packed_arena = torch.empty(total, dtype=torch.float32, device=self._device)
             off = 0
             todo = []
             for _, l in ll:
                 for view, d in ((l._a_batch_view, l.a_dim), (l._g_batch_view, l.g_dim)):
-                    n = d * (d + 1) // 2
+                    n = packed_numel(view, d)
                     todo.append((view, d, self._packed_arena.narrow(0, off, n)))
                     off += n
             for view, d, packed in todo:
-                _cabi.check(lib.kfac_triu_pack(view.data_ptr(), d, packed.data_ptr(), stream), 'kfac_triu_pack')
+                if view.dim() == 1:
+                    packed.copy_(view)
+                else:
+                    _cabi.check(lib.kfac_triu_pack(view.data_ptr(), d, packed.data_ptr(), stream), 'kfac_triu_pack')
             self._tdc.allreduce_average(self._packed_arena, group=None)
             for view, d, packed in todo:
-                _cabi.check(lib.kfac_triu_unpack(packed.data_ptr(), d, view.data_ptr(), stream), 'kfac_triu_unpack')
+                if view.dim() == 1:
+                    view.copy_(packed)
+                else:
+                    _cabi.check(lib.kfac_triu_unpack(packed.data_ptr(), d, view.data_ptr(), stream), 'kfac_triu_unpack')
         elif self._a_block_reduced:
             total = self._batch_arena.numel()
             self._tdc.allreduce_average(self._batch_arena.narrow(0, self._a_block_numel, total - self._a_block_numel),
@@ -714,6 +752,18 @@ class BaseKFACPreconditioner:
             flags = self._ema_scratch.get(sum(sizes), self._device)
             flag_off = 0
         for alpha, todo in self._pending_alpha.items():
+            # diagonal A factors (embeddings): their own EMA, never guarded (a window of token counts is finite)
+            diag = [l for l, which in todo if which == 'a' and l.diag_a]
+            if diag:
+                todo = [(l, which) for l, which in todo if not (which == 'a' and l.diag_a)]
+                ditems = (_cabi.EmaItem * len(diag))()
+                for i, layer in enumerate(diag):
+                    ditems[i] = _cabi.EmaItem(layer._a_view.data_ptr(), layer._a_batch_view.data_ptr(),
+                                              layer.a_dim, int(not layer._has_a), 1.0 / layer._a_count)
+                    layer._has_a, layer._a_count, layer._a_pending = True, 0, False
+                _cabi.check(lib.kfac_factor_ema_diag(ditems, len(diag), alpha, stream), 'kfac_factor_ema_diag')
+                if not todo:
+                    continue
             items = (_cabi.EmaItem * len(todo))()
             scales = (C.c_void_p * len(todo))()      # guarded EMA: loss-scale slot of a G item, NULL otherwise
             for i, (layer, which) in enumerate(todo):
@@ -776,7 +826,9 @@ class BaseKFACPreconditioner:
             return
         self._eig_event.synchronize()
         self._eig_pending = False
-        word = int(self._eig_status.item())
+        word = 0
+        for slot in range(self._eig_slots):
+            word |= int(self._eig_status[slot])
         if word:
             why = ' and '.join(w for b, w in ((1, 'an iteration did not converge'), (2, 'non-finite eigenvalues')) if word & b)
             raise _cabi.KFACNativeError(f'eigendecomposition of the K-FAC factors failed: {why} '
@@ -791,6 +843,7 @@ class BaseKFACPreconditioner:
         damping = float(self.damping)
         stream = _cabi.stream_ptr()
         eig: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
+        eig_emb: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
         post: list[tuple[KFACLayer, str]] = []
         for name, layer in reversed(self._layer_list()):
             mine_a = rank == self._assignment.inv_worker(name, 'A')
@@ -800,7 +853,17 @@ class BaseKFACPreconditioner:
             if mine_g and not layer._has_g:
                 raise RuntimeError('Cannot eigendecompose G before G has been computed')
             I = layer._inv
-            if layer.method == ComputeMethod.EIGEN:
+            if layer.diag_a:
+                # embedding: A is its own eigendecomposition (Qa = I); its snapshot is the one the precondition uses
+                # until the next inverse step, like the eigenvalues of a dense A
+                if mine_a:
+                    I['da'].copy_(layer._a_view)
+                if mine_g and layer.method == ComputeMethod.EIGEN:
+                    eig_emb.append((layer._g_view, I['qg'], I['_qgT'], I['dg'], layer.g_dim))
+                elif mine_g:
+                    eig_emb.append((layer._g_view, I['_qg'], None, I['_dg'], layer.g_dim))
+                    post.append((layer, 'g_inv'))
+            elif layer.method == ComputeMethod.EIGEN:
                 if layer.prediv_eigenvalues:
                     if mine_a:
                         eig.append((layer._a_view, I['qa'], I['_qaT'], I['_da'], layer.a_dim))
@@ -824,24 +887,30 @@ class BaseKFACPreconditioner:
                 if mine_g:
                     eig.append((layer._g_view, I['_qg'], None, I['_dg'], layer.g_dim))
                     post.append((layer, 'g_inv'))
-        if eig:
-            items = (_cabi.EighItem * len(eig))()
-            ns = (C.c_int * len(eig))()
-            for i, (F, Q, QT, d, n) in enumerate(eig):
+        # the G factors of embeddings are decomposed in a call of their own: the batched solver shares its CTAs among
+        # the matrices of a call, so the other layers get the same schedule (and bits) with or without embeddings
+        batches = [b for b in (eig, eig_emb) if b]
+        if batches and self._eig_status is None:
+            self._eig_status = torch.zeros(2, dtype=torch.int32).pin_memory()
+            self._eig_event = torch.cuda.Event()
+        for slot, batch in enumerate(batches):
+            items = (_cabi.EighItem * len(batch))()
+            ns = (C.c_int * len(batch))()
+            for i, (F, Q, QT, d, n) in enumerate(batch):
                 items[i] = _cabi.EighItem(F.data_ptr(), Q.data_ptr(), QT.data_ptr() if QT is not None else None,
                                           d.data_ptr(), n, _cabi.ld4(n), None)
                 ns[i] = n
-            need = lib.kfac_eigh_workspace_bytes(ns, len(eig))
+            need = lib.kfac_eigh_workspace_bytes(ns, len(batch))
             ws = self._eig_scratch.get(need, self._device)
-            _cabi.check(lib.kfac_eigh_batched(items, len(eig), ws.data_ptr(), need, 0, 0.0, stream),
+            _cabi.check(lib.kfac_eigh_batched(items, len(batch), ws.data_ptr(), need, 0, 0.0, stream),
                         'kfac_eigh_batched')
             # status word (non-convergence / non-finite eigenvalues): copied to pinned memory without a sync and
             # inspected before the NEXT use of the second-order data (torch.linalg.eigh raises immediately,
             # kfac/layers/eigen.py:310; here the error surfaces one call later instead of stalling the stream)
-            if self._eig_status is None:
-                self._eig_status = torch.zeros(1, dtype=torch.int32).pin_memory()
-                self._eig_event = torch.cuda.Event()
-            _cabi.check(lib.kfac_eigh_status(ws.data_ptr(), self._eig_status.data_ptr(), stream), 'kfac_eigh_status')
+            _cabi.check(lib.kfac_eigh_status(ws.data_ptr(), self._eig_status[slot:].data_ptr(), stream),
+                        'kfac_eigh_status')
+        if batches:
+            self._eig_slots = len(batches)
             self._eig_event.record()
             self._eig_pending = True
         for layer, what in post:
@@ -947,7 +1016,19 @@ class BaseKFACPreconditioner:
             w, b = self._grad_ptrs(layer)
             I = layer._inv
             ready = layer._inv_ready
-            if layer.method == ComputeMethod.EIGEN:
+            if layer.diag_a:
+                eigen = layer.method == ComputeMethod.EIGEN
+                need = {'da', 'qg', 'dg'} if eigen else {'da', 'g_inv'}
+                if not need <= ready:
+                    raise RuntimeError('The second-order data of the embedding has not been computed')
+                items[i] = _cabi.PrecondItem(
+                    w.data_ptr(), None, _cabi.DTYPE_CODE[w.dtype], layer.g_dim, layer.a_dim,
+                    None, None, I['qg'].data_ptr() if eigen else None, I['_qgT'].data_ptr() if eigen else None,
+                    None, I['da'].data_ptr(), I['dg'].data_ptr() if eigen else None, None,
+                    None if eigen else I['g_inv'].data_ptr(),
+                    0, _cabi.ld4(layer.g_dim), 0, layer._p_store.data_ptr(), _cabi.ld4(layer.g_dim), None, 0,
+                    _cabi.KFAC_ITEM_EMBEDDING)
+            elif layer.method == ComputeMethod.EIGEN:
                 ok = ('qa' in ready and 'qg' in ready and
                       ('dgda' in ready if layer.prediv_eigenvalues else ('da' in ready and 'dg' in ready)))
                 if not ok:
@@ -963,18 +1044,19 @@ class BaseKFACPreconditioner:
                     raise RuntimeError('Cannot precondition gradient before A and G have been inverted')
                 eigen = False
 
-            def p(key):
-                return I[key].data_ptr() if key in ready else None
+            if not layer.diag_a:
+                def p(key):
+                    return I[key].data_ptr() if key in ready else None
 
-            eig_ok = 'qa' in ready and 'qg' in ready
-            items[i] = _cabi.PrecondItem(
-                w.data_ptr(), b.data_ptr() if b is not None else None, _cabi.DTYPE_CODE[w.dtype],
-                layer.g_dim, layer.a_dim,
-                p('qa'), I['_qaT'].data_ptr() if eig_ok else None,
-                p('qg'), I['_qgT'].data_ptr() if eig_ok else None,
-                p('dgda'), p('da'), p('dg'), p('a_inv'), p('g_inv'),
-                _cabi.ld4(layer.a_dim), _cabi.ld4(layer.g_dim), _cabi.ld4(layer.a_dim),
-                layer._p_store.data_ptr(), _cabi.ld4(layer.a_dim), None, 0)
+                eig_ok = 'qa' in ready and 'qg' in ready
+                items[i] = _cabi.PrecondItem(
+                    w.data_ptr(), b.data_ptr() if b is not None else None, _cabi.DTYPE_CODE[w.dtype],
+                    layer.g_dim, layer.a_dim,
+                    p('qa'), I['_qaT'].data_ptr() if eig_ok else None,
+                    p('qg'), I['_qgT'].data_ptr() if eig_ok else None,
+                    p('dgda'), p('da'), p('dg'), p('a_inv'), p('g_inv'),
+                    _cabi.ld4(layer.a_dim), _cabi.ld4(layer.g_dim), _cabi.ld4(layer.a_dim),
+                    layer._p_store.data_ptr(), _cabi.ld4(layer.a_dim), None, 0)
             if fused:
                 off = layer._p_store.data_ptr() - p_base
                 arr = (C.c_void_p * len(self._peer_p_bases))(*[b + off for b in self._peer_p_bases.values()])
@@ -1009,10 +1091,10 @@ class BaseKFACPreconditioner:
         items = (_cabi.GradItem * max(1, len(ll)))()
         for i, (_, layer) in enumerate(ll):
             w, b = self._grad_ptrs(layer)
+            rows, cols = layer.p_shape          # an embedding is a bias-less (V, d) layer here
             items[i] = _cabi.GradItem(layer._p_store.data_ptr(), w.data_ptr(),
                                       b.data_ptr() if b is not None else None,
-                                      _cabi.DTYPE_CODE[w.dtype], layer.g_dim, layer.a_dim,
-                                      _cabi.ld4(layer.a_dim))
+                                      _cabi.DTYPE_CODE[w.dtype], rows, cols, _cabi.ld4(cols))
         stream = _cabi.stream_ptr()
         kl_clip = self.kl_clip
         scale_ptr = None

@@ -387,6 +387,43 @@ __global__ void __launch_bounds__(256) window_scan_kernel(const __grid_constant_
   if (__syncthreads_or(bad) && threadIdx.x == 0) atomicOr(sb.dropped + item, 1);
 }
 
+// ---- embedding layers: diagonal A -------------------------------------------------------------
+// counts[idx[r]] += 1 (integer atomics: the histogram does not depend on the order of the rows)
+template <typename I>
+__global__ void histogram_kernel(const I* __restrict__ idx, int64_t n, unsigned int* counts) {
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x)
+    atomicAdd(counts + idx[r], 1u);
+}
+
+// acc[v] += alpha * counts[v]: one rounding of the product, one of the sum, in a fixed order per entry
+__global__ void scale_add_counts_kernel(const unsigned int* __restrict__ counts, int V, float alpha, float* acc) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < V; v += gridDim.x * blockDim.x)
+    acc[v] = __fadd_rn(acc[v], __fmul_rn(alpha, (float)counts[v]));
+}
+
+// EMA of diagonal factors over up to 40 items: the diagonal of ema_kernel, with its beta and its rounding
+struct EmaDiagBatch {
+  kfac_ema_item it[40];
+  int64_t elem0[41];     // prefix sums of d
+  int count;
+  float alpha;
+};
+
+__global__ void __launch_bounds__(256) ema_diag_kernel(const __grid_constant__ EmaDiagBatch eb) {
+  const int64_t total = eb.elem0[eb.count];
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+    int item = 0;
+    while (item + 1 < eb.count && e >= eb.elem0[item + 1]) ++item;
+    const kfac_ema_item& it = eb.it[item];
+    const int64_t v = e - eb.elem0[item];
+    const float beta = (1.f - eb.alpha) * it.inv_count * 0.5f;
+    const float x = it.batch[v];
+    const float f = it.first ? 1.f : it.factor[v];
+    it.factor[v] = ema_update(eb.alpha, f, beta, x, x);   // (x + x) * 0.5 = x, as batch + batch^T on the diagonal
+    it.batch[v] = 0.f;
+  }
+}
+
 __global__ void dgda_kernel(const float* dg, const float* da, int g, int a, float damping, float* out, int ldo) {
   const int64_t total = (int64_t)g * ldo;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -656,6 +693,53 @@ extern "C" int kfac_factor_ema_guarded(const kfac_ema_item* items, int count, fl
   cudaStream_t s = (cudaStream_t)stream;
   KFAC_CUDA(cudaMemsetAsync(ws, 0, (size_t)count * sizeof(int), s));
   return launch_ema(items, count, alpha, loss_scale, (int*)ws, skipped, s);
+}
+
+extern "C" size_t kfac_factor_embedding_workspace_bytes(int V) {
+  return V > 0 ? align_up((size_t)V * sizeof(unsigned int), 256) : 0;
+}
+
+extern "C" int kfac_factor_embedding(const void* idx, int index_dtype, int64_t N, int V, float alpha, float* acc,
+                                     void* ws, size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(acc && V > 0 && N >= 0 && N < (1ll << 32) && (idx || N == 0), "embedding factor args");
+  KFAC_CHECK_ARG(index_dtype == KFAC_I32 || index_dtype == KFAC_I64, "index dtype");
+  const size_t need = kfac_factor_embedding_workspace_bytes(V);
+  if (!ws || ws_bytes < need) {
+    set_error("factor_embedding: workspace too small (%zu < %zu)", ws_bytes, need);
+    return KFAC_ERR_WORKSPACE;
+  }
+  if (N == 0) return KFAC_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned int* counts = (unsigned int*)ws;
+  KFAC_CUDA(cudaMemsetAsync(counts, 0, (size_t)V * sizeof(unsigned int), s));
+  if (index_dtype == KFAC_I32) histogram_kernel<int><<<grid_for(N), 256, 0, s>>>((const int*)idx, N, counts);
+  else histogram_kernel<long long><<<grid_for(N), 256, 0, s>>>((const long long*)idx, N, counts);
+  KFAC_LAUNCH_CHECK();
+  scale_add_counts_kernel<<<grid_for(V), 256, 0, s>>>(counts, V, alpha, acc);
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
+extern "C" int kfac_factor_ema_diag(const kfac_ema_item* items, int count, float alpha, void* stream) {
+  KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "items");
+  for (int i = 0; i < count; ++i)
+    KFAC_CHECK_ARG(items[i].factor && items[i].batch && items[i].d > 0, "ema item");
+  cudaStream_t s = (cudaStream_t)stream;
+  for (int base = 0; base < count; base += 40) {
+    EmaDiagBatch eb{};
+    eb.count = min(40, count - base);
+    eb.alpha = alpha;
+    int64_t total = 0;
+    for (int i = 0; i < eb.count; ++i) {
+      eb.it[i] = items[base + i];
+      eb.elem0[i] = total;
+      total += eb.it[i].d;
+    }
+    eb.elem0[eb.count] = total;
+    ema_diag_kernel<<<grid_for(total), 256, 0, s>>>(eb);
+    KFAC_LAUNCH_CHECK();
+  }
+  return KFAC_OK;
 }
 
 extern "C" int kfac_dgda(const float* dg, const float* da, int g, int a, float damping, float* out,

@@ -20,6 +20,8 @@ from kfac_b200 import _cabi
 class ModuleHelper:
     """Geometry + native dispatch for one supported module type."""
 
+    diagonal_a = False      # True: A is diagonal and kept as a vector (embeddings)
+
     def __init__(self, module: torch.nn.Module):
         self.module = module
 
@@ -255,15 +257,62 @@ class Conv2dModuleHelper(ModuleHelper):
                     'kfac_rows_conv2d_gradout')
 
 
+class EmbeddingModuleHelper(ModuleHelper):
+    """torch.nn.Embedding (an extension beyond the reference, opt-in through `precondition_embeddings`).
+
+    An embedding is a Linear layer whose input rows are one-hot vectors e_idx, so A = (1/N) sum_r e_r e_r^T is
+    DIAGONAL: the token frequencies counts / N, kept as a vector of V floats (`a_factor_shape` is (V,)).  Every
+    index position is one row, `padding_idx` positions included (their gradient row is zero, so their P row is
+    zero), which keeps N = idx.numel() known on the host.  G is formed from the grad-output rows exactly like a
+    Linear layer's.  The gradient and P use the weight's own layout (V x d)."""
+
+    diagonal_a = True
+
+    @property
+    def a_factor_shape(self):
+        return (self.module.num_embeddings,)
+
+    @property
+    def g_factor_shape(self):
+        d = self.module.embedding_dim
+        return (d, d)
+
+    def has_bias(self) -> bool:
+        return False
+
+    def accumulate_a(self, x, acc, scratch):
+        _cabi.require_device(x)
+        try:
+            code = _cabi.INDEX_DTYPE_CODE[x.dtype]
+        except KeyError:
+            raise ValueError(f'unsupported embedding index dtype {x.dtype}') from None
+        x = x.detach()
+        x = x if x.is_contiguous() else x.contiguous()
+        V = self.module.num_embeddings
+        n = x.numel()
+        if n == 0:
+            return
+        lib = _cabi.load()
+        need = lib.kfac_factor_embedding_workspace_bytes(V)
+        ws = scratch.get(need, x.device)
+        _cabi.check(lib.kfac_factor_embedding(x.data_ptr(), code, n, V, 1.0 / n, acc.data_ptr(), ws.data_ptr(), need,
+                                              _cabi.stream_ptr()), 'kfac_factor_embedding')
+
+    accumulate_g = LinearModuleHelper.accumulate_g
+
+
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
 CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
+EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
 
 
-def get_module_helper(module: torch.nn.Module) -> ModuleHelper | None:
+def get_module_helper(module: torch.nn.Module, embeddings: bool = False) -> ModuleHelper | None:
     if isinstance(module, LINEAR_TYPES):
         return LinearModuleHelper(module)
     if isinstance(module, CONV2D_TYPES):
         return Conv2dModuleHelper(module)
+    if embeddings and isinstance(module, EMBEDDING_TYPES):
+        return EmbeddingModuleHelper(module)
     return None
 
 
@@ -294,6 +343,8 @@ class KFACLayer:
         self.symmetric_factors = module.has_symmetric_factors()
         self.a_dim = module.a_factor_shape[0]
         self.g_dim = module.g_factor_shape[0]
+        # A is a vector of a_dim floats (embeddings); P then has the weight's layout (a x g) instead of (g x a)
+        self.diag_a = module.diagonal_a
         self.index = -1
         # arena views (bound by the preconditioner)
         self._a_view = self._g_view = None
@@ -353,8 +404,13 @@ class KFACLayer:
     g_inv = property(lambda self: self._inv_get('g_inv'))
 
     @property
+    def p_shape(self) -> tuple[int, int]:
+        """Logical shape of P: (g, a), or the weight layout (a, g) = (V, d) of an embedding."""
+        return (self.a_dim, self.g_dim) if self.diag_a else (self.g_dim, self.a_dim)
+
+    @property
     def grad(self):
-        """Preconditioned gradient P (g x a) while it is pending write-back."""
+        """Preconditioned gradient P (g x a; V x d for an embedding) while it is pending write-back."""
         return self._p_view if self._grad_ready else None
 
     def state_dict(self) -> dict[str, torch.Tensor | None]:
@@ -364,6 +420,11 @@ class KFACLayer:
     def load_state_dict(self, state_dict: dict[str, torch.Tensor | None]) -> None:
         if 'A' not in state_dict or 'G' not in state_dict:
             raise KeyError("KFACLayer state_dict must contain keys 'A' and 'G'")
+        if self.diag_a:
+            for key, want in (('A', (self.a_dim,)), ('G', (self.g_dim, self.g_dim))):
+                t = state_dict[key]
+                if t is not None and tuple(t.shape) != want:
+                    raise ValueError(f'embedding factor {key} has shape {tuple(t.shape)}, expected {want}')
         if state_dict['A'] is not None:
             self._a_view.copy_(state_dict['A'].to(torch.float32))
             self._has_a = True
@@ -373,10 +434,11 @@ class KFACLayer:
 
     def memory_usage(self) -> dict[str, int]:
         b = 4
+        a_numel = self.a_dim if self.diag_a else self.a_dim * self.a_dim
         out = {
-            'a_factors': self.a_dim * self.a_dim * b if self._has_a else 0,
+            'a_factors': a_numel * b if self._has_a else 0,
             'g_factors': self.g_dim * self.g_dim * b if self._has_g else 0,
-            'a_batch': self.a_dim * self.a_dim * b if self._a_count else 0,
+            'a_batch': a_numel * b if self._a_count else 0,
             'g_batch': self.g_dim * self.g_dim * b if self._g_count else 0,
             'a_inverses': 0, 'g_inverses': 0,
         }
@@ -402,10 +464,11 @@ def any_match(query: str, patterns: list[str]) -> bool:
     return any(re.compile(p).search(query) for p in patterns)
 
 
-def register_modules(model: torch.nn.Module, skip_layers: list[str],
+def register_modules(model: torch.nn.Module, skip_layers: list[str], precondition_embeddings: bool = False,
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
-    (kfac/layers/register.py:57-95)."""
+    (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
+    modules (not in the reference)."""
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     for name, module in model.named_modules():
         if len(list(module.children())) != 0:
@@ -414,7 +477,7 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str],
             continue
         if not all(p.requires_grad for p in module.parameters()):
             continue
-        helper = get_module_helper(module)
+        helper = get_module_helper(module, embeddings=precondition_embeddings)
         if helper is None:
             continue
         assert module not in layers

@@ -22,13 +22,48 @@ from kfac_b200.base_preconditioner import BaseKFACPreconditioner
 from kfac_b200.distributed import ArenaCommunicator, get_rank, get_world_size
 from kfac_b200.enums import (AllreduceMethod, AssignmentStrategy, ComputeMethod,
                              DistributedStrategy)
-from kfac_b200.layers import register_modules
+from kfac_b200.layers import KFACLayer, register_modules
 
 logger = logging.getLogger(__name__)
 
 
 def _mock_new_group(x: list[int]) -> None:
     return None
+
+
+def layer_work(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
+               assignment_strategy: AssignmentStrategy) -> dict[str, dict[str, float]]:
+    """Per-factor cost the KAISA placement balances: d^3 (COMPUTE) or d^2 (MEMORY) for a dense factor.  A diagonal
+    factor (an embedding's A) is never decomposed and takes V floats, so its cost is V under both strategies;
+    a V^3 cost would let one vocabulary dominate the greedy placement."""
+    if assignment_strategy == AssignmentStrategy.COMPUTE:
+        cost = lambda n: n ** 3  # noqa: E731
+    elif assignment_strategy == AssignmentStrategy.MEMORY:
+        cost = lambda n: n ** 2  # noqa: E731
+    else:
+        raise AssertionError(f'Unknown assignment_strategy={assignment_strategy}')
+    return {name: {'A': l.a_dim if l.diag_a else cost(l.a_dim), 'G': cost(l.g_dim)} for name, l in layers.values()}
+
+
+def _check_embeddings(layers: dict[torch.nn.Module, tuple[str, KFACLayer]], compute_method: ComputeMethod) -> None:
+    """Reject the registered embeddings this preconditioner cannot handle."""
+    emb = [(module, name) for module, (name, l) in layers.items() if l.diag_a]
+    if not emb:
+        return
+    if compute_method == ComputeMethod.EKFAC:
+        raise ValueError(f'precondition_embeddings does not support compute_method=EKFAC (embedding "{emb[0][1]}"); '
+                         'add the embeddings to skip_layers')
+    for module, name in emb:
+        if module.sparse:
+            raise ValueError(f'embedding "{name}" has sparse=True: K-FAC needs a dense weight gradient '
+                             '(add it to skip_layers or use sparse=False)')
+        if module.scale_grad_by_freq:
+            raise ValueError(f'embedding "{name}" has scale_grad_by_freq=True: its weight gradient is then not the '
+                             'one the K-FAC factors model (add it to skip_layers)')
+        for other, (other_name, _) in layers.items():
+            if other is not module and any(p is module.weight for p in other.parameters()):
+                raise ValueError(f'embedding "{name}" shares its weight with "{other_name}": two layers would '
+                                 f'precondition one gradient; add one of them to skip_layers')
 
 
 class KFACPreconditioner(BaseKFACPreconditioner):
@@ -39,6 +74,13 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     factor step (George et al., 2018).  EKFAC needs `grad_worker_fraction` to resolve to COMM_OPT,
     `accumulation_steps=1` and, for integer schedules, `inv_update_steps` a multiple of
     `factor_update_steps`; `compute_eigenvalue_outer_product` is ignored with it.
+
+    `precondition_embeddings=True` also registers leaf `torch.nn.Embedding` modules (not `EmbeddingBag`), which
+    the reference leaves to the first-order optimizer.  Their A factor is diagonal (the token frequencies) and
+    kept as a vector; see `kfac_b200.layers.EmbeddingModuleHelper`.  The embedding's P is always formed from the
+    eigenvalue vectors (`compute_eigenvalue_outer_product` does not apply to it, so no V x d matrix is stored),
+    and its damping is the one of the step that preconditions.  It cannot be combined with EKFAC, sparse
+    gradients, `scale_grad_by_freq`, or a weight shared with another registered module (a tied LM head).
     """
 
     def __init__(
@@ -65,6 +107,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         skip_layers: list[str] | None = None,
         update_factors_in_hook: bool = True,
         loglevel: int = logging.DEBUG,
+        precondition_embeddings: bool = False,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -145,19 +188,14 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         self.tdc = ArenaCommunicator(bucket_cap_mb=allreduce_bucket_cap_mb)
 
         kfac_layers = register_modules(
-            model, self.skip_layers, method=compute_method,
+            model, self.skip_layers, precondition_embeddings=precondition_embeddings, method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
+        _check_embeddings(kfac_layers, compute_method)
         for name, kfac_layer in kfac_layers.values():
             logger.log(loglevel, f'Registered name="{name}": {repr(kfac_layer)}')
 
-        if assignment_strategy == AssignmentStrategy.COMPUTE:
-            cost = lambda n: n ** 3  # noqa: E731
-        elif assignment_strategy == AssignmentStrategy.MEMORY:
-            cost = lambda n: n ** 2  # noqa: E731
-        else:
-            raise AssertionError(f'Unknown assignment_strategy={assignment_strategy}')
-        work = {name: {'A': cost(l.a_dim), 'G': cost(l.g_dim)} for name, l in kfac_layers.values()}
+        work = layer_work(kfac_layers, assignment_strategy)
 
         assignment = KAISAAssignment(
             work, local_rank=get_rank(), world_size=size,
@@ -180,6 +218,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'inv_dtype': inv_dtype,
             'skip_layers': self.skip_layers,
             'symmetry_aware': symmetry_aware,
+            'precondition_embeddings': precondition_embeddings,
         }
         super().__init__(
             kfac_layers, factor_update_steps=factor_update_steps,
