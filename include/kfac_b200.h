@@ -132,10 +132,37 @@ int kfac_factor_embedding(const void* idx, int index_dtype, int64_t N, int V, fl
 /* EMA of diagonal factors (vectors of d = V floats), the schedule of kfac_factor_ema on the
  * diagonal and with the same rounding (the bits kfac_factor_ema gives on diag(batch)):
  *   factor = alpha*(first ? 1 : factor) + (1-alpha)*inv_count*batch;   batch = 0
- * There is no guarded variant: a window of token counts is finite whatever the loss scale, so
- * under a grad_scaler the A side of an embedding is never dropped, and its G side (a dense
- * d x d factor) goes through kfac_factor_ema_guarded like every other G.  One launch per 40 items. */
+ * A window of token counts (the A side of an embedding) is finite whatever the loss scale and
+ * always takes this unguarded EMA.  One launch per 40 items. */
 int kfac_factor_ema_diag(const kfac_ema_item* items, int count, float alpha, void* stream);
+/* Guarded EMA of diagonal factors: the contract of kfac_factor_ema_guarded on vectors of d
+ * floats (the diagonal G of a large-output Linear layer can overflow under fp16).  loss_scale:
+ * HOST array of `count` DEVICE pointers (NULL array or entry = 1), u = (1 / *loss_scale[i])^2.
+ * A window with an entry whose unscaled value is not finite or exceeds 1e15 is dropped: the
+ * factor keeps its value (all ones when `first` = 1), the batch is zeroed and *skipped (may be
+ * NULL) is incremented.  Every kept window gets the bits kfac_factor_ema_diag gives on batch * u.
+ * ws: kfac_factor_ema_diag_guarded_workspace_bytes(count) bytes (one drop flag per item).
+ * Two launches per 40 items (scan, EMA). */
+size_t kfac_factor_ema_diag_guarded_workspace_bytes(int count);
+int kfac_factor_ema_diag_guarded(const kfac_ema_item* items, int count, float alpha,
+                                 const float* const* loss_scale, unsigned long long* skipped,
+                                 void* ws, size_t ws_bytes, void* stream);
+
+/* Diagonal-G Linear layers (an extension beyond the reference, opt-in): the G factor of a layer
+ * with many outputs (an LM head, V = 50257) is approximated by its diagonal, kept as V floats.
+ * kfac_factor_linear_diag: acc[j] += scale * sum_r x[r, j]^2 over x (rows x features, dtype
+ * KFAC_F32/F16/BF16, contiguous), the diagonal of what kfac_factor_linear accumulates for the same
+ * input.  Deterministic and without a host sync: the rows are split into a number of chunks that
+ * depends on `rows` only, each chunk's column sums (accumulated in fp64, stored as fp32) go to ws
+ * (kfac_factor_linear_diag_workspace_bytes(rows, features) bytes), and a second launch adds them
+ * in a fixed order.  No floating-point atomics. */
+size_t kfac_factor_linear_diag_workspace_bytes(int64_t rows, int features);
+int kfac_factor_linear_diag(const void* x, int dtype, int64_t rows, int features, float scale,
+                            float* acc, void* ws, size_t ws_bytes, void* stream);
+/* dst[i] = src[i] for n floats; ORs 2 (the non-finite bit of the kfac_eigh_batched status word)
+ * into the DEVICE int *status when an entry is not finite or exceeds 1e15 in magnitude.  The
+ * snapshot of a diagonal factor at an inverse step, checked like a decomposed factor. */
+int kfac_diag_snapshot(const float* src, float* dst, int n, int* status, void* stream);
 
 /* ------------------------------------------------------- eigendecomposition
  * K5: replaces torch.linalg.eigh + clamp(min=0) in
@@ -197,8 +224,14 @@ int kfac_transpose(const float* src, int ld_src, float* dst, int ld_dst, int row
  *   EIGEN  : P = [(wgrad Qg) / (da x dg + damping)] Qg^T     (qg, qgT, dg; dgda is not used)
  *   INVERSE: P = diag(1 / (da + damping)) wgrad Ginv          (g_inv)
  * qa, qaT, a_inv, dgda and ldqa are ignored.  The two (one) GEMMs join the grouped launches of
- * the dense items; the other items' results do not depend on the embedding items. */
-enum kfac_item_kind { KFAC_ITEM_DENSE = 0, KFAC_ITEM_EMBEDDING = 1 };
+ * the dense items; the other items' results do not depend on the embedding items.
+ * Diagonal-G items (kind = KFAC_ITEM_DIAG_G): wgrad (g = V, a - has_bias) and bgrad as for a
+ * dense item, dg the diagonal G factor (V floats; its own eigenvalues), P (g x ldp, ldp >= a):
+ *   EIGEN  : P = [(grad Qa) / (dg x da + damping)] Qa^T      (qa, qaT, da; dgda is not used)
+ *   INVERSE: P = diag(1 / (dg + damping)) grad Ainv           (a_inv)
+ * qg, qgT, g_inv, dgda, ldqg and ld_dgda are ignored.  This is the embedding item with the dense
+ * factor on the A side. */
+enum kfac_item_kind { KFAC_ITEM_DENSE = 0, KFAC_ITEM_EMBEDDING = 1, KFAC_ITEM_DIAG_G = 2 };
 typedef struct kfac_precond_item {
   const void* wgrad; /* (g, a - has_bias) */
   const void* bgrad; /* (g) or NULL */

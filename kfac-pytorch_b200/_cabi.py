@@ -21,7 +21,7 @@ KFAC_ERR_WORKSPACE, KFAC_ERR_NO_CONVERGE, KFAC_ERR_UNSUPPORTED = -4, -5, -6
 KFAC_EIGEN, KFAC_INVERSE = 1, 2
 KFAC_EKFAC_KEEP, KFAC_EKFAC_EMA, KFAC_EKFAC_RESET, KFAC_EKFAC_SEED = 0, 1, 2, 3
 
-KFAC_ITEM_DENSE, KFAC_ITEM_EMBEDDING = 0, 1
+KFAC_ITEM_DENSE, KFAC_ITEM_EMBEDDING, KFAC_ITEM_DIAG_G = 0, 1, 2
 
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 INDEX_DTYPE_CODE = {torch.int32: 3, torch.int64: 4}
@@ -83,6 +83,13 @@ SIGNATURES = {
     'kfac_factor_embedding': (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_void_p, c_void_p, c_size_t,
                                       c_void_p]),
     'kfac_factor_ema_diag': (c_int, [C.POINTER(EmaItem), c_int, c_float, c_void_p]),
+    'kfac_factor_ema_diag_guarded_workspace_bytes': (c_size_t, [c_int]),
+    'kfac_factor_ema_diag_guarded': (c_int, [C.POINTER(EmaItem), c_int, c_float, C.POINTER(c_void_p), c_void_p,
+                                             c_void_p, c_size_t, c_void_p]),
+    'kfac_factor_linear_diag_workspace_bytes': (c_size_t, [c_int64, c_int]),
+    'kfac_factor_linear_diag': (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_void_p, c_void_p, c_size_t,
+                                        c_void_p]),
+    'kfac_diag_snapshot': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     'kfac_eigh_workspace_bytes': (c_size_t, [C.POINTER(c_int), c_int]),
     'kfac_eigh_batched': (c_int, [C.POINTER(EighItem), c_int, c_void_p, c_size_t, c_int, c_float, c_void_p]),
     'kfac_eigh_status': (c_int, [c_void_p, c_void_p, c_void_p]),

@@ -49,6 +49,7 @@ from __future__ import annotations
 
 import ctypes as C
 import logging
+import math
 import warnings
 from collections import defaultdict
 from typing import Any, Callable
@@ -132,15 +133,18 @@ def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignm
                 inv[key] = _Segment(src, group)
             return inv[key]
 
-        if layer.diag_a:
-            # embedding: the A snapshot (its own eigenvalues) and the data of G; never a V x d dgda
-            seg(src_a).add(layer, 'da', (a,))
-            sg = seg(src_g)
+        if layer.diag_side:
+            # embedding / diagonal-G layer: the snapshot of the diagonal factor (its own eigenvalues) and the data of
+            # the dense one; never a V x d dgda
+            d, f = layer.diag_side, layer.dense_side
+            dims, srcs = {'a': a, 'g': g}, {'a': src_a, 'g': src_g}
+            seg(srcs[d]).add(layer, 'd' + d, (dims[d],))
+            sf, n = seg(srcs[f]), dims[f]
             if layer.method == ComputeMethod.EIGEN:
-                sg.add(layer, 'qg', (g, g))
-                sg.add(layer, 'dg', (g,))
+                sf.add(layer, 'q' + f, (n, n))
+                sf.add(layer, 'd' + f, (n,))
             else:
-                sg.add(layer, 'g_inv', (g, g))
+                sf.add(layer, f + '_inv', (n, n))
         elif layer.method == ComputeMethod.EIGEN:
             if layer.prediv_eigenvalues:
                 s = seg(src_g)
@@ -270,6 +274,7 @@ class BaseKFACPreconditioner:
         # store preconditioned gradients straight into the receivers' arenas (P2P) instead of broadcasting
         self.fused_grad_broadcast = True
         self._eig_status: torch.Tensor | None = None     # pinned host int: status word of the last eigensolver call
+        self._diag_status: torch.Tensor | None = None    # device int: status of the diagonal-factor snapshots
 
         for module, (_, layer) in self._layers.items():
             module.register_forward_pre_hook(self._save_input)
@@ -338,8 +343,9 @@ class BaseKFACPreconditioner:
         _cabi.load()
         self._device = device
         ll = self._layer_list()
-        # dense d x d factors (a vector of V floats for the diagonal A of an embedding), each starting 16-byte aligned
-        total = sum(_cabi.ld4(l.a_dim if l.diag_a else l.a_dim ** 2) + _cabi.ld4(l.g_dim ** 2) for _, l in ll)
+        # dense d x d factors (a vector of V floats for the diagonal A of an embedding or the diagonal G of a
+        # diagonal-G layer), each starting 16-byte aligned
+        total = sum(_cabi.ld4(math.prod(l.a_factor_shape)) + _cabi.ld4(math.prod(l.g_factor_shape)) for _, l in ll)
         self._factor_arena = torch.zeros(total, dtype=torch.float32, device=device)
         self._batch_arena = torch.zeros(total, dtype=torch.float32, device=device)
         # layout: all A factors, then all G factors -- the A block is complete after the forward pass and is
@@ -347,9 +353,8 @@ class BaseKFACPreconditioner:
         off = 0
         for which in ('a', 'g'):
             for _, l in ll:
-                dim = l.a_dim if which == 'a' else l.g_dim
-                shape = (dim,) if which == 'a' and l.diag_a else (dim, dim)
-                n = dim if len(shape) == 1 else dim * dim
+                shape = l.a_factor_shape if which == 'a' else l.g_factor_shape
+                n = math.prod(shape)
                 setattr(l, f'_{which}_view', self._factor_arena.narrow(0, off, n).view(shape))
                 setattr(l, f'_{which}_batch_view', self._batch_arena.narrow(0, off, n).view(shape))
                 off += _cabi.ld4(n)
@@ -381,13 +386,16 @@ class BaseKFACPreconditioner:
         for name, l in ll:
             mine_a = rank == self._assignment.inv_worker(name, 'A')
             mine_g = rank == self._assignment.inv_worker(name, 'G')
-            if l.diag_a:
-                # embedding: only G is decomposed; its K-major basis for the GEMM engine, or the scratch of G_inv
+            if l.diag_side:
+                # embedding / diagonal-G layer: only the dense factor f is decomposed; its K-major basis for the GEMM
+                # engine, or the scratch of its inverse
+                f = l.dense_side
+                n = l.a_dim if f == 'a' else l.g_dim
                 if l.method == ComputeMethod.EIGEN:
                     if self._assignment.is_grad_worker(name):
-                        plan.append((l, '_qgT', (l.g_dim, l.g_dim)))
-                elif mine_g:
-                    plan += [(l, '_qg', (l.g_dim, l.g_dim)), (l, '_dg', (l.g_dim,))]
+                        plan.append((l, f'_q{f}T', (n, n)))
+                elif mine_a if f == 'a' else mine_g:
+                    plan += [(l, f'_q{f}', (n, n)), (l, f'_d{f}', (n,))]
             elif l.method == ComputeMethod.EIGEN:
                 if self._assignment.is_grad_worker(name):
                     # K-major (transposed) copies of the eigenbases for the GEMM engine
@@ -746,37 +754,45 @@ class BaseKFACPreconditioner:
         lib = _cabi.load()
         stream = _cabi.stream_ptr()
         flags = None
+        # diagonal factors (an embedding's A, a diagonal-G layer's G) take the EMA of vectors.  A window of token counts
+        # is finite whatever the loss scale and is never guarded; a diagonal G is guarded like every G
+        split = {alpha: ([(l, w) for l, w in todo if l.diag_side == w and not (self._guard_factors and w == 'g')],
+                         [(l, w) for l, w in todo if l.diag_side == w and self._guard_factors and w == 'g'],
+                         [(l, w) for l, w in todo if l.diag_side != w])
+                 for alpha, todo in self._pending_alpha.items()}
         if self._guard_factors:
             # one drop-flag region per call, kept until step() has read the flags of its EKFAC layers
-            sizes = [lib.kfac_factor_ema_guarded_workspace_bytes(len(todo)) for todo in self._pending_alpha.values()]
+            sizes = [lib.kfac_factor_ema_diag_guarded_workspace_bytes(len(guarded)) +
+                     lib.kfac_factor_ema_guarded_workspace_bytes(len(todo)) for _, guarded, todo in split.values()]
             flags = self._ema_scratch.get(sum(sizes), self._device)
             flag_off = 0
-        for alpha, todo in self._pending_alpha.items():
-            # diagonal A factors (embeddings): their own EMA, never guarded (a window of token counts is finite)
-            diag = [l for l, which in todo if which == 'a' and l.diag_a]
+        for alpha, (diag, guarded, todo) in split.items():
             if diag:
-                todo = [(l, which) for l, which in todo if not (which == 'a' and l.diag_a)]
-                ditems = (_cabi.EmaItem * len(diag))()
-                for i, layer in enumerate(diag):
-                    ditems[i] = _cabi.EmaItem(layer._a_view.data_ptr(), layer._a_batch_view.data_ptr(),
-                                              layer.a_dim, int(not layer._has_a), 1.0 / layer._a_count)
-                    layer._has_a, layer._a_count, layer._a_pending = True, 0, False
-                _cabi.check(lib.kfac_factor_ema_diag(ditems, len(diag), alpha, stream), 'kfac_factor_ema_diag')
-                if not todo:
-                    continue
+                items = (_cabi.EmaItem * len(diag))()
+                for i, (layer, which) in enumerate(diag):
+                    items[i] = self._take_window(layer, which)
+                _cabi.check(lib.kfac_factor_ema_diag(items, len(diag), alpha, stream), 'kfac_factor_ema_diag')
+            if guarded:
+                items = (_cabi.EmaItem * len(guarded))()
+                scales = (C.c_void_p * len(guarded))()
+                for i, (layer, which) in enumerate(guarded):
+                    items[i] = self._take_window(layer, which)
+                    if layer.device_grad_scaler:
+                        scales[i] = layer._g_scale_slot.data_ptr()
+                need = lib.kfac_factor_ema_diag_guarded_workspace_bytes(len(guarded))
+                ws = flags.data_ptr() + flag_off
+                flag_off += need
+                _cabi.check(lib.kfac_factor_ema_diag_guarded(items, len(guarded), alpha, scales,
+                                                             self._skipped.data_ptr(), ws, need, stream),
+                            'kfac_factor_ema_diag_guarded')
+            if not todo:
+                continue
             items = (_cabi.EmaItem * len(todo))()
             scales = (C.c_void_p * len(todo))()      # guarded EMA: loss-scale slot of a G item, NULL otherwise
             for i, (layer, which) in enumerate(todo):
-                if which == 'a':
-                    items[i] = _cabi.EmaItem(layer._a_view.data_ptr(), layer._a_batch_view.data_ptr(),
-                                             layer.a_dim, int(not layer._has_a), 1.0 / layer._a_count)
-                    layer._has_a, layer._a_count, layer._a_pending = True, 0, False
-                else:
-                    items[i] = _cabi.EmaItem(layer._g_view.data_ptr(), layer._g_batch_view.data_ptr(),
-                                             layer.g_dim, int(not layer._has_g), 1.0 / layer._g_count)
-                    if layer.device_grad_scaler:
-                        scales[i] = layer._g_scale_slot.data_ptr()
-                    layer._has_g, layer._g_count, layer._g_pending = True, 0, False
+                items[i] = self._take_window(layer, which)
+                if which == 'g' and layer.device_grad_scaler:
+                    scales[i] = layer._g_scale_slot.data_ptr()
             if not self._guard_factors:
                 _cabi.check(lib.kfac_factor_ema(items, len(todo), alpha, stream), 'kfac_factor_ema')
                 continue
@@ -789,6 +805,19 @@ class BaseKFACPreconditioner:
             for i, (layer, which) in enumerate(todo):
                 setattr(layer, '_drop_' + which, ws + 4 * i)
         self._pending_alpha = {}
+
+    @staticmethod
+    def _take_window(layer: KFACLayer, which: str) -> _cabi.EmaItem:
+        """EMA item of the closed window of one factor; the window is consumed."""
+        if which == 'a':
+            item = _cabi.EmaItem(layer._a_view.data_ptr(), layer._a_batch_view.data_ptr(), layer.a_dim,
+                                 int(not layer._has_a), 1.0 / layer._a_count)
+            layer._has_a, layer._a_count, layer._a_pending = True, 0, False
+        else:
+            item = _cabi.EmaItem(layer._g_view.data_ptr(), layer._g_batch_view.data_ptr(), layer.g_dim,
+                                 int(not layer._has_g), 1.0 / layer._g_count)
+            layer._has_g, layer._g_count, layer._g_pending = True, 0, False
+        return item
 
     # ------------------------------------------------------------ step
     @torch.no_grad()
@@ -827,7 +856,7 @@ class BaseKFACPreconditioner:
         self._eig_event.synchronize()
         self._eig_pending = False
         word = 0
-        for slot in range(self._eig_slots):
+        for slot in self._eig_slots:
             word |= int(self._eig_status[slot])
         if word:
             why = ' and '.join(w for b, w in ((1, 'an iteration did not converge'), (2, 'non-finite eigenvalues')) if word & b)
@@ -843,8 +872,9 @@ class BaseKFACPreconditioner:
         damping = float(self.damping)
         stream = _cabi.stream_ptr()
         eig: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
-        eig_emb: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
+        eig_diag: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
         post: list[tuple[KFACLayer, str]] = []
+        snapshots = False
         for name, layer in reversed(self._layer_list()):
             mine_a = rank == self._assignment.inv_worker(name, 'A')
             mine_g = rank == self._assignment.inv_worker(name, 'G')
@@ -853,16 +883,27 @@ class BaseKFACPreconditioner:
             if mine_g and not layer._has_g:
                 raise RuntimeError('Cannot eigendecompose G before G has been computed')
             I = layer._inv
-            if layer.diag_a:
-                # embedding: A is its own eigendecomposition (Qa = I); its snapshot is the one the precondition uses
-                # until the next inverse step, like the eigenvalues of a dense A
-                if mine_a:
-                    I['da'].copy_(layer._a_view)
-                if mine_g and layer.method == ComputeMethod.EIGEN:
-                    eig_emb.append((layer._g_view, I['qg'], I['_qgT'], I['dg'], layer.g_dim))
-                elif mine_g:
-                    eig_emb.append((layer._g_view, I['_qg'], None, I['_dg'], layer.g_dim))
-                    post.append((layer, 'g_inv'))
+            if layer.diag_side:
+                # embedding / diagonal-G layer: the diagonal factor d is its own eigendecomposition; its snapshot is the
+                # one the precondition uses until the next inverse step, like the eigenvalues of a dense factor, and
+                # an entry that is not finite (or exceeds 1e15) is reported through the eigensolver's status path
+                d, f = layer.diag_side, layer.dense_side
+                mine = {'a': mine_a, 'g': mine_g}
+                if mine[d]:
+                    if self._diag_status is None:
+                        self._diag_status = torch.zeros(1, dtype=torch.int32, device=self._device)
+                    if not snapshots:
+                        self._diag_status.zero_()
+                        snapshots = True
+                    view = layer._a_view if d == 'a' else layer._g_view
+                    _cabi.check(lib.kfac_diag_snapshot(view.data_ptr(), I['d' + d].data_ptr(), view.numel(),
+                                                       self._diag_status.data_ptr(), stream), 'kfac_diag_snapshot')
+                F, n = (layer._a_view, layer.a_dim) if f == 'a' else (layer._g_view, layer.g_dim)
+                if mine[f] and layer.method == ComputeMethod.EIGEN:
+                    eig_diag.append((F, I['q' + f], I[f'_q{f}T'], I['d' + f], n))
+                elif mine[f]:
+                    eig_diag.append((F, I['_q' + f], None, I['_d' + f], n))
+                    post.append((layer, f + '_inv'))
             elif layer.method == ComputeMethod.EIGEN:
                 if layer.prediv_eigenvalues:
                     if mine_a:
@@ -887,11 +928,12 @@ class BaseKFACPreconditioner:
                 if mine_g:
                     eig.append((layer._g_view, I['_qg'], None, I['_dg'], layer.g_dim))
                     post.append((layer, 'g_inv'))
-        # the G factors of embeddings are decomposed in a call of their own: the batched solver shares its CTAs among
-        # the matrices of a call, so the other layers get the same schedule (and bits) with or without embeddings
-        batches = [b for b in (eig, eig_emb) if b]
-        if batches and self._eig_status is None:
-            self._eig_status = torch.zeros(2, dtype=torch.int32).pin_memory()
+        # the dense factors of diagonal layers are decomposed in a call of their own: the batched solver shares its
+        # CTAs among the matrices of a call, so the other layers get the same schedule (and bits) with or without
+        # embeddings and diagonal-G layers
+        batches = [b for b in (eig, eig_diag) if b]
+        if (batches or snapshots) and self._eig_status is None:
+            self._eig_status = torch.zeros(3, dtype=torch.int32).pin_memory()
             self._eig_event = torch.cuda.Event()
         for slot, batch in enumerate(batches):
             items = (_cabi.EighItem * len(batch))()
@@ -909,8 +951,11 @@ class BaseKFACPreconditioner:
             # kfac/layers/eigen.py:310; here the error surfaces one call later instead of stalling the stream)
             _cabi.check(lib.kfac_eigh_status(ws.data_ptr(), self._eig_status[slot:].data_ptr(), stream),
                         'kfac_eigh_status')
-        if batches:
-            self._eig_slots = len(batches)
+        if snapshots:
+            # status word of the diagonal snapshots: same pinned path, no host sync
+            self._eig_status[2:].copy_(self._diag_status, non_blocking=True)
+        if batches or snapshots:
+            self._eig_slots = list(range(len(batches))) + ([2] if snapshots else [])
             self._eig_event.record()
             self._eig_pending = True
         for layer, what in post:
@@ -1016,18 +1061,26 @@ class BaseKFACPreconditioner:
             w, b = self._grad_ptrs(layer)
             I = layer._inv
             ready = layer._inv_ready
-            if layer.diag_a:
+            if layer.diag_side:
+                # embedding (d = 'a') or diagonal-G layer (d = 'g'): the diagonal factor's snapshot and the dense
+                # factor f's eigendecomposition (eigen) or inverse
+                d, f = layer.diag_side, layer.dense_side
                 eigen = layer.method == ComputeMethod.EIGEN
-                need = {'da', 'qg', 'dg'} if eigen else {'da', 'g_inv'}
+                need = {'d' + d, 'q' + f, 'd' + f} if eigen else {'d' + d, f + '_inv'}
                 if not need <= ready:
-                    raise RuntimeError('The second-order data of the embedding has not been computed')
+                    kind = 'embedding' if layer.diag_a else 'diagonal-G layer'
+                    raise RuntimeError(f'The second-order data of the {kind} has not been computed')
+                ptr = {k: I[k].data_ptr() for k in need}
+                if eigen:
+                    ptr[f'q{f}T'] = I[f'_q{f}T'].data_ptr()
+                n = layer.a_dim if f == 'a' else layer.g_dim
                 items[i] = _cabi.PrecondItem(
-                    w.data_ptr(), None, _cabi.DTYPE_CODE[w.dtype], layer.g_dim, layer.a_dim,
-                    None, None, I['qg'].data_ptr() if eigen else None, I['_qgT'].data_ptr() if eigen else None,
-                    None, I['da'].data_ptr(), I['dg'].data_ptr() if eigen else None, None,
-                    None if eigen else I['g_inv'].data_ptr(),
-                    0, _cabi.ld4(layer.g_dim), 0, layer._p_store.data_ptr(), _cabi.ld4(layer.g_dim), None, 0,
-                    _cabi.KFAC_ITEM_EMBEDDING)
+                    w.data_ptr(), b.data_ptr() if b is not None else None, _cabi.DTYPE_CODE[w.dtype],
+                    layer.g_dim, layer.a_dim, ptr.get('qa'), ptr.get('qaT'), ptr.get('qg'), ptr.get('qgT'),
+                    None, ptr.get('da'), ptr.get('dg'), ptr.get('a_inv'), ptr.get('g_inv'),
+                    _cabi.ld4(n) if f == 'a' else 0, _cabi.ld4(n) if f == 'g' else 0, 0,
+                    layer._p_store.data_ptr(), _cabi.ld4(layer.p_shape[1]), None, 0,
+                    _cabi.KFAC_ITEM_EMBEDDING if layer.diag_a else _cabi.KFAC_ITEM_DIAG_G)
             elif layer.method == ComputeMethod.EIGEN:
                 ok = ('qa' in ready and 'qg' in ready and
                       ('dgda' in ready if layer.prediv_eigenvalues else ('da' in ready and 'dg' in ready)))
@@ -1044,7 +1097,7 @@ class BaseKFACPreconditioner:
                     raise RuntimeError('Cannot precondition gradient before A and G have been inverted')
                 eigen = False
 
-            if not layer.diag_a:
+            if not layer.diag_side:
                 def p(key):
                     return I[key].data_ptr() if key in ready else None
 

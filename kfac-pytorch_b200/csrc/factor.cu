@@ -7,6 +7,7 @@
 #include "common.cuh"
 
 #include <algorithm>
+#include <type_traits>
 
 namespace kfac {
 
@@ -407,8 +408,15 @@ struct EmaDiagBatch {
   int64_t elem0[41];     // prefix sums of d
   int count;
   float alpha;
+  // guarded EMA only: as in EmaBatch
+  const float* scale[40];
+  const int* dropped;
+  unsigned long long* skipped;
 };
 
+// GUARD = false: kfac_factor_ema_diag.  GUARD = true: the window is multiplied by window_unscale() as it is read, and a
+// window flagged by window_scan_kernel is dropped (factor unchanged, or ones when it is the first window; batch = 0).
+template <bool GUARD>
 __global__ void __launch_bounds__(256) ema_diag_kernel(const __grid_constant__ EmaDiagBatch eb) {
   const int64_t total = eb.elem0[eb.count];
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
@@ -417,11 +425,108 @@ __global__ void __launch_bounds__(256) ema_diag_kernel(const __grid_constant__ E
     const kfac_ema_item& it = eb.it[item];
     const int64_t v = e - eb.elem0[item];
     const float beta = (1.f - eb.alpha) * it.inv_count * 0.5f;
-    const float x = it.batch[v];
+    float x = it.batch[v];
+    if (GUARD) {
+      if (eb.dropped[item]) {
+        if (v == 0 && eb.skipped) atomicAdd(eb.skipped, 1ull);
+        if (it.first) it.factor[v] = 1.f;
+        it.batch[v] = 0.f;
+        continue;
+      }
+      x *= window_unscale(eb.scale[item]);
+    }
     const float f = it.first ? 1.f : it.factor[v];
     it.factor[v] = ema_update(eb.alpha, f, beta, x, x);   // (x + x) * 0.5 = x, as batch + batch^T on the diagonal
     it.batch[v] = 0.f;
   }
+}
+
+// ---- diagonal-G Linear layers: column sums of squares -----------------------------------------
+// The rows are split into linear_diag_chunks(rows) chunks (a function of the shape only); the thread of column group
+// j0..j0+VEC-1 and chunk c sums x[r, j]^2 over the chunk's rows -- in fp32 over 16 rows, then in fp64 -- and stores
+// the chunk's sums as fp32 partials.  A row of V elements starts at any element offset modulo the 16-byte vector
+// (V = 50257 is odd), so each thread loads the aligned vector holding its first column and, when the row is
+// misaligned, the next one, and picks its VEC columns out of the pair.  The offset is the same for every thread of
+// a row (j0 is a multiple of VEC), so the selection does not diverge.
+static int64_t linear_diag_chunks(int64_t rows) { return std::max<int64_t>(1, std::min<int64_t>(128, (rows + 31) / 32)); }
+
+template <typename T>
+__device__ __forceinline__ float vec_lane(const uint32_t (&w)[8], int i) {
+  if constexpr (sizeof(T) == 4) {
+    return __uint_as_float(w[i]);
+  } else {
+    const unsigned short h = (unsigned short)(w[i >> 1] >> ((i & 1) * 16));
+    if constexpr (std::is_same<T, __half>::value) return __half2float(__ushort_as_half(h));
+    else return __bfloat162float(__ushort_as_bfloat16(h));
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) linear_diag_kernel(const T* __restrict__ x, int64_t rows, int V,
+                                                          int64_t chunk_rows, float* __restrict__ partial) {
+  constexpr int VEC = 16 / sizeof(T);
+  const int j0 = (blockIdx.x * blockDim.x + threadIdx.x) * VEC;
+  if (j0 >= V) return;
+  const int64_t r_begin = (int64_t)blockIdx.y * chunk_rows, r_end = min(rows, r_begin + chunk_rows);
+  double acc[VEC];
+#pragma unroll
+  for (int k = 0; k < VEC; ++k) acc[k] = 0.0;
+  const bool full = j0 + VEC <= V;
+  for (int64_t r0 = r_begin; r0 < r_end; r0 += 16) {
+    float s[VEC];
+#pragma unroll
+    for (int k = 0; k < VEC; ++k) s[k] = 0.f;
+    const int64_t r1 = min(r_end, r0 + 16);
+    if (full) {
+#pragma unroll 4
+      for (int64_t r = r0; r < r1; ++r) {
+        const uintptr_t addr = reinterpret_cast<uintptr_t>(x + r * V + j0);
+        const int off = (int)((addr & 15) / sizeof(T));
+        const uint4* q = reinterpret_cast<const uint4*>(addr & ~(uintptr_t)15);
+        const uint4 lo = __ldg(q);
+        const uint4 hi = off ? __ldg(q + 1) : make_uint4(0u, 0u, 0u, 0u);   // both vectors hold a column of this row
+        const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+#pragma unroll
+        for (int o = 0; o < VEC; ++o) {
+          if (o == off) {
+#pragma unroll
+            for (int k = 0; k < VEC; ++k) { const float v = vec_lane<T>(w, o + k); s[k] = fmaf(v, v, s[k]); }
+          }
+        }
+      }
+    } else {
+      for (int64_t r = r0; r < r1; ++r)
+#pragma unroll
+        for (int k = 0; k < VEC; ++k)
+          if (j0 + k < V) { const float v = to_float<T>(x[r * V + j0 + k]); s[k] = fmaf(v, v, s[k]); }
+    }
+#pragma unroll
+    for (int k = 0; k < VEC; ++k) acc[k] += (double)s[k];
+  }
+  float* out = partial + (int64_t)blockIdx.y * V;
+#pragma unroll
+  for (int k = 0; k < VEC; ++k)
+    if (j0 + k < V) out[j0 + k] = (float)acc[k];
+}
+
+// acc[j] += scale * sum_c partial[c][j], the chunks added in order in fp64
+__global__ void linear_diag_reduce_kernel(const float* __restrict__ partial, int chunks, int V, float scale, float* acc) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < V; j += gridDim.x * blockDim.x) {
+    double t = 0.0;
+    for (int c = 0; c < chunks; ++c) t += (double)partial[(int64_t)c * V + j];
+    acc[j] = __fadd_rn(acc[j], (float)((double)scale * t));
+  }
+}
+
+// dst = src; status |= 2 when an entry is not finite or exceeds 1e15 in magnitude
+__global__ void __launch_bounds__(256) diag_snapshot_kernel(const float* __restrict__ src, float* dst, int n, int* status) {
+  bool bad = false;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = src[i];
+    dst[i] = v;
+    bad |= window_entry_bad(v, 1.f);
+  }
+  if (__syncthreads_or(bad) && threadIdx.x == 0) atomicOr(status, 2);
 }
 
 __global__ void dgda_kernel(const float* dg, const float* da, int g, int a, float damping, float* out, int ldo) {
@@ -625,6 +730,26 @@ extern "C" int kfac_factor_conv2d_gradout(const void* g, int dtype, int batch, i
   return launch_cov<true>(a, dtype, (cudaStream_t)stream);
 }
 
+// Drop flags of the guarded EMAs for the (up to 40) items it[0, count): windows of d x d floats, or of d (diag).
+static int launch_window_scan(const kfac_ema_item* it, int count, const float* const* scale, bool diag, int* dropped,
+                              cudaStream_t s) {
+  ScanBatch sb{};
+  sb.count = count;
+  sb.dropped = dropped;
+  int scan_blocks = 0;
+  for (int i = 0; i < count; ++i) {
+    sb.scale[i] = scale[i];
+    sb.batch[i] = it[i].batch;
+    sb.n[i] = diag ? (int64_t)it[i].d : (int64_t)it[i].d * it[i].d;
+    sb.first_block[i] = scan_blocks;
+    scan_blocks += (int)std::min<int64_t>(ceil_div(sb.n[i], 256 * 4 * 8), 1024);   // ~32 floats per thread
+  }
+  sb.first_block[count] = scan_blocks;
+  window_scan_kernel<<<scan_blocks, 256, 0, s>>>(sb);
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
 // EMA over up to 40 items per launch.  guard: `dropped` (one int per item, zeroed) receives the drop flags of a scan
 // launch that precedes each EMA launch.
 static int launch_ema(const kfac_ema_item* items, int count, float alpha, const float* const* loss_scale,
@@ -647,20 +772,9 @@ static int launch_ema(const kfac_ema_item* items, int count, float alpha, const 
       KFAC_LAUNCH_CHECK();
       continue;
     }
-    ScanBatch sb{};
-    sb.count = eb.count;
-    sb.dropped = dropped + base;
-    int scan_blocks = 0;
-    for (int i = 0; i < eb.count; ++i) {
-      eb.scale[i] = sb.scale[i] = loss_scale ? loss_scale[base + i] : nullptr;
-      sb.batch[i] = eb.it[i].batch;
-      sb.n[i] = (int64_t)eb.it[i].d * eb.it[i].d;
-      sb.first_block[i] = scan_blocks;
-      scan_blocks += (int)std::min<int64_t>(ceil_div(sb.n[i], 256 * 4 * 8), 1024);   // ~32 floats per thread
-    }
-    sb.first_block[eb.count] = scan_blocks;
-    window_scan_kernel<<<scan_blocks, 256, 0, s>>>(sb);
-    KFAC_LAUNCH_CHECK();
+    for (int i = 0; i < eb.count; ++i) eb.scale[i] = loss_scale ? loss_scale[base + i] : nullptr;
+    const int rc = launch_window_scan(eb.it, eb.count, eb.scale, false, dropped + base, s);
+    if (rc) return rc;
     eb.dropped = dropped + base;
     eb.skipped = skipped;
     ema_kernel<true><<<blocks, 256, 0, s>>>(eb);
@@ -720,11 +834,11 @@ extern "C" int kfac_factor_embedding(const void* idx, int index_dtype, int64_t N
   return KFAC_OK;
 }
 
-extern "C" int kfac_factor_ema_diag(const kfac_ema_item* items, int count, float alpha, void* stream) {
-  KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "items");
+// The diagonal counterpart of launch_ema (same arguments, same guard).
+static int launch_ema_diag(const kfac_ema_item* items, int count, float alpha, const float* const* loss_scale,
+                           int* dropped, unsigned long long* skipped, cudaStream_t s) {
   for (int i = 0; i < count; ++i)
     KFAC_CHECK_ARG(items[i].factor && items[i].batch && items[i].d > 0, "ema item");
-  cudaStream_t s = (cudaStream_t)stream;
   for (int base = 0; base < count; base += 40) {
     EmaDiagBatch eb{};
     eb.count = min(40, count - base);
@@ -736,9 +850,81 @@ extern "C" int kfac_factor_ema_diag(const kfac_ema_item* items, int count, float
       total += eb.it[i].d;
     }
     eb.elem0[eb.count] = total;
-    ema_diag_kernel<<<grid_for(total), 256, 0, s>>>(eb);
+    if (!dropped) {
+      ema_diag_kernel<false><<<grid_for(total), 256, 0, s>>>(eb);
+      KFAC_LAUNCH_CHECK();
+      continue;
+    }
+    for (int i = 0; i < eb.count; ++i) eb.scale[i] = loss_scale ? loss_scale[base + i] : nullptr;
+    const int rc = launch_window_scan(eb.it, eb.count, eb.scale, true, dropped + base, s);
+    if (rc) return rc;
+    eb.dropped = dropped + base;
+    eb.skipped = skipped;
+    ema_diag_kernel<true><<<grid_for(total), 256, 0, s>>>(eb);
     KFAC_LAUNCH_CHECK();
   }
+  return KFAC_OK;
+}
+
+extern "C" int kfac_factor_ema_diag(const kfac_ema_item* items, int count, float alpha, void* stream) {
+  KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "items");
+  return launch_ema_diag(items, count, alpha, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" size_t kfac_factor_ema_diag_guarded_workspace_bytes(int count) {
+  return kfac_factor_ema_guarded_workspace_bytes(count);
+}
+
+extern "C" int kfac_factor_ema_diag_guarded(const kfac_ema_item* items, int count, float alpha,
+                                            const float* const* loss_scale, unsigned long long* skipped, void* ws,
+                                            size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "items");
+  if (count == 0) return KFAC_OK;
+  for (int i = 0; i < count; ++i)   // every item is checked before anything is launched
+    KFAC_CHECK_ARG(items[i].factor && items[i].batch && items[i].d > 0, "ema item");
+  const size_t need = kfac_factor_ema_diag_guarded_workspace_bytes(count);
+  if (!ws || ws_bytes < need) {
+    set_error("factor_ema_diag_guarded: workspace too small (%zu < %zu)", ws_bytes, need);
+    return KFAC_ERR_WORKSPACE;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  KFAC_CUDA(cudaMemsetAsync(ws, 0, (size_t)count * sizeof(int), s));
+  return launch_ema_diag(items, count, alpha, loss_scale, (int*)ws, skipped, s);
+}
+
+extern "C" size_t kfac_factor_linear_diag_workspace_bytes(int64_t rows, int features) {
+  if (rows <= 0 || features <= 0) return 0;
+  return align_up((size_t)linear_diag_chunks(rows) * (size_t)features * sizeof(float), 256);
+}
+
+extern "C" int kfac_factor_linear_diag(const void* x, int dtype, int64_t rows, int features, float scale, float* acc,
+                                       void* ws, size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(acc && features > 0 && rows >= 0 && (x || rows == 0), "linear_diag args");
+  KFAC_CHECK_ARG(dtype == KFAC_F32 || dtype == KFAC_F16 || dtype == KFAC_BF16, "dtype");
+  if (rows == 0) return KFAC_OK;
+  const size_t need = kfac_factor_linear_diag_workspace_bytes(rows, features);
+  if (!ws || ws_bytes < need) {
+    set_error("factor_linear_diag: workspace too small (%zu < %zu)", ws_bytes, need);
+    return KFAC_ERR_WORKSPACE;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t chunks = linear_diag_chunks(rows), chunk_rows = (rows + chunks - 1) / chunks;
+  const int vec = dtype == KFAC_F32 ? 4 : 8;
+  const dim3 grid((unsigned)ceil_div(ceil_div(features, vec), 256), (unsigned)chunks);
+  float* partial = (float*)ws;
+  if (dtype == KFAC_F32) linear_diag_kernel<float><<<grid, 256, 0, s>>>((const float*)x, rows, features, chunk_rows, partial);
+  else if (dtype == KFAC_F16) linear_diag_kernel<__half><<<grid, 256, 0, s>>>((const __half*)x, rows, features, chunk_rows, partial);
+  else linear_diag_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, rows, features, chunk_rows, partial);
+  KFAC_LAUNCH_CHECK();
+  linear_diag_reduce_kernel<<<grid_for(features), 256, 0, s>>>(partial, (int)chunks, features, scale, acc);
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
+extern "C" int kfac_diag_snapshot(const float* src, float* dst, int n, int* status, void* stream) {
+  KFAC_CHECK_ARG(src && dst && status && n > 0, "diag_snapshot args");
+  diag_snapshot_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(src, dst, n, status);
+  KFAC_LAUNCH_CHECK();
   return KFAC_OK;
 }
 

@@ -251,15 +251,30 @@ extern "C" int kfac_transpose(const float* src, int ld_src, float* dst, int ld_d
 
 // ---- precondition: stage-wise over ALL layers ------------------------------------------------------
 // workspace: [GatherDev table][grouped-GEMM tables][ones vector][per layer: GR (g x ld4 a), T1 (a x ld4 g),
-// T2 (g x ld4 a)][slabs].  An embedding item (a = V rows of d = g) takes GR and T1 as V x ld4(d) and no T2.
+// T2 (g x ld4 a)][slabs].  A diagonal item (rows x n, see DiagItem) takes GR and T1 as rows x ld4(n) and no T2.
 struct PrecondLayout {
   size_t off_gather, off_gemm, off_ones, off_tiles, off_slab, total;
-  int ones_n;                                          // length of the ones vector (inverse method, embedding items)
+  int ones_n;                                          // length of the ones vector (inverse method, diagonal items)
   std::vector<size_t> gr, t1, t2, slab_a, slab_g;     // byte offsets per layer (slab_*: 0 = no split)
   std::vector<int> splits_a, splits_g;
 };
 
-static bool is_embedding(const kfac_precond_item& it) { return it.kind == KFAC_ITEM_EMBEDDING; }
+// An embedding item and a diagonal-G item are the same problem with the sides swapped: a gradient of `rows` x n
+// (V x d for an embedding, V x a for a diagonal-G layer), one dense factor of size n on its columns (G, resp. A:
+// basis q, its transpose qT, inverse inv, eigenvalues vcol) and one diagonal factor vrow on its rows.  P has the
+// gradient's layout, rows x n.
+struct DiagItem {
+  int rows, n;
+  const float *q, *qT, *inv, *vrow, *vcol;
+  int ldq;
+};
+
+static bool is_diag(const kfac_precond_item& it) { return it.kind != KFAC_ITEM_DENSE; }
+
+static DiagItem diag_view(const kfac_precond_item& it) {
+  if (it.kind == KFAC_ITEM_EMBEDDING) return DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg};
+  return DiagItem{it.g, it.a, it.qa, it.qaT, it.a_inv, it.dg, it.da, it.ldqa};
+}
 
 static void precond_layout(const kfac_precond_item* items, int count, PrecondLayout& L) {
   size_t off = 0;
@@ -268,16 +283,17 @@ static void precond_layout(const kfac_precond_item* items, int count, PrecondLay
   L.off_gemm = take(grouped_gemm_ws_bytes(count));
   L.ones_n = 0;
   for (int i = 0; i < count; ++i)
-    if (is_embedding(items[i])) L.ones_n = std::max(L.ones_n, items[i].g);
+    if (is_diag(items[i])) L.ones_n = std::max(L.ones_n, diag_view(items[i]).n);
   L.off_ones = L.ones_n ? take((size_t)L.ones_n * sizeof(float)) : off;
   L.off_tiles = off;
   L.gr.resize(count); L.t1.resize(count); L.t2.resize(count);
   L.slab_a.assign(count, 0); L.slab_g.assign(count, 0); L.splits_a.assign(count, 1); L.splits_g.assign(count, 1);
   for (int i = 0; i < count; ++i) {
     const size_t a = items[i].a, g = items[i].g;
-    if (is_embedding(items[i])) {
-      L.gr[i] = take(a * ld4((int)g) * sizeof(float));
-      L.t1[i] = take(a * ld4((int)g) * sizeof(float));
+    if (is_diag(items[i])) {
+      const DiagItem D = diag_view(items[i]);
+      L.gr[i] = take((size_t)D.rows * ld4(D.n) * sizeof(float));
+      L.t1[i] = take((size_t)D.rows * ld4(D.n) * sizeof(float));
       L.t2[i] = 0;
       continue;
     }
@@ -291,10 +307,12 @@ static void precond_layout(const kfac_precond_item* items, int count, PrecondLay
   // (deterministic: every replica that preconditions a layer locally must get the same bits)
   for (int i = 0; i < count; ++i) {
     const size_t a = items[i].a, g = items[i].g;
-    if (is_embedding(items[i])) {
-      // only the plain product with Qg^T (K = d) can split; the products with an epilogue run unsplit, like stage (2)
-      if (g > 1024 && items[i].n_peers == 0) {
-        L.splits_g[i] = ceil_div(g, 512); L.slab_g[i] = take((size_t)L.splits_g[i] * a * ld4((int)g) * sizeof(float));
+    if (is_diag(items[i])) {
+      // only the plain product with Q^T (K = n) can split; the products with an epilogue run unsplit, like stage (2)
+      const DiagItem D = diag_view(items[i]);
+      if (D.n > 1024 && items[i].n_peers == 0) {
+        L.splits_g[i] = ceil_div(D.n, 512);
+        L.slab_g[i] = take((size_t)L.splits_g[i] * D.rows * ld4(D.n) * sizeof(float));
       }
       continue;
     }
@@ -336,19 +354,23 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
   long long total = 0;
   for (int i = 0; i < count; ++i) {
     const kfac_precond_item& it = items[i];
-    KFAC_CHECK_ARG(it.kind == KFAC_ITEM_DENSE || it.kind == KFAC_ITEM_EMBEDDING, "precond item kind");
+    KFAC_CHECK_ARG(it.kind == KFAC_ITEM_DENSE || it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_G,
+                   "precond item kind");
     KFAC_CHECK_ARG(it.n_peers >= 0 && it.n_peers <= 7 && (it.n_peers == 0 || it.peer_P), "precond peers");
-    if (is_embedding(it)) {
-      KFAC_CHECK_ARG(it.wgrad && !it.bgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= it.g && it.ldqg >= it.g,
-                     "precond embedding item");
-      const bool ready = it.da && (method == KFAC_EIGEN ? (it.qg && it.qgT && it.dg) : it.g_inv != nullptr);
+    if (is_diag(it)) {
+      const DiagItem D = diag_view(it);
+      KFAC_CHECK_ARG(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= D.n && D.ldq >= D.n &&
+                     (it.kind != KFAC_ITEM_EMBEDDING || !it.bgrad), "precond diagonal item");
+      const bool ready = D.vrow && (method == KFAC_EIGEN ? (D.q && D.qT && D.vcol) : D.inv != nullptr);
       if (!ready) {
-        set_error("precondition: the second-order data of an embedding layer has not been computed");
+        set_error(it.kind == KFAC_ITEM_EMBEDDING
+                      ? "precondition: the second-order data of an embedding layer has not been computed"
+                      : "precondition: the second-order data of a diagonal-G layer has not been computed");
         return KFAC_ERR_NOT_READY;
       }
-      // the weight gradient (V x d) is gathered as a bias-less (V, d) layer
-      gat[i] = GatherDev{it.wgrad, nullptr, it.grad_dtype, it.a, it.g, ld4(it.g), F(L.gr[i]), total};
-      total += (long long)it.a * ld4(it.g);
+      // [wgrad | bgrad] as a (rows, n) layer: an embedding's V x d weight gradient, or a diagonal-G layer's own
+      gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, D.rows, D.n, ld4(D.n), F(L.gr[i]), total};
+      total += (long long)D.rows * ld4(D.n);
       continue;
     }
     KFAC_CHECK_ARG(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= it.a, "precond item");
@@ -383,20 +405,21 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
     st[i] = g;
   };
   auto none = [&](int i) { st[i] = GroupedGemm{}; };   // M = N = K = 0: the item has no problem in this stage
-  // 1 / (da[v] * col[j] + damping) on the rows of an embedding product: col = dg (eigen) or ones (inverse)
-  auto div_rows = [&](int i, const kfac_precond_item& it, const float* col) {
-    st[i].epi = EPI_DIV_OUTER; st[i].dg = it.da; st[i].da = col; st[i].damping = damping;
+  // 1 / (vrow[v] * col[j] + damping) on the rows of a diagonal item's product: col = vcol (eigen) or ones (inverse)
+  auto div_rows = [&](int i, const DiagItem& D, const float* col) {
+    st[i].epi = EPI_DIV_OUTER; st[i].dg = D.vrow; st[i].da = col; st[i].damping = damping;
   };
   int rc;
-  // the four (two) GEMMs of every layer form a chain; stage k of all layers is one grouped launch.  An embedding
+  // the four (two) GEMMs of every layer form a chain; stage k of all layers is one grouped launch.  A diagonal
   // item runs its first product in stage (1) (eigen) and its last in stage (4).
   for (int i = 0; i < count; ++i) {     // (1) T^T[a', r] = sum_k (QaT | Ainv)[a', k] grad[r, k]          (a x g, K = a)
     const kfac_precond_item& it = items[i];
     const int g = it.g, a = it.a;
-    if (is_embedding(it)) {             // (1e) T[v, j] = (sum_k grad[v, k] Qg[k, j]) / (da[v] dg[j] + damping)   (V x d, K = d)
+    if (is_diag(it)) {                  // (1d) T[v, j] = (sum_k grad[v, k] Q[k, j]) / (vrow[v] vcol[j] + damping)   (rows x n, K = n)
+      const DiagItem D = diag_view(it);
       if (method == KFAC_EIGEN) {
-        plain(i, F(L.gr[i]), ld4(g), it.qgT, it.ldqg, F(L.t1[i]), ld4(g), a, g, g);
-        div_rows(i, it, it.dg);
+        plain(i, F(L.gr[i]), ld4(D.n), D.qT, D.ldq, F(L.t1[i]), ld4(D.n), D.rows, D.n, D.n);
+        div_rows(i, D, D.vcol);
       } else {
         none(i);
       }
@@ -410,7 +433,7 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
     for (int i = 0; i < count; ++i) {   // (2) V2[g', a'] = (sum_k QgT[g', k] T^T[a', k]) * dgda[g', a']     (g x a, K = g)
       const kfac_precond_item& it = items[i];
       const int g = it.g, a = it.a;
-      if (is_embedding(it)) { none(i); continue; }
+      if (is_diag(it)) { none(i); continue; }
       plain(i, it.qgT, it.ldqg, F(L.t1[i]), ld4(g), F(L.t2[i]), ld4(a), g, a, g);
       if (it.dgda) { st[i].epi = EPI_MUL; st[i].E = it.dgda; st[i].lde = it.ld_dgda; }
       else { st[i].epi = EPI_DIV_OUTER; st[i].dg = it.dg; st[i].da = it.da; st[i].damping = damping; }
@@ -419,7 +442,7 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
     for (int i = 0; i < count; ++i) {   // (3) U^T[c, g'] = sum_k Qa[c, k] V2[g', k]                         (a x g, K = a)
       const kfac_precond_item& it = items[i];
       const int g = it.g, a = it.a;
-      if (is_embedding(it)) { none(i); continue; }
+      if (is_diag(it)) { none(i); continue; }
       plain(i, it.qa, it.ldqa, F(L.t2[i]), ld4(a), F(L.t1[i]), ld4(g), a, g, a);
       if (L.splits_a[i] > 1) { st[i].splits = L.splits_a[i]; st[i].slab = F(L.slab_a[i]); st[i].slab_stride = (int64_t)a * ld4(g); }
     }
@@ -428,17 +451,19 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
   for (int i = 0; i < count; ++i) {     // (4) P[r, c] = sum_k (Qg | Ginv)[r, k] U^T[c, k]                  (g x a, K = g)
     const kfac_precond_item& it = items[i];
     const int g = it.g, a = it.a;
-    if (is_embedding(it)) {
-      if (method == KFAC_EIGEN) {       // (4e) P[v, c] = sum_k T[v, k] Qg[c, k]                             (V x d, K = d)
-        plain(i, F(L.t1[i]), ld4(g), it.qg, it.ldqg, it.P, it.ldp, a, g, g);
-      } else {                          // (4e) P[v, c] = (sum_k grad[v, k] Ginv[c, k]) / (da[v] + damping)  (V x d, K = d)
-        plain(i, F(L.gr[i]), ld4(g), it.g_inv, it.ldqg, it.P, it.ldp, a, g, g);
-        div_rows(i, it, ones);
+    int64_t p_rows = g, p_ld = ld4(a);
+    if (is_diag(it)) {
+      const DiagItem D = diag_view(it);
+      if (method == KFAC_EIGEN) {       // (4d) P[v, c] = sum_k T[v, k] Q[c, k]                              (rows x n, K = n)
+        plain(i, F(L.t1[i]), ld4(D.n), D.q, D.ldq, it.P, it.ldp, D.rows, D.n, D.n);
+      } else {                          // (4d) P[v, c] = (sum_k grad[v, k] Inv[c, k]) / (vrow[v] + damping)  (rows x n, K = n)
+        plain(i, F(L.gr[i]), ld4(D.n), D.inv, D.ldq, it.P, it.ldp, D.rows, D.n, D.n);
+        div_rows(i, D, ones);
       }
+      p_rows = D.rows; p_ld = ld4(D.n);
     } else {
       plain(i, method == KFAC_EIGEN ? it.qg : it.g_inv, it.ldqg, F(L.t1[i]), ld4(g), it.P, it.ldp, g, a, g);
     }
-    const int64_t p_rows = is_embedding(it) ? a : g, p_ld = is_embedding(it) ? ld4(g) : ld4(a);
     if (it.n_peers > 0) {               // fused compute + broadcast: no split (the tiles are final when stored)
       st[i].npeer = it.n_peers;
       for (int q = 0; q < it.n_peers; ++q) st[i].peerD[q] = it.peer_P[q];

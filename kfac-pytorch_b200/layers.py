@@ -21,6 +21,7 @@ class ModuleHelper:
     """Geometry + native dispatch for one supported module type."""
 
     diagonal_a = False      # True: A is diagonal and kept as a vector (embeddings)
+    diagonal_g = False      # True: G is approximated by its diagonal and kept as a vector (diagonal_g_layers)
 
     def __init__(self, module: torch.nn.Module):
         self.module = module
@@ -301,14 +302,44 @@ class EmbeddingModuleHelper(ModuleHelper):
     accumulate_g = LinearModuleHelper.accumulate_g
 
 
+class DiagonalGLinearModuleHelper(LinearModuleHelper):
+    """torch.nn.Linear with G approximated by its diagonal (an extension beyond the reference, opt-in through
+    `diagonal_g_layers`), for layers with too many outputs for a dense G: an LM head of V = 50257 outputs would need
+    a V x V factor (10 GB) beyond the eigensolver.  diag(G) = (1/N) sum_r g_r^2 is kept as a vector of V floats
+    (`g_factor_shape` is (V,)); it is its own eigendecomposition (Qg = I).  A, the gradient and P are those of a
+    Linear layer."""
+
+    diagonal_g = True
+
+    @property
+    def g_factor_shape(self):
+        return (self.module.weight.size(0),)
+
+    def accumulate_g(self, g, acc, grad_scale, scratch=None):
+        _cabi.require_device(g)
+        g = g.detach()
+        g = g if g.is_contiguous() else g.contiguous()
+        feat = g.size(-1)
+        rows = g.numel() // feat
+        if rows == 0:
+            return
+        lib = _cabi.load()
+        need = lib.kfac_factor_linear_diag_workspace_bytes(rows, feat)
+        ws = scratch.get(need, g.device)
+        _cabi.check(lib.kfac_factor_linear_diag(g.data_ptr(), _dtype_code(g), rows, feat,
+                                                1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
+                                                ws.data_ptr(), need, _cabi.stream_ptr()), 'kfac_factor_linear_diag')
+
+
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
 CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
 EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
 
 
-def get_module_helper(module: torch.nn.Module, embeddings: bool = False) -> ModuleHelper | None:
+def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
+                      diagonal_g: bool = False) -> ModuleHelper | None:
     if isinstance(module, LINEAR_TYPES):
-        return LinearModuleHelper(module)
+        return DiagonalGLinearModuleHelper(module) if diagonal_g else LinearModuleHelper(module)
     if isinstance(module, CONV2D_TYPES):
         return Conv2dModuleHelper(module)
     if embeddings and isinstance(module, EMBEDDING_TYPES):
@@ -345,6 +376,8 @@ class KFACLayer:
         self.g_dim = module.g_factor_shape[0]
         # A is a vector of a_dim floats (embeddings); P then has the weight's layout (a x g) instead of (g x a)
         self.diag_a = module.diagonal_a
+        # G is a vector of g_dim floats (diagonal_g_layers); P keeps the dense layout (g x a)
+        self.diag_g = module.diagonal_g
         self.index = -1
         # arena views (bound by the preconditioner)
         self._a_view = self._g_view = None
@@ -404,6 +437,24 @@ class KFACLayer:
     g_inv = property(lambda self: self._inv_get('g_inv'))
 
     @property
+    def a_factor_shape(self) -> tuple[int, ...]:
+        return (self.a_dim,) if self.diag_a else (self.a_dim, self.a_dim)
+
+    @property
+    def g_factor_shape(self) -> tuple[int, ...]:
+        return (self.g_dim,) if self.diag_g else (self.g_dim, self.g_dim)
+
+    @property
+    def diag_side(self) -> str | None:
+        """'a' or 'g': the factor kept as a vector (the other one is dense); None for a dense layer."""
+        return 'a' if self.diag_a else 'g' if self.diag_g else None
+
+    @property
+    def dense_side(self) -> str | None:
+        """The dense factor of a diagonal layer ('g' for an embedding, 'a' for a diagonal-G layer)."""
+        return {'a': 'g', 'g': 'a'}.get(self.diag_side)
+
+    @property
     def p_shape(self) -> tuple[int, int]:
         """Logical shape of P: (g, a), or the weight layout (a, g) = (V, d) of an embedding."""
         return (self.a_dim, self.g_dim) if self.diag_a else (self.g_dim, self.a_dim)
@@ -420,11 +471,12 @@ class KFACLayer:
     def load_state_dict(self, state_dict: dict[str, torch.Tensor | None]) -> None:
         if 'A' not in state_dict or 'G' not in state_dict:
             raise KeyError("KFACLayer state_dict must contain keys 'A' and 'G'")
-        if self.diag_a:
-            for key, want in (('A', (self.a_dim,)), ('G', (self.g_dim, self.g_dim))):
+        if self.diag_side:
+            for key, want in (('A', self.a_factor_shape), ('G', self.g_factor_shape)):
                 t = state_dict[key]
                 if t is not None and tuple(t.shape) != want:
-                    raise ValueError(f'embedding factor {key} has shape {tuple(t.shape)}, expected {want}')
+                    kind = 'embedding' if self.diag_a else 'diagonal-G layer'
+                    raise ValueError(f'{kind} factor {key} has shape {tuple(t.shape)}, expected {want}')
         if state_dict['A'] is not None:
             self._a_view.copy_(state_dict['A'].to(torch.float32))
             self._has_a = True
@@ -435,11 +487,12 @@ class KFACLayer:
     def memory_usage(self) -> dict[str, int]:
         b = 4
         a_numel = self.a_dim if self.diag_a else self.a_dim * self.a_dim
+        g_numel = self.g_dim if self.diag_g else self.g_dim * self.g_dim
         out = {
             'a_factors': a_numel * b if self._has_a else 0,
-            'g_factors': self.g_dim * self.g_dim * b if self._has_g else 0,
+            'g_factors': g_numel * b if self._has_g else 0,
             'a_batch': a_numel * b if self._a_count else 0,
-            'g_batch': self.g_dim * self.g_dim * b if self._g_count else 0,
+            'g_batch': g_numel * b if self._g_count else 0,
             'a_inverses': 0, 'g_inverses': 0,
         }
         for k in self._inv_ready:
@@ -465,10 +518,14 @@ def any_match(query: str, patterns: list[str]) -> bool:
 
 
 def register_modules(model: torch.nn.Module, skip_layers: list[str], precondition_embeddings: bool = False,
+                     diagonal_g_layers: list[str] | None = None,
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
-    modules (not in the reference)."""
+    modules (not in the reference).  diagonal_g_layers: regexes on name and class name; a registered
+    torch.nn.Linear that matches keeps a diagonal G (not in the reference); any other registered
+    module that matches is an error."""
+    diagonal_g_layers = diagonal_g_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     for name, module in model.named_modules():
         if len(list(module.children())) != 0:
@@ -477,9 +534,13 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
             continue
         if not all(p.requires_grad for p in module.parameters()):
             continue
-        helper = get_module_helper(module, embeddings=precondition_embeddings)
+        diag_g = any_match(name, diagonal_g_layers) or any_match(module.__class__.__name__, diagonal_g_layers)
+        helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g)
         if helper is None:
             continue
+        if diag_g and not helper.diagonal_g:
+            raise ValueError(f'diagonal_g_layers matches "{name}" ({module.__class__.__name__}): only torch.nn.Linear '
+                             'layers can keep a diagonal G (add it to skip_layers or narrow the pattern)')
         assert module not in layers
         layer = KFACLayer(helper, **layer_kwargs)
         layer.index = len(layers)

@@ -34,35 +34,36 @@ def _mock_new_group(x: list[int]) -> None:
 def layer_work(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
                assignment_strategy: AssignmentStrategy) -> dict[str, dict[str, float]]:
     """Per-factor cost the KAISA placement balances: d^3 (COMPUTE) or d^2 (MEMORY) for a dense factor.  A diagonal
-    factor (an embedding's A) is never decomposed and takes V floats, so its cost is V under both strategies;
-    a V^3 cost would let one vocabulary dominate the greedy placement."""
+    factor (an embedding's A, a diagonal-G layer's G) is never decomposed and takes V floats, so its cost is V under
+    both strategies; a V^3 cost would let one vocabulary dominate the greedy placement."""
     if assignment_strategy == AssignmentStrategy.COMPUTE:
         cost = lambda n: n ** 3  # noqa: E731
     elif assignment_strategy == AssignmentStrategy.MEMORY:
         cost = lambda n: n ** 2  # noqa: E731
     else:
         raise AssertionError(f'Unknown assignment_strategy={assignment_strategy}')
-    return {name: {'A': l.a_dim if l.diag_a else cost(l.a_dim), 'G': cost(l.g_dim)} for name, l in layers.values()}
+    return {name: {'A': l.a_dim if l.diag_a else cost(l.a_dim), 'G': l.g_dim if l.diag_g else cost(l.g_dim)}
+            for name, l in layers.values()}
 
 
-def _check_embeddings(layers: dict[torch.nn.Module, tuple[str, KFACLayer]], compute_method: ComputeMethod) -> None:
-    """Reject the registered embeddings this preconditioner cannot handle."""
-    emb = [(module, name) for module, (name, l) in layers.items() if l.diag_a]
-    if not emb:
-        return
-    if compute_method == ComputeMethod.EKFAC:
-        raise ValueError(f'precondition_embeddings does not support compute_method=EKFAC (embedding "{emb[0][1]}"); '
-                         'add the embeddings to skip_layers')
-    for module, name in emb:
-        if module.sparse:
+def _check_diagonal_layers(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
+                           compute_method: ComputeMethod) -> None:
+    """Reject the registered diagonal layers (embeddings, diagonal-G layers) this preconditioner cannot handle."""
+    diag = [(module, name, l) for module, (name, l) in layers.items() if l.diag_side]
+    for module, name, l in diag:
+        kind, keyword = ('embedding', 'precondition_embeddings') if l.diag_a else ('layer', 'diagonal_g_layers')
+        if compute_method == ComputeMethod.EKFAC:
+            raise ValueError(f'{keyword} does not support compute_method=EKFAC ({kind} "{name}"); '
+                             f'add the {kind}s to skip_layers')
+        if l.diag_a and module.sparse:
             raise ValueError(f'embedding "{name}" has sparse=True: K-FAC needs a dense weight gradient '
                              '(add it to skip_layers or use sparse=False)')
-        if module.scale_grad_by_freq:
+        if l.diag_a and module.scale_grad_by_freq:
             raise ValueError(f'embedding "{name}" has scale_grad_by_freq=True: its weight gradient is then not the '
                              'one the K-FAC factors model (add it to skip_layers)')
         for other, (other_name, _) in layers.items():
             if other is not module and any(p is module.weight for p in other.parameters()):
-                raise ValueError(f'embedding "{name}" shares its weight with "{other_name}": two layers would '
+                raise ValueError(f'{kind} "{name}" shares its weight with "{other_name}": two layers would '
                                  f'precondition one gradient; add one of them to skip_layers')
 
 
@@ -81,6 +82,18 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     eigenvalue vectors (`compute_eigenvalue_outer_product` does not apply to it, so no V x d matrix is stored),
     and its damping is the one of the step that preconditions.  It cannot be combined with EKFAC, sparse
     gradients, `scale_grad_by_freq`, or a weight shared with another registered module (a tied LM head).
+
+    `diagonal_g_layers` takes regexes matched against module names and class names, like `skip_layers`.  A
+    registered `torch.nn.Linear` that matches keeps its G factor as the vector diag(G) of `out_features` floats
+    (another registered module type that matches is an error; patterns that match nothing are not).  This is for
+    layers with more outputs than the eigensolver takes (`KFAC_EIGH_MAX_N` = 8192), such as an untied LM head:
+    A stays dense, and the layer's P is
+        eigen:   P = [(grad Qa) / (dg x da + damping)] Qa^T
+        inverse: P = diag(1 / (dg + damping)) grad (A + damping I)^-1
+    with dg = diag(G) its own eigenvalues (Qg = I).  It is a different approximation of the curvature, not a faster
+    path to the same one, hence opt-in.  `compute_eigenvalue_outer_product` does not apply to such a layer (no
+    V x a matrix is stored) and its damping is the one of the step that preconditions.  It cannot be combined
+    with EKFAC or with a weight shared with another registered module.
     """
 
     def __init__(
@@ -108,6 +121,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         update_factors_in_hook: bool = True,
         loglevel: int = logging.DEBUG,
         precondition_embeddings: bool = False,
+        diagonal_g_layers: list[str] | None = None,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -188,10 +202,11 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         self.tdc = ArenaCommunicator(bucket_cap_mb=allreduce_bucket_cap_mb)
 
         kfac_layers = register_modules(
-            model, self.skip_layers, precondition_embeddings=precondition_embeddings, method=compute_method,
+            model, self.skip_layers, precondition_embeddings=precondition_embeddings,
+            diagonal_g_layers=diagonal_g_layers, method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
-        _check_embeddings(kfac_layers, compute_method)
+        _check_diagonal_layers(kfac_layers, compute_method)
         for name, kfac_layer in kfac_layers.values():
             logger.log(loglevel, f'Registered name="{name}": {repr(kfac_layer)}')
 
@@ -219,6 +234,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'skip_layers': self.skip_layers,
             'symmetry_aware': symmetry_aware,
             'precondition_embeddings': precondition_embeddings,
+            'diagonal_g_layers': diagonal_g_layers,
         }
         super().__init__(
             kfac_layers, factor_update_steps=factor_update_steps,
