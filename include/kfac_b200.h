@@ -164,6 +164,47 @@ int kfac_factor_linear_diag(const void* x, int dtype, int64_t rows, int features
  * snapshot of a diagonal factor at an inverse step, checked like a decomposed factor. */
 int kfac_diag_snapshot(const float* src, float* dst, int n, int* status, void* stream);
 
+/* Normalization layers (an extension beyond the reference, opt-in): BatchNorm1d/2d, LayerNorm and
+ * RMSNorm keep the exact per-channel Fisher block of their affine part y = s * xhat + b instead of
+ * two Kronecker factors.  Channel c is a one-input layer with bias on xhat: rows a_r = (xhat_rc, 1)
+ * (or (xhat_rc) without a bias) and g_r = dL/dy_rc, and
+ *   F_c = (1/N) sum_r g_rc^2 a_r a_r^T,  packed as k = 3 floats (F_ss, F_sb, F_bb) or k = 1 (F_ss).
+ * kfac_factor_norm: acc (C x k, row-major) += scale * sum_r g_rc^2 a_r a_r^T for one layer call:
+ *   KFAC_NORM_BATCH  x, g are (rows = B, C, S) contiguous; xhat uses the biased statistics of each
+ *                    channel over its B * S entries, plus eps;
+ *   KFAC_NORM_LAYER  x, g are (rows, C) row-major (C = the product of normalized_shape); xhat uses
+ *                    the mean and biased variance of each row, plus eps;
+ *   KFAC_NORM_RMS    as LAYER with xhat = x / sqrt(mean(x^2) + eps) (k must be 1).
+ * scale folds 1/N, the 1/S^4 of rows and gradients scaled by 1/S like a Conv2d layer's, and the
+ * AMP 1/grad_scale^2.  x (the layer INPUT: xhat does not depend on the gain) and g take any of
+ * KFAC_F32/F16/BF16 independently and are read once each (LAYER / RMS read x a second time for the
+ * row statistics).  All sums are fp64; the chunking depends on the shape only and the chunk partials
+ * are added in a fixed order, so the same input gives the same bits.  No floating-point atomics, no
+ * host sync.  ws: kfac_factor_norm_workspace_bytes(kind, rows, C, S) bytes.  Three launches (two
+ * for BATCH). */
+enum kfac_norm_kind { KFAC_NORM_BATCH = 0, KFAC_NORM_LAYER = 1, KFAC_NORM_RMS = 2 };
+size_t kfac_factor_norm_workspace_bytes(int kind, int64_t rows, int C, int64_t S);
+int kfac_factor_norm(const void* x, int x_dtype, const void* g, int g_dtype, int kind, int64_t rows,
+                     int C, int64_t S, int k, double eps, float scale, float* acc, void* ws,
+                     size_t ws_bytes, void* stream);
+/* P_c = (F_c + damping I)^-1 (wgrad[c], bgrad[c]) for every channel of every item, in fp64, written
+ * as P (C x np, ld = np, np = 2 with a bias, else 1): the weight in column 0 and the bias in the last
+ * column, the layout kfac_grad_scale / kfac_grad_update read for g = C, a = np.  F is the C x k
+ * snapshot of the running block (k = 3 with a bias, k = 1 without).  One launch over all items;
+ * every channel is one thread, so the result does not depend on the other items.
+ * ws: kfac_norm_precondition_workspace_bytes(count) bytes (the item table). */
+typedef struct kfac_norm_item {
+  const float* F;     /* C x k */
+  const void* wgrad;  /* (C), grad_dtype */
+  const void* bgrad;  /* (C) when k = 3, else NULL */
+  int grad_dtype;
+  int C, k;
+  float* P;           /* out: C x np */
+} kfac_norm_item;
+size_t kfac_norm_precondition_workspace_bytes(int count);
+int kfac_norm_precondition(const kfac_norm_item* items, int count, float damping, void* ws,
+                           size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------- eigendecomposition
  * K5: replaces torch.linalg.eigh + clamp(min=0) in
  * KFACEigenLayer.compute_{a,g}_inv (kfac/layers/eigen.py:295-344).

@@ -47,6 +47,14 @@ class PrecondItem(C.Structure):
                 ('peer_P', C.POINTER(c_void_p)), ('n_peers', c_int), ('kind', c_int)]
 
 
+KFAC_NORM_BATCH, KFAC_NORM_LAYER, KFAC_NORM_RMS = 0, 1, 2
+
+
+class NormItem(C.Structure):
+    _fields_ = [('F', c_void_p), ('wgrad', c_void_p), ('bgrad', c_void_p), ('grad_dtype', c_int),
+                ('C', c_int), ('k', c_int), ('P', c_void_p)]
+
+
 class GradItem(C.Structure):
     _fields_ = [('P', c_void_p), ('wgrad', c_void_p), ('bgrad', c_void_p),
                 ('grad_dtype', c_int), ('g', c_int), ('a', c_int), ('ldp', c_int)]
@@ -90,6 +98,11 @@ SIGNATURES = {
     'kfac_factor_linear_diag': (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_void_p, c_void_p, c_size_t,
                                         c_void_p]),
     'kfac_diag_snapshot': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    'kfac_factor_norm_workspace_bytes': (c_size_t, [c_int, c_int64, c_int, c_int64]),
+    'kfac_factor_norm': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int64, c_int, c_int64, c_int, C.c_double,
+                                 c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'kfac_norm_precondition_workspace_bytes': (c_size_t, [c_int]),
+    'kfac_norm_precondition': (c_int, [C.POINTER(NormItem), c_int, c_float, c_void_p, c_size_t, c_void_p]),
     'kfac_eigh_workspace_bytes': (c_size_t, [C.POINTER(c_int), c_int]),
     'kfac_eigh_batched': (c_int, [C.POINTER(EighItem), c_int, c_void_p, c_size_t, c_int, c_float, c_void_p]),
     'kfac_eigh_status': (c_int, [c_void_p, c_void_p, c_void_p]),

@@ -44,6 +44,13 @@ factor EMA and after the eigendecompositions of an inverse step:
     new basis without a window    S <- dg x da       (also after load_state_dict)
     every step                    dgda <- 1 / (S + damping)
 and the eigen precondition runs with that dgda.  S is not part of state_dict().
+
+Normalization layers (`norm_layers`, precondition_norms): their C x k Fisher blocks live at the end of the G block
+of the factor and batch arenas (they are complete only after backward; the A block and its overlapped all-reduce are
+those of the other layers) and take the vector EMA, guarded under a loss scale.  A tensor hook on each call's output,
+registered by a forward hook at factor steps, pairs the gradient with that call's input.  The blocks are snapshotted
+at inverse steps and every rank preconditions its normalization layers locally at every step, outside the work
+assignment and its broadcasts; kl-clip and the write-back run over all layers.
 """
 from __future__ import annotations
 
@@ -201,6 +208,7 @@ class BaseKFACPreconditioner:
         self,
         layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
         *,
+        norm_layers: dict[torch.nn.Module, tuple[str, KFACLayer]] | None = None,
         assignment: WorkAssignment,
         tdc: ArenaCommunicator,
         factor_update_steps: Callable[[int], int] | int = 1,
@@ -243,6 +251,8 @@ class BaseKFACPreconditioner:
         self._inv_update_steps = inv_update_steps
         self._kl_clip = kl_clip
         self._layers = layers
+        # normalization layers (layer.norm): outside the work assignment, preconditioned locally on every rank
+        self._norm_layers = norm_layers or {}
         self._loglevel = loglevel
         self._lr = lr
         self._tdc = tdc
@@ -260,7 +270,7 @@ class BaseKFACPreconditioner:
         self._grad_scratch = _Scratch()     # kl-clip / write-back item table + partial sums
         self._pending_alpha: dict[float, list[tuple[KFACLayer, str]]] = {}
         # with a loss scale every factor goes through the guarded EMA (non-finite windows are dropped and counted)
-        self._guard_factors = any(l.grad_scaler is not None for _, l in self._layers.values())
+        self._guard_factors = any(l.grad_scaler is not None for _, l in self._all_layer_list())
         self._ema_scratch = _Scratch()        # drop flags of the guarded EMA
         self._skipped: torch.Tensor | None = None   # device counter of dropped windows
         self._ekfac_scratch = _Scratch()      # EKFAC projections + split partials, and the update's item table
@@ -275,7 +285,11 @@ class BaseKFACPreconditioner:
         self.fused_grad_broadcast = True
         self._eig_status: torch.Tensor | None = None     # pinned host int: status word of the last eigensolver call
         self._diag_status: torch.Tensor | None = None    # device int: status of the diagonal-factor snapshots
+        self._norm_scratch = _Scratch()       # statistics of the normalization layers (autograd thread)
+        self._norm_p_scratch = _Scratch()     # item table of their precondition
 
+        for module in self._norm_layers:
+            module.register_forward_hook(self._hook_norm_output)
         for module, (_, layer) in self._layers.items():
             module.register_forward_pre_hook(self._save_input)
             if layer.diag_a:
@@ -331,11 +345,19 @@ class BaseKFACPreconditioner:
     def _layer_list(self) -> list[tuple[str, KFACLayer]]:
         return list(self._layers.values())
 
+    def _norm_list(self) -> list[tuple[str, KFACLayer]]:
+        return list(self._norm_layers.values())
+
+    def _all_layer_list(self) -> list[tuple[str, KFACLayer]]:
+        """The layers of the work assignment, then the normalization layers."""
+        return self._layer_list() + self._norm_list()
+
     def _ensure_arenas(self, device: torch.device | None = None) -> None:
         if self._arenas_ready:
             return
         if device is None:
-            device = next(iter(self._layers.values()))[1].module.device if self._layers else torch.device('cuda')
+            al = self._all_layer_list()
+            device = al[0][1].module.device if al else torch.device('cuda')
         if device.type != 'cuda':
             raise _cabi.KFACNativeError(
                 f'kfac_b200 needs the model on a CUDA (sm_90a) device, found {device}; '
@@ -345,14 +367,17 @@ class BaseKFACPreconditioner:
         ll = self._layer_list()
         # dense d x d factors (a vector of V floats for the diagonal A of an embedding or the diagonal G of a
         # diagonal-G layer), each starting 16-byte aligned
+        nl = self._norm_list()
         total = sum(_cabi.ld4(math.prod(l.a_factor_shape)) + _cabi.ld4(math.prod(l.g_factor_shape)) for _, l in ll)
+        total += sum(_cabi.ld4(math.prod(l.g_factor_shape)) for _, l in nl)
         self._factor_arena = torch.zeros(total, dtype=torch.float32, device=device)
         self._batch_arena = torch.zeros(total, dtype=torch.float32, device=device)
         # layout: all A factors, then all G factors -- the A block is complete after the forward pass and is
-        # all-reduced on its own while backward produces the G statistics
+        # all-reduced on its own while backward produces the G statistics.  The blocks of the normalization layers
+        # (no A factor) close the G block
         off = 0
         for which in ('a', 'g'):
-            for _, l in ll:
+            for _, l in ll + (nl if which == 'g' else []):
                 shape = l.a_factor_shape if which == 'a' else l.g_factor_shape
                 n = math.prod(shape)
                 setattr(l, f'_{which}_view', self._factor_arena.narrow(0, off, n).view(shape))
@@ -360,6 +385,22 @@ class BaseKFACPreconditioner:
                 off += _cabi.ld4(n)
             if which == 'a':
                 self._a_block_numel = off
+        # a normalization block is seeded with the identity (F_ss, F_sb, F_bb) = (1, 0, 1): its EMA runs with
+        # first = 0 on this seed, which gives the bits of a first window on the identity, dropped windows included
+        for _, l in nl:
+            l._g_view[:, 0] = 1.0
+            l._g_view[:, -1] = 1.0
+        # snapshots (C x k, in layer._inv['dg']) and P (C x a_dim) of the normalization layers: local to every rank
+        self._norm_arena = torch.zeros(max(1, sum(l.g_dim * (l.module.k + l.a_dim) for _, l in nl)),
+                                       dtype=torch.float32, device=device)
+        off = 0
+        for _, l in nl:
+            k, C = l.module.k, l.g_dim
+            l._inv['dg'] = self._norm_arena.narrow(0, off, C * k).view(C, k)
+            l._inv_cols['dg'] = k
+            off += C * k
+            l._p_store = l._p_view = self._norm_arena.narrow(0, off, C * l.a_dim).view(C, l.a_dim)
+            off += C * l.a_dim
         # second-order data + preconditioned gradients
         self._inv_segments, self._grad_segments = build_comm_plan(ll, self._assignment)
         inv_total = sum(s.numel for s in self._inv_segments)
@@ -434,8 +475,8 @@ class BaseKFACPreconditioner:
         if self._guard_factors or ek:
             self._skipped = torch.zeros(1, dtype=torch.int64, device=device)
         if self._guard_factors:
-            self._g_scales = torch.ones(len(ll), dtype=torch.float32, device=device)
-            for i, (_, l) in enumerate(ll):
+            self._g_scales = torch.ones(len(ll) + len(nl), dtype=torch.float32, device=device)
+            for i, (_, l) in enumerate(ll + nl):
                 l._g_scale_slot = self._g_scales.narrow(0, i, 1)
         self._vg = torch.zeros(1, dtype=torch.float64, device=device)
         self._nu = torch.ones(1, dtype=torch.float32, device=device)
@@ -542,7 +583,7 @@ class BaseKFACPreconditioner:
             # snapshots (the arena views keep changing in place)
             if self._arenas_ready:
                 self._flush_factor_updates()
-            sd['layers'] = {name: layer.state_dict() for name, layer in self._layers.values()}
+            sd['layers'] = {name: layer.state_dict() for name, layer in self._all_layer_list()}
         return sd
 
     def load_state_dict(self, state_dict: dict[str, Any], compute_inverses: bool = True) -> None:
@@ -551,10 +592,10 @@ class BaseKFACPreconditioner:
             if key in state_dict:
                 setattr(self, '_' + key, state_dict[key])
         if 'layers' in state_dict:
-            if len(state_dict['layers']) != len(self._layers):
+            if len(state_dict['layers']) != len(self._layers) + len(self._norm_layers):
                 raise ValueError('loaded state dict contains a different number of layers')
             self._ensure_arenas()
-            by_name = {name: layer for name, layer in self._layers.values()}
+            by_name = {name: layer for name, layer in self._all_layer_list()}
             for found_name, layer_state in state_dict['layers'].items():
                 if found_name in by_name:
                     by_name[found_name].load_state_dict(layer_state)
@@ -659,6 +700,42 @@ class BaseKFACPreconditioner:
         if self._update_factors_in_hook and self._mini_steps[name] % self._accumulation_steps == 0:
             self._mark_pending(layer, 'g')
 
+    def _hook_norm_output(self, module: torch.nn.Module, input_, output) -> None:
+        """Forward hook of a normalization layer.  Its statistic needs each call's input together with the gradient of
+        that call's output, so at factor steps a tensor hook on the output closes over the input; at other steps
+        nothing is registered and no reference to the input is kept.  A module called twice contributes both calls;
+        under torch.utils.checkpoint the call whose output receives a gradient is the one paired.
+
+        Memory: the input is held until the output's gradient arrives.  Outside checkpointing that costs nothing, since
+        autograd already saves the same storage for the norm's own backward.  Inside a non-reentrant checkpoint region
+        it keeps, at factor steps, inputs that checkpointing would have dropped, about one activation per norm call in
+        the region.  The recomputed call also registers a hook; it never fires and is released with the recomputed
+        graph.  With use_reentrant=True the first forward runs without grad, so nothing is held."""
+        if not module.training or not isinstance(output, torch.Tensor) or not output.requires_grad:
+            return
+        if self.steps % self.factor_update_steps != 0:
+            return
+        x = input_[0].detach()
+        output.register_hook(lambda g: self._save_norm_grad(module, x, g))
+
+    @torch.no_grad()
+    def _save_norm_grad(self, module: torch.nn.Module, x: torch.Tensor, g: torch.Tensor) -> None:
+        """Tensor hook on a normalization layer's output: accumulate the blocks of one call into the batch arena."""
+        _, layer = self._norm_layers[module]
+        self._ensure_arenas(g.device)
+        if layer.device_grad_scaler:
+            self._snapshot_loss_scale(layer)
+        eps = layer.module.eps_for(x)
+        x = cast_for_factor(x, layer.factor_dtype)
+        g = cast_for_factor(g, layer.factor_dtype)
+        layer.module.accumulate_norm(x, g, layer._g_batch_view, self._grad_scale_value(layer), eps, self._norm_scratch)
+        layer._g_count += 1
+        # a pending window stays open until it is consumed, so that every call of a module used more than once in
+        # a pass lands in the same window (the mean of its calls)
+        if (self._update_factors_in_hook and not layer._g_pending
+                and layer._g_count % self._accumulation_steps == 0):
+            self._mark_pending(layer, 'g')
+
     def _row_buffer(self, buf: torch.Tensor | None, numel: int) -> torch.Tensor:
         """Grow-only fp32 row buffer of one layer and side (EKFAC)."""
         if buf is None or buf.numel() < numel:
@@ -709,25 +786,26 @@ class BaseKFACPreconditioner:
             self._a_reduce_work = None
             self._a_block_reduced = True
         ll = self._layer_list()
-        if ll and ll[0][1].symmetry_aware:
+        al = self._all_layer_list()
+        if al and al[0][1].symmetry_aware:
             # communicate only the upper triangles (kfac/distributed.py:422-465):
             # pack -> one all-reduce of the packed arena -> mirror back
             lib = _cabi.load()
             stream = _cabi.stream_ptr()
-            # (a diagonal A -- a vector -- is passed through as it is)
+            # (a diagonal factor -- a vector -- and the blocks of a normalization layer are passed through as they are)
             def packed_numel(view, d):
                 return d if view.dim() == 1 else d * (d + 1) // 2
+            views = [v for _, l in ll for v in ((l._a_batch_view, l.a_dim), (l._g_batch_view, l.g_dim))]
+            views += [(l._g_batch_view.view(-1), l._g_batch_view.numel()) for _, l in self._norm_list()]
             if getattr(self, '_packed_arena', None) is None:
-                total = sum(packed_numel(l._a_batch_view, l.a_dim) + packed_numel(l._g_batch_view, l.g_dim)
-                            for _, l in ll)
+                total = sum(packed_numel(view, d) for view, d in views)
                 self._packed_arena = torch.empty(total, dtype=torch.float32, device=self._device)
             off = 0
             todo = []
-            for _, l in ll:
-                for view, d in ((l._a_batch_view, l.a_dim), (l._g_batch_view, l.g_dim)):
-                    n = packed_numel(view, d)
-                    todo.append((view, d, self._packed_arena.narrow(0, off, n)))
-                    off += n
+            for view, d in views:
+                n = packed_numel(view, d)
+                todo.append((view, d, self._packed_arena.narrow(0, off, n)))
+                off += n
             for view, d, packed in todo:
                 if view.dim() == 1:
                     packed.copy_(view)
@@ -755,10 +833,13 @@ class BaseKFACPreconditioner:
         stream = _cabi.stream_ptr()
         flags = None
         # diagonal factors (an embedding's A, a diagonal-G layer's G) take the EMA of vectors.  A window of token counts
-        # is finite whatever the loss scale and is never guarded; a diagonal G is guarded like every G
-        split = {alpha: ([(l, w) for l, w in todo if l.diag_side == w and not (self._guard_factors and w == 'g')],
-                         [(l, w) for l, w in todo if l.diag_side == w and self._guard_factors and w == 'g'],
-                         [(l, w) for l, w in todo if l.diag_side != w])
+        # is finite whatever the loss scale and is never guarded; a diagonal G is guarded like every G.  The blocks of a
+        # normalization layer (G side) are element-wise too and take the same path
+        def vec(l, w):
+            return l.diag_side == w or l.norm
+        split = {alpha: ([(l, w) for l, w in todo if vec(l, w) and not (self._guard_factors and w == 'g')],
+                         [(l, w) for l, w in todo if vec(l, w) and self._guard_factors and w == 'g'],
+                         [(l, w) for l, w in todo if not vec(l, w)])
                  for alpha, todo in self._pending_alpha.items()}
         if self._guard_factors:
             # one drop-flag region per call, kept until step() has read the flags of its EKFAC layers
@@ -813,6 +894,11 @@ class BaseKFACPreconditioner:
             item = _cabi.EmaItem(layer._a_view.data_ptr(), layer._a_batch_view.data_ptr(), layer.a_dim,
                                  int(not layer._has_a), 1.0 / layer._a_count)
             layer._has_a, layer._a_count, layer._a_pending = True, 0, False
+        elif layer.norm:
+            # C x k blocks as one vector; first = 0 on the identity seed the arena was given
+            item = _cabi.EmaItem(layer._g_view.data_ptr(), layer._g_batch_view.data_ptr(), layer._g_view.numel(),
+                                 0, 1.0 / layer._g_count)
+            layer._has_g, layer._g_count, layer._g_pending = True, 0, False
         else:
             item = _cabi.EmaItem(layer._g_view.data_ptr(), layer._g_batch_view.data_ptr(), layer.g_dim,
                                  int(not layer._has_g), 1.0 / layer._g_count)
@@ -832,6 +918,8 @@ class BaseKFACPreconditioner:
             for name, layer in reversed(self._layer_list()):
                 self._mini_steps[name] = 0
                 self._mark_pending(layer, 'a')
+                self._mark_pending(layer, 'g')
+            for _, layer in self._norm_list():
                 self._mark_pending(layer, 'g')
         self._flush_factor_updates()      # C1 (average of the batch statistics) + EMA
 
@@ -928,6 +1016,21 @@ class BaseKFACPreconditioner:
                 if mine_g:
                     eig.append((layer._g_view, I['_qg'], None, I['_dg'], layer.g_dim))
                     post.append((layer, 'g_inv'))
+        # normalization layers: every rank snapshots its (all-reduced) blocks, which are their own decomposition; an
+        # entry that is not finite is reported like a diagonal factor's
+        for name, layer in self._norm_list():
+            if not layer._has_g:
+                raise RuntimeError(f'Cannot snapshot the blocks of the normalization layer "{name}" before they have '
+                                   'been computed')
+            if self._diag_status is None:
+                self._diag_status = torch.zeros(1, dtype=torch.int32, device=self._device)
+            if not snapshots:
+                self._diag_status.zero_()
+                snapshots = True
+            _cabi.check(lib.kfac_diag_snapshot(layer._g_view.data_ptr(), layer._inv['dg'].data_ptr(),
+                                               layer._g_view.numel(), self._diag_status.data_ptr(), stream),
+                        'kfac_diag_snapshot')
+            layer._inv_ready.add('dg')
         # the dense factors of diagonal layers are decomposed in a call of their own: the batched solver shares its
         # CTAs among the matrices of a call, so the other layers get the same schedule (and bits) with or without
         # embeddings and diagonal-G layers
@@ -1134,20 +1237,40 @@ class BaseKFACPreconditioner:
                 for seg in self._grad_segments:
                     self._tdc.broadcast(self._p_arena.narrow(0, seg.offset, seg.numel), src=seg.src,
                                         group=seg.group)
-        for _, layer in self._layer_list():
+        self._precondition_norms()
+        for _, layer in self._all_layer_list():
             layer._grad_ready = True
+
+    def _precondition_norms(self) -> None:
+        """P_c = (F_c + damping I)^-1 grad_c of every normalization layer, on every rank, in one launch."""
+        nl = self._norm_list()
+        if not nl:
+            return
+        lib = _cabi.load()
+        items = (_cabi.NormItem * len(nl))()
+        for i, (name, layer) in enumerate(nl):
+            if 'dg' not in layer._inv_ready:
+                raise RuntimeError(f'The blocks of the normalization layer "{name}" have not been snapshotted')
+            w, b = self._grad_ptrs(layer)
+            items[i] = _cabi.NormItem(layer._inv['dg'].data_ptr(), w.data_ptr(), b.data_ptr() if b is not None else None,
+                                      _cabi.DTYPE_CODE[w.dtype], layer.g_dim, layer.module.k, layer._p_store.data_ptr())
+        need = lib.kfac_norm_precondition_workspace_bytes(len(nl))
+        ws = self._norm_p_scratch.get(need, self._device)
+        _cabi.check(lib.kfac_norm_precondition(items, len(nl), float(self.damping), ws.data_ptr(), need,
+                                               _cabi.stream_ptr()), 'kfac_norm_precondition')
 
     # K11/K12 --------------------------------------------------------------
     def _scale_and_write_back(self) -> None:
         lib = _cabi.load()
-        ll = list(reversed(self._layer_list()))
+        ll = list(reversed(self._layer_list())) + self._norm_list()    # nu over all layers
         items = (_cabi.GradItem * max(1, len(ll)))()
         for i, (_, layer) in enumerate(ll):
             w, b = self._grad_ptrs(layer)
             rows, cols = layer.p_shape          # an embedding is a bias-less (V, d) layer here
+            # ld4(cols) in the P arena, cols for a normalization layer's P
             items[i] = _cabi.GradItem(layer._p_store.data_ptr(), w.data_ptr(),
                                       b.data_ptr() if b is not None else None,
-                                      _cabi.DTYPE_CODE[w.dtype], rows, cols, _cabi.ld4(cols))
+                                      _cabi.DTYPE_CODE[w.dtype], rows, cols, layer._p_store.stride(0))
         stream = _cabi.stream_ptr()
         kl_clip = self.kl_clip
         scale_ptr = None
@@ -1169,13 +1292,13 @@ class BaseKFACPreconditioner:
             self._a_reduce_work.wait()
             self._a_reduce_work = None
         self._a_block_reduced = False
-        for _, layer in self._layers.values():
+        for _, layer in self._all_layer_list():
             layer.reset_batch()
         self._pending_alpha = {}
 
     def memory_usage(self) -> dict[str, int]:
         sizes: dict[str, int] = defaultdict(int)
-        for _, layer in self._layers.values():
+        for _, layer in self._all_layer_list():
             for key, size in layer.memory_usage().items():
                 sizes[key] += size
         if 'ekfac' in sizes and self._ekfac_scratch.buf is not None:

@@ -9,6 +9,7 @@ happens in libkfac_b200.so.
 """
 from __future__ import annotations
 
+import math
 import re
 from typing import Any, Callable
 
@@ -22,6 +23,7 @@ class ModuleHelper:
 
     diagonal_a = False      # True: A is diagonal and kept as a vector (embeddings)
     diagonal_g = False      # True: G is approximated by its diagonal and kept as a vector (diagonal_g_layers)
+    norm = False            # True: exact per-channel Fisher blocks instead of two factors (precondition_norms)
 
     def __init__(self, module: torch.nn.Module):
         self.module = module
@@ -331,19 +333,118 @@ class DiagonalGLinearModuleHelper(LinearModuleHelper):
                                                 ws.data_ptr(), need, _cabi.stream_ptr()), 'kfac_factor_linear_diag')
 
 
+class NormModuleHelper(ModuleHelper):
+    """torch.nn.BatchNorm1d / BatchNorm2d / LayerNorm / RMSNorm with an affine part (an extension beyond the
+    reference, opt-in through `precondition_norms`).
+
+    The affine part y = s * xhat + b is a depthwise layer with bias on the normalized input, so each channel c is a
+    one-input layer with rows a_r = (xhat_rc, 1) (or (xhat_rc) for a scale-only layer) and g_r = dL/dy_rc.  Instead
+    of a Kronecker factorization the exact per-channel block of the row-level Fisher is kept,
+        F_c = (1/N) sum_r g_rc^2 a_r a_r^T,
+    packed as k = 3 floats (F_ss, F_sb, F_bb) or k = 1 (`g_factor_shape` is (C, k)); there is no A factor.
+    P_c = (F_c + damping I)^-1 (weight.grad[c], bias.grad[c]) is stored as C x (1 + has_bias), the layout of a
+    Linear layer's P with the weight in column 0 and the bias in the last column.
+
+    Rows and xhat:
+      * BatchNorm2d, BatchNorm1d on (B, C, L): the B * S positions (S = H * W or L) with a_r and g_r scaled by 1/S,
+        as a Conv2d layer's rows; xhat from the biased batch statistics of each channel plus eps;
+      * BatchNorm1d on (B, C), LayerNorm, RMSNorm: every leading position is a row, unscaled, as for nn.Linear;
+        xhat from the statistics of each row over `normalized_shape` (mean and biased variance plus eps, or
+        x / sqrt(mean(x^2) + eps); when the module's eps is None, torch's: finfo(float32).eps for fp16, bf16 and
+        fp32 inputs, finfo(float64).eps for fp64 inputs).
+    xhat is recomputed from the layer input, so a gain near zero does not affect it."""
+
+    norm = True
+
+    def __init__(self, module: torch.nn.Module):
+        super().__init__(module)
+        if isinstance(module, (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d)):
+            self.kind = _cabi.KFAC_NORM_BATCH
+        elif isinstance(module, torch.nn.LayerNorm):
+            self.kind = _cabi.KFAC_NORM_LAYER
+        else:
+            self.kind = _cabi.KFAC_NORM_RMS
+
+    @property
+    def channels(self) -> int:
+        return self.module.weight.numel()
+
+    @property
+    def k(self) -> int:
+        """Packed entries of one block: 3 (F_ss, F_sb, F_bb) with a bias, 1 (F_ss) without."""
+        return 3 if self.has_bias() else 1
+
+    @property
+    def a_factor_shape(self):
+        """(width of a_r,): only its length is used (the columns of P); no A factor is stored."""
+        return (1 + int(self.has_bias()),)
+
+    @property
+    def g_factor_shape(self):
+        return (self.channels, self.k)
+
+    def get_grad(self) -> torch.Tensor:
+        g = self.module.weight.grad.reshape(-1, 1)
+        if self.has_bias():
+            g = torch.cat([g, self.module.bias.grad.reshape(-1, 1)], 1)
+        return g
+
+    def eps_for(self, x: torch.Tensor) -> float:
+        """The module's eps; for eps=None (RMSNorm) the machine epsilon of torch's computation type: that of float32
+        for fp16, bf16 and fp32 inputs, that of float64 for fp64 inputs."""
+        eps = self.module.eps
+        if eps is None:
+            return float(torch.finfo(torch.float64 if x.dtype == torch.float64 else torch.float32).eps)
+        return float(eps)
+
+    def accumulate_norm(self, x: torch.Tensor, g: torch.Tensor, acc: torch.Tensor, grad_scale: float, eps: float,
+                        scratch) -> None:
+        """acc (C x k) += the window's share of F_c for one call: x the layer input, g the gradient of its output."""
+        _cabi.require_device(x)
+        _cabi.require_device(g)
+        x = x.detach()
+        g = g.detach()
+        x = x if x.is_contiguous() else x.contiguous()
+        g = g if g.is_contiguous() else g.contiguous()
+        if x.shape != g.shape:
+            raise ValueError(f'normalization layer: input {tuple(x.shape)} and output gradient {tuple(g.shape)} differ')
+        C = self.channels
+        if x.numel() == 0:
+            return
+        if self.kind == _cabi.KFAC_NORM_BATCH:
+            if x.dim() not in (2, 3, 4) or x.size(1) != C:
+                raise ValueError(f'BatchNorm input of shape {tuple(x.shape)} for {C} channels')
+            rows, S = x.size(0), x.numel() // (x.size(0) * C)
+            # N = B * S rows, a_r and g_r scaled by 1/S (as a Conv2d layer's): 1 / (N * S^4)
+            scale = 1.0 / (float(rows) * float(S) ** 5 * grad_scale * grad_scale)
+        else:
+            rows, S = x.numel() // C, 1
+            scale = 1.0 / (float(rows) * grad_scale * grad_scale)
+        lib = _cabi.load()
+        need = lib.kfac_factor_norm_workspace_bytes(self.kind, rows, C, S)
+        ws = scratch.get(need, x.device)
+        _cabi.check(lib.kfac_factor_norm(x.data_ptr(), _dtype_code(x), g.data_ptr(), _dtype_code(g), self.kind, rows,
+                                         C, S, self.k, eps, scale, acc.data_ptr(), ws.data_ptr(), need,
+                                         _cabi.stream_ptr()), 'kfac_factor_norm')
+
+
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
 CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
 EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
+# SyncBatchNorm (global statistics), BatchNorm3d, GroupNorm and InstanceNorm* are not among them
+NORM_TYPES: tuple[type, ...] = (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d, torch.nn.LayerNorm, torch.nn.RMSNorm)
 
 
 def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
-                      diagonal_g: bool = False) -> ModuleHelper | None:
+                      diagonal_g: bool = False, norms: bool = False) -> ModuleHelper | None:
     if isinstance(module, LINEAR_TYPES):
         return DiagonalGLinearModuleHelper(module) if diagonal_g else LinearModuleHelper(module)
     if isinstance(module, CONV2D_TYPES):
         return Conv2dModuleHelper(module)
     if embeddings and isinstance(module, EMBEDDING_TYPES):
         return EmbeddingModuleHelper(module)
+    if norms and isinstance(module, NORM_TYPES) and getattr(module, 'weight', None) is not None:
+        return NormModuleHelper(module)      # affine=False / elementwise_affine=False: nothing to precondition
     return None
 
 
@@ -378,6 +479,9 @@ class KFACLayer:
         self.diag_a = module.diagonal_a
         # G is a vector of g_dim floats (diagonal_g_layers); P keeps the dense layout (g x a)
         self.diag_g = module.diagonal_g
+        # normalization layer (precondition_norms): no A factor, G holds the C x k blocks, P is C x a_dim
+        # (a_dim = 1 + has_bias); it is preconditioned locally on every rank, outside the work assignment
+        self.norm = module.norm
         self.index = -1
         # arena views (bound by the preconditioner)
         self._a_view = self._g_view = None
@@ -438,10 +542,14 @@ class KFACLayer:
 
     @property
     def a_factor_shape(self) -> tuple[int, ...]:
+        if self.norm:
+            return ()           # a normalization layer has no A factor
         return (self.a_dim,) if self.diag_a else (self.a_dim, self.a_dim)
 
     @property
     def g_factor_shape(self) -> tuple[int, ...]:
+        if self.norm:
+            return self.module.g_factor_shape
         return (self.g_dim,) if self.diag_g else (self.g_dim, self.g_dim)
 
     @property
@@ -477,6 +585,13 @@ class KFACLayer:
                 if t is not None and tuple(t.shape) != want:
                     kind = 'embedding' if self.diag_a else 'diagonal-G layer'
                     raise ValueError(f'{kind} factor {key} has shape {tuple(t.shape)}, expected {want}')
+        if self.norm:
+            if state_dict['A'] is not None:
+                raise ValueError('a normalization layer has no A factor (expected None)')
+            t = state_dict['G']
+            if t is not None and tuple(t.shape) != self.g_factor_shape:
+                raise ValueError(f'normalization layer block G has shape {tuple(t.shape)}, '
+                                 f'expected {self.g_factor_shape}')
         if state_dict['A'] is not None:
             self._a_view.copy_(state_dict['A'].to(torch.float32))
             self._has_a = True
@@ -486,8 +601,8 @@ class KFACLayer:
 
     def memory_usage(self) -> dict[str, int]:
         b = 4
-        a_numel = self.a_dim if self.diag_a else self.a_dim * self.a_dim
-        g_numel = self.g_dim if self.diag_g else self.g_dim * self.g_dim
+        a_numel = 0 if self.norm else self.a_dim if self.diag_a else self.a_dim * self.a_dim
+        g_numel = math.prod(self.g_factor_shape)
         out = {
             'a_factors': a_numel * b if self._has_a else 0,
             'g_factors': g_numel * b if self._has_g else 0,
@@ -506,6 +621,7 @@ class KFACLayer:
     def reset_batch(self) -> None:
         if self._a_batch_view is not None:
             self._a_batch_view.zero_()
+        if self._g_batch_view is not None:
             self._g_batch_view.zero_()
         self._a_count = self._g_count = 0
         self._a_pending = self._g_pending = False
@@ -518,15 +634,18 @@ def any_match(query: str, patterns: list[str]) -> bool:
 
 
 def register_modules(model: torch.nn.Module, skip_layers: list[str], precondition_embeddings: bool = False,
-                     diagonal_g_layers: list[str] | None = None,
+                     diagonal_g_layers: list[str] | None = None, precondition_norms: bool = False,
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
     modules (not in the reference).  diagonal_g_layers: regexes on name and class name; a registered
     torch.nn.Linear that matches keeps a diagonal G (not in the reference); any other registered
-    module that matches is an error."""
+    module that matches is an error.  precondition_norms: also register BatchNorm1d/2d, LayerNorm and
+    RMSNorm modules with affine parameters (not in the reference; `layer.norm`).  `layer.index` counts
+    the other layers and the normalization layers separately."""
     diagonal_g_layers = diagonal_g_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
+    counts = [0, 0]
     for name, module in model.named_modules():
         if len(list(module.children())) != 0:
             continue
@@ -535,7 +654,8 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
         if not all(p.requires_grad for p in module.parameters()):
             continue
         diag_g = any_match(name, diagonal_g_layers) or any_match(module.__class__.__name__, diagonal_g_layers)
-        helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g)
+        helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g,
+                                   norms=precondition_norms)
         if helper is None:
             continue
         if diag_g and not helper.diagonal_g:
@@ -543,6 +663,7 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
                              'layers can keep a diagonal G (add it to skip_layers or narrow the pattern)')
         assert module not in layers
         layer = KFACLayer(helper, **layer_kwargs)
-        layer.index = len(layers)
+        layer.index = counts[helper.norm]
+        counts[helper.norm] += 1
         layers[module] = (name, layer)
     return layers

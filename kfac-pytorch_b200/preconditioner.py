@@ -94,6 +94,21 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     path to the same one, hence opt-in.  `compute_eigenvalue_outer_product` does not apply to such a layer (no
     V x a matrix is stored) and its damping is the one of the step that preconditions.  It cannot be combined
     with EKFAC or with a weight shared with another registered module.
+
+    `precondition_norms=True` also registers leaf `torch.nn.BatchNorm1d`, `BatchNorm2d`, `LayerNorm` and `RMSNorm`
+    modules whose affine parameters require grad.  Their affine part y = s * xhat + b makes every channel c a one-input
+    layer with bias on the normalized input, and its exact 2 x 2 Fisher block (1 x 1 without a bias) is kept instead
+    of a Kronecker factorization:
+        F_c = (1/N) sum_r g_rc^2 (xhat_rc, 1)(xhat_rc, 1)^T,    P_c = (F_c + damping I)^-1 (dW_c, db_c)
+    with the rows of a Conv2d layer (scaled by 1/S) for BatchNorm on maps and sequences, and the rows of a Linear
+    layer otherwise; see `kfac_b200.layers.NormModuleHelper`.  The blocks follow the factor schedule (EMA,
+    `accumulation_steps`, the guarded EMA under a `grad_scaler`) and are snapshotted at inverse steps; P uses the
+    damping of the step that preconditions and is the same under every `compute_method`.  Normalization layers take
+    no part in the KAISA placement: every rank preconditions them locally from the all-reduced blocks.  Without
+    SyncBatchNorm the BatchNorm statistics are those of each rank's batch, so the all-reduced block is the mean of
+    the ranks' blocks.  At factor steps each norm call's input is held until its output's gradient arrives; inside a
+    non-reentrant `torch.utils.checkpoint` region that keeps activations the checkpointing would drop.  Not
+    registered: modules without affine parameters, SyncBatchNorm, BatchNorm3d, GroupNorm and InstanceNorm*.
     """
 
     def __init__(
@@ -122,6 +137,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         loglevel: int = logging.DEBUG,
         precondition_embeddings: bool = False,
         diagonal_g_layers: list[str] | None = None,
+        precondition_norms: bool = False,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -203,11 +219,14 @@ class KFACPreconditioner(BaseKFACPreconditioner):
 
         kfac_layers = register_modules(
             model, self.skip_layers, precondition_embeddings=precondition_embeddings,
-            diagonal_g_layers=diagonal_g_layers, method=compute_method,
+            diagonal_g_layers=diagonal_g_layers, precondition_norms=precondition_norms, method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
+        # normalization layers are preconditioned locally on every rank: the placement never sees them
+        norm_layers = {m: v for m, v in kfac_layers.items() if v[1].norm}
+        kfac_layers = {m: v for m, v in kfac_layers.items() if not v[1].norm}
         _check_diagonal_layers(kfac_layers, compute_method)
-        for name, kfac_layer in kfac_layers.values():
+        for name, kfac_layer in list(kfac_layers.values()) + list(norm_layers.values()):
             logger.log(loglevel, f'Registered name="{name}": {repr(kfac_layer)}')
 
         work = layer_work(kfac_layers, assignment_strategy)
@@ -235,9 +254,10 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'symmetry_aware': symmetry_aware,
             'precondition_embeddings': precondition_embeddings,
             'diagonal_g_layers': diagonal_g_layers,
+            'precondition_norms': precondition_norms,
         }
         super().__init__(
-            kfac_layers, factor_update_steps=factor_update_steps,
+            kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
             inv_update_steps=inv_update_steps, factor_decay=factor_decay, damping=damping,
             kl_clip=kl_clip, lr=lr, accumulation_steps=accumulation_steps,
             assignment=assignment, update_factors_in_hook=update_factors_in_hook,
