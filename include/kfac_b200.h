@@ -347,6 +347,31 @@ int kfac_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho,
                              float scale, const float* loss_scale, float* out, int ld_out,
                              void* stream);
 
+/* K-FAC-reduce rows (Eschenhagen et al., 2023) of a weight-shared layer: ONE row per example,
+ * the sum of the example's R expand rows (those of the kfac_rows_* writer with scale 1),
+ * multiplied by scale / *loss_scale (loss_scale: optional DEVICE float; NULL = 1).  Output
+ * fp32, SAMPLE-major, batch x ld_out (ld_out >= d, any value; columns [d, ld_out) are written
+ * as 0), usable as the rows of kfac_factor_linear (ld_out = d) or of the EKFAC statistics
+ * (ld_out = ld4(d)).  Every input element is read once; the sums run in fp32 over runs of at
+ * most 16 elements, then in fp64, in a fixed order (no atomics: the same bits on every run).
+ * One launch each, no workspace.
+ *   linear:   x (B, R, features) in f32/f16/bf16; the ones column is scale * R.
+ *   conv2d_input:  x NCHW; the window sums of every (b, c) plane over the output lattice,
+ *             computed from the plane (no im2col); feature order (C, kh, kw) [+ ones], the
+ *             ones column scale * Ho * Wo; zero padding, dilation and groups ignored, as in
+ *             kfac_factor_conv2d_input.  kh * kw <= 2048.
+ *   conv2d_gradout:  g (batch, C, Ho, Wo) -> the spatial sum of every (b, c) plane. */
+int kfac_reduce_rows_linear(const void* x, int dtype, int64_t B, int64_t R, int features,
+                            int append_ones, float scale, const float* loss_scale, float* out,
+                            int ld_out, void* stream);
+int kfac_reduce_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W,
+                                  int kh, int kw, int sh, int sw, int ph, int pw,
+                                  int append_ones, float scale, float* out, int ld_out,
+                                  void* stream);
+int kfac_reduce_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo,
+                                    float scale, const float* loss_scale, float* out,
+                                    int ld_out, void* stream);
+
 /* S_batch of every item, for all items together; no floating-point atomics, the same bits on
  * every run.  Launches: one grouped wgmma launch of the projections (x^2 epilogue), the K = N
  * product as one grouped launch, and the fixed-order sum of its split partials.  Extra launches:

@@ -118,6 +118,11 @@ SIGNATURES = {
     'kfac_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
     'kfac_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
                                          c_void_p]),
+    'kfac_reduce_rows_linear': (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_float, c_void_p, c_void_p,
+                                        c_int, c_void_p]),
+    'kfac_reduce_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
+    'kfac_reduce_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
+                                                c_void_p, c_int, c_void_p]),
     'kfac_ekfac_statistics_workspace_bytes': (c_size_t, [C.POINTER(EkfacStatItem), c_int]),
     'kfac_ekfac_statistics': (c_int, [C.POINTER(EkfacStatItem), c_int, c_void_p, c_size_t, c_void_p]),
     'kfac_ekfac_update_workspace_bytes': (c_size_t, [c_int]),

@@ -25,8 +25,11 @@ class ModuleHelper:
     diagonal_g = False      # True: G is approximated by its diagonal and kept as a vector (diagonal_g_layers)
     norm = False            # True: exact per-channel Fisher blocks instead of two factors (precondition_norms)
 
-    def __init__(self, module: torch.nn.Module):
+    def __init__(self, module: torch.nn.Module, reduce: bool = False):
         self.module = module
+        # K-FAC-reduce (kfac_approx='reduce', Linear and Conv2d only): a call with R > 1 shared positions per example
+        # forms its statistics from one row per example; R = 1 takes the expand path
+        self.reduce = reduce
 
     def __repr__(self) -> str:
         return f'{self.__class__.__name__}({repr(self.module)})'
@@ -110,8 +113,34 @@ def _dtype_code(t: torch.Tensor) -> int:
         raise ValueError(f'unsupported activation/gradient dtype {t.dtype}') from None
 
 
+def _reduced_factor(write: Callable[[int, int], None], B: int, d: int, scale: float, acc: torch.Tensor, scratch,
+                    device: torch.device, diagonal: bool = False) -> None:
+    """K-FAC-reduce statistics of one call: `write(ptr, ld)` writes the B reduced rows (fp32, B x d, ld = d) at the
+    start of the scratch buffer, and the existing statistics call adds scale * rows^T rows to acc (the column sums of
+    squares for a diagonal G)."""
+    lib = _cabi.load()
+    row_bytes = (B * d * 4 + 255) // 256 * 256
+    need = (lib.kfac_factor_linear_diag_workspace_bytes(B, d) if diagonal
+            else lib.kfac_factor_linear_workspace_bytes(B, d, 0))
+    buf = (scratch.get(row_bytes + need, device) if scratch is not None
+           else torch.empty(row_bytes + need, dtype=torch.uint8, device=device))
+    rows = buf.data_ptr()
+    write(rows, d)
+    ws = rows + row_bytes if need else None
+    if diagonal:
+        _cabi.check(lib.kfac_factor_linear_diag(rows, _cabi.DTYPE_CODE[torch.float32], B, d, scale, acc.data_ptr(), ws,
+                                                need, _cabi.stream_ptr()), 'kfac_factor_linear_diag')
+    else:
+        _cabi.check(lib.kfac_factor_linear(rows, _cabi.DTYPE_CODE[torch.float32], B, d, 0, scale, acc.data_ptr(), ws,
+                                           need, _cabi.stream_ptr()), 'kfac_factor_linear')
+
+
 class LinearModuleHelper(ModuleHelper):
-    """torch.nn.Linear: A = [x,1]^T[x,1]/rows, G = g^T g/rows (modules.py:100-141)."""
+    """torch.nn.Linear: A = [x,1]^T[x,1]/rows, G = g^T g/rows (modules.py:100-141).
+
+    Under K-FAC-reduce, dimension 0 is the example dimension (B; an unbatched 1-D input is one example) and every
+    dimension between it and the last is shared (R = numel / (B * features) positions).  For R > 1 each example gives
+    one row: the mean of its R A rows, and the sum of its R G rows divided by sqrt(R)."""
 
     @property
     def a_factor_shape(self):
@@ -123,10 +152,37 @@ class LinearModuleHelper(ModuleHelper):
         d = self.module.weight.size(0)
         return (d, d)
 
+    def _positions(self, t: torch.Tensor) -> tuple[int, int] | None:
+        """(B, R) when this call takes the K-FAC-reduce path (reduce on and R > 1), else None."""
+        if not self.reduce or t.numel() == 0:
+            return None
+        B = t.size(0) if t.dim() > 1 else 1
+        R = t.numel() // (B * t.size(-1))
+        return (B, R) if R > 1 else None
+
+    def _write_reduced(self, t, side, scale, loss_scale, out_ptr, ld):
+        """The reduced rows of side 'a' (the mean of the R rows, ones column included) or 'g' (their sum / sqrt(R)),
+        times scale / *loss_scale."""
+        B, R = self._positions(t)
+        ones = int(self.has_bias()) if side == 'a' else 0
+        per = 1.0 / R if side == 'a' else 1.0 / math.sqrt(R)
+        _cabi.check(_cabi.load().kfac_reduce_rows_linear(t.data_ptr(), _dtype_code(t), B, R, t.size(-1), ones,
+                                                         scale * per, loss_scale, out_ptr, ld, _cabi.stream_ptr()),
+                    'kfac_reduce_rows_linear')
+
+    def _accumulate_reduced_g(self, g, acc, grad_scale, scratch, diagonal=False):
+        B = self._positions(g)[0]
+        _reduced_factor(lambda p, ld: self._write_reduced(g, 'g', 1.0, None, p, ld), B, g.size(-1),
+                        1.0 / (B * grad_scale * grad_scale), acc, scratch, g.device, diagonal=diagonal)
+
     def accumulate_a(self, x, acc, scratch):
         _cabi.require_device(x)
         x = x.detach()
         x = x if x.is_contiguous() else x.contiguous()
+        if self._positions(x) is not None:
+            _reduced_factor(lambda p, ld: self._write_reduced(x, 'a', 1.0, None, p, ld), x.size(0),
+                            x.size(-1) + int(self.has_bias()), 1.0 / x.size(0), acc, scratch, x.device)
+            return
         feat = x.size(-1)
         rows = x.numel() // feat
         lib = _cabi.load()
@@ -141,6 +197,8 @@ class LinearModuleHelper(ModuleHelper):
         _cabi.require_device(g)
         g = g.detach()
         g = g if g.is_contiguous() else g.contiguous()
+        if self.reduce and self._positions(g) is not None:     # (an embedding shares this method, never reduced)
+            return self._accumulate_reduced_g(g, acc, grad_scale, scratch)
         feat = g.size(-1)
         rows = g.numel() // feat
         lib = _cabi.load()
@@ -152,24 +210,29 @@ class LinearModuleHelper(ModuleHelper):
                                            _cabi.stream_ptr()), 'kfac_factor_linear')
 
     def num_rows_a(self, x):
-        return x.numel() // x.size(-1)
+        pos = self._positions(x)
+        return pos[0] if pos is not None else x.numel() // x.size(-1)
 
     num_rows_g = num_rows_a
 
-    def _write_rows(self, t, out, ones, scale, loss_scale):
+    def _write_rows(self, t, out, side, scale, loss_scale):
         _cabi.require_device(t)
         t = t.detach()
         t = t if t.is_contiguous() else t.contiguous()
         feat = t.size(-1)
+        ones = int(self.has_bias()) if side == 'a' else 0
+        if self._positions(t) is not None:
+            self._write_reduced(t, side, scale, loss_scale, out.data_ptr(), _cabi.ld4(feat + ones))
+            return
         _cabi.check(_cabi.load().kfac_rows_linear(t.data_ptr(), _dtype_code(t), t.numel() // feat, feat, ones, scale,
                                                   loss_scale, out.data_ptr(), _cabi.ld4(feat + ones),
                                                   _cabi.stream_ptr()), 'kfac_rows_linear')
 
     def write_rows_a(self, x, out):
-        self._write_rows(x, out, int(self.has_bias()), 1.0, None)
+        self._write_rows(x, out, 'a', 1.0, None)
 
     def write_rows_g(self, g, out, grad_scale, loss_scale):
-        self._write_rows(g, out, 0, 1.0 / grad_scale, loss_scale)
+        self._write_rows(g, out, 'g', 1.0 / grad_scale, loss_scale)
 
 
 class Conv2dModuleHelper(ModuleHelper):
@@ -195,6 +258,26 @@ class Conv2dModuleHelper(ModuleHelper):
         return (B, Cc, H, W, m.kernel_size[0], m.kernel_size[1], m.stride[0], m.stride[1],
                 pad[0], pad[1])
 
+    @staticmethod
+    def _spatial(geo) -> int:
+        B, _, H, W, kh, kw, sh, sw, ph, pw = geo
+        return ((H + 2 * ph - kh) // sh + 1) * ((W + 2 * pw - kw) // sw + 1)
+
+    # K-FAC-reduce (S = Ho * Wo > 1): one row per example, the mean of its S A rows and the sum of its S G rows divided
+    # by sqrt(S), the rows carrying the 1/S of the expand rows: scale 1/S^2 (A) and S^-3/2 (G) on the plain sums
+    def _write_reduced_a(self, x, geo, out_ptr, ld):
+        S = self._spatial(geo)
+        _cabi.check(_cabi.load().kfac_reduce_rows_conv2d_input(x.data_ptr(), _dtype_code(x), *geo, int(self.has_bias()),
+                                                               1.0 / (float(S) * S), out_ptr, ld, _cabi.stream_ptr()),
+                    'kfac_reduce_rows_conv2d_input')
+
+    def _write_reduced_g(self, g, scale, loss_scale, out_ptr, ld):
+        B, Cc, Ho, Wo = g.shape
+        _cabi.check(_cabi.load().kfac_reduce_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, Ho, Wo,
+                                                                 scale / float(Ho * Wo) ** 1.5, loss_scale, out_ptr,
+                                                                 ld, _cabi.stream_ptr()),
+                    'kfac_reduce_rows_conv2d_gradout')
+
     def accumulate_a(self, x, acc, scratch):
         _cabi.require_device(x)
         x = x.detach()
@@ -203,6 +286,10 @@ class Conv2dModuleHelper(ModuleHelper):
         B, Cc, H, W, kh, kw, sh, sw, ph, pw = geo
         Ho, Wo = (H + 2 * ph - kh) // sh + 1, (W + 2 * pw - kw) // sw + 1
         S = Ho * Wo
+        if self.reduce and S > 1:
+            _reduced_factor(lambda p, ld: self._write_reduced_a(x, geo, p, ld), B, self.a_factor_shape[0], 1.0 / B,
+                            acc, scratch, x.device)
+            return
         # rows = B*S, features scaled by 1/S  ->  scale = 1/(B*S) * 1/S^2   (modules.py:170-178)
         scale = 1.0 / (float(B) * float(S) ** 3)
         lib = _cabi.load()
@@ -219,6 +306,10 @@ class Conv2dModuleHelper(ModuleHelper):
         g = g if g.is_contiguous() else g.contiguous()
         B, Cc, Ho, Wo = g.shape
         S = Ho * Wo
+        if self.reduce and S > 1:
+            _reduced_factor(lambda p, ld: self._write_reduced_g(g, 1.0, None, p, ld), B, Cc,
+                            1.0 / (B * grad_scale * grad_scale), acc, scratch, g.device)
+            return
         scale = 1.0 / (float(B) * float(S) ** 3 * grad_scale * grad_scale)
         lib = _cabi.load()
         need = lib.kfac_factor_conv2d_gradout_workspace_bytes(B, Cc, Ho, Wo) if scratch is not None else 0
@@ -230,11 +321,13 @@ class Conv2dModuleHelper(ModuleHelper):
                     'kfac_factor_conv2d_gradout')
 
     def num_rows_a(self, x):
-        B, _, H, W, kh, kw, sh, sw, ph, pw = self._geometry(x)
-        return B * ((H + 2 * ph - kh) // sh + 1) * ((W + 2 * pw - kw) // sw + 1)
+        geo = self._geometry(x)
+        S = self._spatial(geo)
+        return geo[0] if self.reduce and S > 1 else geo[0] * S
 
     def num_rows_g(self, g):
-        return g.size(0) * g.size(2) * g.size(3)
+        S = g.size(2) * g.size(3)
+        return g.size(0) if self.reduce and S > 1 else g.size(0) * S
 
     def write_rows_a(self, x, out):
         _cabi.require_device(x)
@@ -244,6 +337,9 @@ class Conv2dModuleHelper(ModuleHelper):
         B, Cc, H, W, kh, kw, sh, sw, ph, pw = geo
         S = ((H + 2 * ph - kh) // sh + 1) * ((W + 2 * pw - kw) // sw + 1)
         ones = int(self.has_bias())
+        if self.reduce and S > 1:
+            self._write_reduced_a(x, geo, out.data_ptr(), _cabi.ld4(Cc * kh * kw + ones))
+            return
         # rows scaled by 1/S, the ones column included (modules.py:170-178)
         _cabi.check(_cabi.load().kfac_rows_conv2d_input(x.data_ptr(), _dtype_code(x), *geo, ones, 1.0 / S, out.data_ptr(),
                                                         _cabi.ld4(Cc * kh * kw + ones), _cabi.stream_ptr()),
@@ -254,6 +350,9 @@ class Conv2dModuleHelper(ModuleHelper):
         g = g.detach()
         g = g if g.is_contiguous() else g.contiguous()
         B, Cc, Ho, Wo = g.shape
+        if self.reduce and Ho * Wo > 1:
+            self._write_reduced_g(g, 1.0 / grad_scale, loss_scale, out.data_ptr(), _cabi.ld4(Cc))
+            return
         _cabi.check(_cabi.load().kfac_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, Ho, Wo,
                                                           1.0 / (float(Ho * Wo) * grad_scale), loss_scale,
                                                           out.data_ptr(), _cabi.ld4(Cc), _cabi.stream_ptr()),
@@ -321,6 +420,8 @@ class DiagonalGLinearModuleHelper(LinearModuleHelper):
         _cabi.require_device(g)
         g = g.detach()
         g = g if g.is_contiguous() else g.contiguous()
+        if self._positions(g) is not None:      # diag(G) of the reduced rows
+            return self._accumulate_reduced_g(g, acc, grad_scale, scratch, diagonal=True)
         feat = g.size(-1)
         rows = g.numel() // feat
         if rows == 0:
@@ -436,11 +537,13 @@ NORM_TYPES: tuple[type, ...] = (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d, torc
 
 
 def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
-                      diagonal_g: bool = False, norms: bool = False) -> ModuleHelper | None:
+                      diagonal_g: bool = False, norms: bool = False, reduce: bool = False) -> ModuleHelper | None:
+    """reduce: K-FAC-reduce statistics for Linear (dense and diagonal-G) and Conv2d layers; embeddings and
+    normalization layers keep their own statistics."""
     if isinstance(module, LINEAR_TYPES):
-        return DiagonalGLinearModuleHelper(module) if diagonal_g else LinearModuleHelper(module)
+        return (DiagonalGLinearModuleHelper if diagonal_g else LinearModuleHelper)(module, reduce=reduce)
     if isinstance(module, CONV2D_TYPES):
-        return Conv2dModuleHelper(module)
+        return Conv2dModuleHelper(module, reduce=reduce)
     if embeddings and isinstance(module, EMBEDDING_TYPES):
         return EmbeddingModuleHelper(module)
     if norms and isinstance(module, NORM_TYPES) and getattr(module, 'weight', None) is not None:
@@ -635,14 +738,16 @@ def any_match(query: str, patterns: list[str]) -> bool:
 
 def register_modules(model: torch.nn.Module, skip_layers: list[str], precondition_embeddings: bool = False,
                      diagonal_g_layers: list[str] | None = None, precondition_norms: bool = False,
+                     kfac_approx: str = 'expand',
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
     modules (not in the reference).  diagonal_g_layers: regexes on name and class name; a registered
     torch.nn.Linear that matches keeps a diagonal G (not in the reference); any other registered
     module that matches is an error.  precondition_norms: also register BatchNorm1d/2d, LayerNorm and
-    RMSNorm modules with affine parameters (not in the reference; `layer.norm`).  `layer.index` counts
-    the other layers and the normalization layers separately."""
+    RMSNorm modules with affine parameters (not in the reference; `layer.norm`).  kfac_approx: 'expand'
+    or 'reduce' (K-FAC-reduce statistics for the Linear and Conv2d layers; not in the reference).
+    `layer.index` counts the other layers and the normalization layers separately."""
     diagonal_g_layers = diagonal_g_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     counts = [0, 0]
@@ -655,7 +760,7 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
             continue
         diag_g = any_match(name, diagonal_g_layers) or any_match(module.__class__.__name__, diagonal_g_layers)
         helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g,
-                                   norms=precondition_norms)
+                                   norms=precondition_norms, reduce=kfac_approx == 'reduce')
         if helper is None:
             continue
         if diag_g and not helper.diagonal_g:

@@ -109,6 +109,21 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     the ranks' blocks.  At factor steps each norm call's input is held until its output's gradient arrives; inside a
     non-reentrant `torch.utils.checkpoint` region that keeps activations the checkpointing would drop.  Not
     registered: modules without affine parameters, SyncBatchNorm, BatchNorm3d, GroupNorm and InstanceNorm*.
+
+    `kfac_approx` chooses the statistics of weight-sharing layers (Eschenhagen et al., 2023): a `torch.nn.Linear`
+    on (B, ..., d) applies one weight at R = numel / (B * d) positions of each example, a `torch.nn.Conv2d` at
+    R = Ho * Wo.  'expand' (the default, the reference's) makes every position a row.  'reduce' makes every example
+    one row, formed from the expand rows:
+        x_b = (1/R) sum_t x_bt,    g_b = R^-1/2 sum_t g_bt,    A = (1/B) sum_b x_b x_b^T,    G = (1/B) sum_b g_b g_b^T
+    (the conv rows keep their 1/Ho*Wo scaling, the ones column is averaged with the others).  It is a different
+    approximation, R times cheaper to form: A is unchanged when x is constant over the positions and E[G] is unchanged
+    when g is uncorrelated over them, so `damping` and `kl_clip` keep their scale.  It applies to dense and
+    diagonal-G Linear layers and to Conv2d layers; a call with R = 1 (a Linear on (B, d), a conv with a 1 x 1 output)
+    takes the expand path with the same bits.  Dimension 0 is always the example dimension: a sequence-first input
+    (T, B, d) is read as T examples.  Embeddings (their diagonal A counts one-hot rows) and normalization layers (their
+    exact per-channel blocks) keep their statistics.  Under EKFAC the reduced rows are the rows of S_batch (N = B),
+    which makes it the per-example EKFAC of George et al.  Factor shapes do not change, so checkpoints move between the
+    two settings.
     """
 
     def __init__(
@@ -138,9 +153,12 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         precondition_embeddings: bool = False,
         diagonal_g_layers: list[str] | None = None,
         precondition_norms: bool = False,
+        kfac_approx: str = 'expand',
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
+        if kfac_approx not in ('expand', 'reduce'):
+            raise ValueError(f"kfac_approx must be 'expand' or 'reduce', got {kfac_approx!r}")
         if isinstance(assignment_strategy, str):
             assignment_strategy = AssignmentStrategy[assignment_strategy.upper()]
         if isinstance(compute_method, str):
@@ -219,7 +237,8 @@ class KFACPreconditioner(BaseKFACPreconditioner):
 
         kfac_layers = register_modules(
             model, self.skip_layers, precondition_embeddings=precondition_embeddings,
-            diagonal_g_layers=diagonal_g_layers, precondition_norms=precondition_norms, method=compute_method,
+            diagonal_g_layers=diagonal_g_layers, precondition_norms=precondition_norms, kfac_approx=kfac_approx,
+            method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
         # normalization layers are preconditioned locally on every rank: the placement never sees them
@@ -255,6 +274,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'precondition_embeddings': precondition_embeddings,
             'diagonal_g_layers': diagonal_g_layers,
             'precondition_norms': precondition_norms,
+            'kfac_approx': kfac_approx,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
