@@ -66,6 +66,14 @@ size_t kfac_factor_linear_workspace_bytes(int64_t rows, int features, int append
 int kfac_factor_linear(const void* x, int dtype, int64_t rows, int features,
                        int append_ones, float scale, float* acc, void* ws,
                        size_t ws_bytes, void* stream);
+/* The same statistics on rows with a row stride ld >= features (elements), e.g. a column block
+ * of a packed projection's gradient.  ld == features gives the bits of kfac_factor_linear, and a
+ * column block the bits of kfac_factor_linear on a contiguous copy of it. */
+size_t kfac_factor_linear_strided_workspace_bytes(int64_t rows, int features, int64_t ld,
+                                                  int append_ones);
+int kfac_factor_linear_strided(const void* x, int dtype, int64_t rows, int features, int64_t ld,
+                               int append_ones, float scale, float* acc, void* ws,
+                               size_t ws_bytes, void* stream);
 
 /* replaces Conv2dModuleHelper._extract_patches + get_a_factor
  * (kfac/layers/modules.py:170-178,210-237).  x is NCHW; feature order
@@ -339,6 +347,10 @@ int kfac_grad_update(const kfac_grad_item* items, int count, const float* scale,
  * The feature order is that of the factor calls above.  No workspace. */
 int kfac_rows_linear(const void* x, int dtype, int64_t rows, int features, int append_ones,
                      float scale, const float* loss_scale, float* out, int ld_out, void* stream);
+/* kfac_rows_linear on input rows with a row stride ld >= features (elements) */
+int kfac_rows_linear_strided(const void* x, int dtype, int64_t rows, int features, int64_t ld,
+                             int append_ones, float scale, const float* loss_scale, float* out,
+                             int ld_out, void* stream);
 int kfac_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W, int kh,
                            int kw, int sh, int sw, int ph, int pw, int append_ones, float scale,
                            float* out, int ld_out, void* stream);
@@ -364,6 +376,14 @@ int kfac_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho,
 int kfac_reduce_rows_linear(const void* x, int dtype, int64_t B, int64_t R, int features,
                             int append_ones, float scale, const float* loss_scale, float* out,
                             int ld_out, void* stream);
+/* kfac_reduce_rows_linear with the element (b, t, f) at x[b * example_stride + t * position_stride
+ * + f]: a sequence-first (R, B, ld) tensor, or a column block of one, is reduced in place with
+ * example_stride = ld and position_stride = B * ld.  The contiguous strides (R * features,
+ * features) give the bits of kfac_reduce_rows_linear. */
+int kfac_reduce_rows_linear_strided(const void* x, int dtype, int64_t B, int64_t R, int features,
+                                    int64_t example_stride, int64_t position_stride,
+                                    int append_ones, float scale, const float* loss_scale,
+                                    float* out, int ld_out, void* stream);
 int kfac_reduce_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W,
                                   int kh, int kw, int sh, int sw, int ph, int pw,
                                   int append_ones, float scale, float* out, int ld_out,

@@ -79,6 +79,9 @@ SIGNATURES = {
     'kfac_launch_count': (C.c_longlong, []),
     'kfac_factor_linear_workspace_bytes': (c_size_t, [c_int64, c_int, c_int]),
     'kfac_factor_linear': (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'kfac_factor_linear_strided_workspace_bytes': (c_size_t, [c_int64, c_int, c_int64, c_int]),
+    'kfac_factor_linear_strided': (c_int, [c_void_p, c_int, c_int64, c_int, c_int64, c_int, c_float, c_void_p, c_void_p,
+                                           c_size_t, c_void_p]),
     'kfac_factor_conv2d_input_workspace_bytes': (c_size_t, [c_int] * 11),
     'kfac_factor_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     'kfac_factor_conv2d_gradout_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
@@ -115,11 +118,15 @@ SIGNATURES = {
     'kfac_grad_scale': (c_int, [C.POINTER(GradItem), c_int, c_float, c_float, c_void_p, c_size_t, c_void_p, c_void_p]),
     'kfac_grad_update': (c_int, [C.POINTER(GradItem), c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     'kfac_rows_linear': (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p]),
+    'kfac_rows_linear_strided': (c_int, [c_void_p, c_int, c_int64, c_int, c_int64, c_int, c_float, c_void_p, c_void_p,
+                                         c_int, c_void_p]),
     'kfac_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
     'kfac_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
                                          c_void_p]),
     'kfac_reduce_rows_linear': (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_float, c_void_p, c_void_p,
                                         c_int, c_void_p]),
+    'kfac_reduce_rows_linear_strided': (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int64, c_int64, c_int,
+                                                c_float, c_void_p, c_void_p, c_int, c_void_p]),
     'kfac_reduce_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
     'kfac_reduce_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                                 c_void_p, c_int, c_void_p]),

@@ -67,7 +67,7 @@ from kfac_b200 import _cabi
 from kfac_b200.assignment import WorkAssignment
 from kfac_b200.distributed import ArenaCommunicator, get_rank
 from kfac_b200.enums import ComputeMethod
-from kfac_b200.layers import KFACLayer, cast_for_factor
+from kfac_b200.layers import AttentionProjectionHelper, KFACLayer, cast_for_factor
 
 logger = logging.getLogger(__name__)
 
@@ -288,9 +288,15 @@ class BaseKFACPreconditioner:
         self._norm_scratch = _Scratch()       # statistics of the normalization layers (autograd thread)
         self._norm_p_scratch = _Scratch()     # item table of their precondition
 
+        # attention projections (precondition_attention): attention module -> {'q', 'k', 'v', 'o'} -> the helper that
+        # keys the projection's layer; their statistics arrive through taps inside the attention's forward
+        self._attention_taps: dict[torch.nn.Module, dict[str, AttentionProjectionHelper]] = {}
         for module in self._norm_layers:
             module.register_forward_hook(self._hook_norm_output)
         for module, (_, layer) in self._layers.items():
+            if isinstance(module, AttentionProjectionHelper):
+                self._attention_taps.setdefault(module.attn, {})[module.which[0]] = module
+                continue
             module.register_forward_pre_hook(self._save_input)
             if layer.diag_a:
                 # the input of an embedding (the indices) never requires grad: a full backward hook would fire through
@@ -628,15 +634,30 @@ class BaseKFACPreconditioner:
         else:
             layer._g_scale_slot.fill_(scaler._init_scale if scaler.is_enabled() else 1.0)
 
-    @torch.no_grad()
     def _save_input(self, module: torch.nn.Module, input_: tuple[torch.Tensor, ...]) -> None:
         """Forward pre-hook: accumulate A statistics (base_preconditioner.py:437-457)."""
         if not module.training:
             return
         if self.steps % self.factor_update_steps != 0:
             return
-        name, layer = self._layers[module]
-        x = input_[0]
+        self._accumulate_input(*self._layers[module], input_[0])
+
+    def _active_attention_taps(self, module: torch.nn.Module) -> dict[str, AttentionProjectionHelper] | None:
+        """The registered projections of an attention module at a factor step (its forward taps them), else None."""
+        if self.steps % self.factor_update_steps != 0:
+            return None
+        return self._attention_taps.get(module)
+
+    def _attention_input(self, key: AttentionProjectionHelper, x: torch.Tensor) -> None:
+        """A tap of an attention projection: x is its input, (L, B, features)."""
+        self._accumulate_input(*self._layers[key], x)
+
+    def _attention_grad_output(self, key: AttentionProjectionHelper, g: torch.Tensor) -> None:
+        """G tap of an attention projection: g is the gradient of its output, (L, B, E), possibly a column block."""
+        self._accumulate_grad_output(*self._layers[key], g)
+
+    @torch.no_grad()
+    def _accumulate_input(self, name: str, layer: KFACLayer, x: torch.Tensor) -> None:
         self._ensure_arenas(x.device)
         if layer.method == ComputeMethod.EKFAC and layer._rows_n_a:
             raise RuntimeError(f'EKFAC: {name} was called a second time in one factor window (one forward and one '
@@ -667,15 +688,17 @@ class BaseKFACPreconditioner:
         if module.training and output.requires_grad:
             output.register_hook(lambda g: self._save_grad_output(module, None, g))
 
-    @torch.no_grad()
     def _save_grad_output(self, module: torch.nn.Module, grad_input, grad_output) -> None:
         """Full backward hook: accumulate G statistics (base_preconditioner.py:459-479)."""
         if not module.training:
             return
         if self.steps % self.factor_update_steps != 0:
             return
-        name, layer = self._layers[module]
         g = grad_output if isinstance(grad_output, torch.Tensor) else grad_output[0]
+        self._accumulate_grad_output(*self._layers[module], g)
+
+    @torch.no_grad()
+    def _accumulate_grad_output(self, name: str, layer: KFACLayer, g: torch.Tensor) -> None:
         self._ensure_arenas(g.device)
         if layer.method == ComputeMethod.EKFAC and layer._rows_n_g:
             raise RuntimeError(f'EKFAC: {name} was called a second time in one factor window (one forward and one '

@@ -77,17 +77,18 @@ __global__ void __launch_bounds__(256) rows_im2col_kernel(RowsArgs a) {
   }
 }
 
-// out[r][f] = s * x[r][f] (f < feat), s (f == feat, ones), 0 up to ld: a (rows, feat) input is already sample-major
+// out[r][f] = s * x[r][f] (f < feat), s (f == feat, ones), 0 up to ld: a (rows, feat) input with row stride ldx is
+// already sample-major
 template <typename T>
-__global__ void __launch_bounds__(256) rows_linear_kernel(const void* xin, int64_t rows, int feat, int ones, float scale,
-                                                          const float* loss_scale, float* out, int64_t ld) {
+__global__ void __launch_bounds__(256) rows_linear_kernel(const void* xin, int64_t rows, int feat, int64_t ldx, int ones,
+                                                          float scale, const float* loss_scale, float* out, int64_t ld) {
   const T* __restrict__ x = reinterpret_cast<const T*>(xin);
   const float s = row_scale(scale, loss_scale);
   const int64_t total = rows * ld;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = idx / ld;
     const int f = (int)(idx - r * ld);
-    out[idx] = f < feat ? to_float<T>(x[r * feat + f]) * s : (f == feat && ones ? s : 0.f);
+    out[idx] = f < feat ? to_float<T>(x[r * ldx + f]) * s : (f == feat && ones ? s : 0.f);
   }
 }
 
@@ -275,20 +276,31 @@ static size_t upd_table_bytes(int count) { return align_up(sizeof(UpdDev) * (siz
 using namespace kfac;
 
 // ---------------------------------------------------------------------------------------------------- row writers
-extern "C" int kfac_rows_linear(const void* x, int dtype, int64_t rows, int features, int append_ones, float scale,
-                                const float* loss_scale, float* out, int ld_out, void* stream) {
+extern "C" int kfac_rows_linear_strided(const void* x, int dtype, int64_t rows, int features, int64_t ldx,
+                                        int append_ones, float scale, const float* loss_scale, float* out, int ld_out,
+                                        void* stream) {
   KFAC_CHECK_ARG(x && out, "null pointer");
   KFAC_CHECK_ARG(rows > 0 && rows < (1ll << 31) && features > 0, "dims");
+  KFAC_CHECK_ARG(ldx >= features, "ld");
   KFAC_CHECK_ARG(ld_out >= features + (append_ones ? 1 : 0) && ld_out % 4 == 0, "ld_out");
   cudaStream_t s = (cudaStream_t)stream;
   const int ones = append_ones ? 1 : 0;
   const int grid = grid_for(rows * ld_out);
-  if (dtype == KFAC_F32) rows_linear_kernel<float><<<grid, 256, 0, s>>>(x, rows, features, ones, scale, loss_scale, out, ld_out);
-  else if (dtype == KFAC_F16) rows_linear_kernel<__half><<<grid, 256, 0, s>>>(x, rows, features, ones, scale, loss_scale, out, ld_out);
-  else if (dtype == KFAC_BF16) rows_linear_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(x, rows, features, ones, scale, loss_scale, out, ld_out);
+  if (dtype == KFAC_F32)
+    rows_linear_kernel<float><<<grid, 256, 0, s>>>(x, rows, features, ldx, ones, scale, loss_scale, out, ld_out);
+  else if (dtype == KFAC_F16)
+    rows_linear_kernel<__half><<<grid, 256, 0, s>>>(x, rows, features, ldx, ones, scale, loss_scale, out, ld_out);
+  else if (dtype == KFAC_BF16)
+    rows_linear_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(x, rows, features, ldx, ones, scale, loss_scale, out, ld_out);
   else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   KFAC_LAUNCH_CHECK();
   return KFAC_OK;
+}
+
+extern "C" int kfac_rows_linear(const void* x, int dtype, int64_t rows, int features, int append_ones, float scale,
+                                const float* loss_scale, float* out, int ld_out, void* stream) {
+  return kfac_rows_linear_strided(x, dtype, rows, features, features, append_ones, scale, loss_scale, out, ld_out,
+                                  stream);
 }
 
 extern "C" int kfac_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W, int kh, int kw, int sh,

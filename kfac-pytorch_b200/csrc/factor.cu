@@ -232,9 +232,11 @@ __global__ void __launch_bounds__(256) im2col_kernel(Im2colArgs a) {
   *reinterpret_cast<float4*>(a.out + (int64_t)f * a.ld + r4) = make_float4(v[0], v[1], v[2], v[3]);
 }
 
-// X (rows x feat, sample-major, any dtype) -> out (feat [+1 ones row]) x ld, feature-major fp32
+// X (rows x feat, sample-major with row stride ldx >= feat, any dtype) -> out (feat [+1 ones row]) x ld, feature-major
+// fp32
 template <typename T>
-__global__ void to_feature_major_kernel(const void* xin, int64_t rows, int feat, int ones, float* out, int64_t ld) {
+__global__ void to_feature_major_kernel(const void* xin, int64_t rows, int feat, int64_t ldx, int ones, float* out,
+                                        int64_t ld) {
   __shared__ float tile[32][33];
   const T* __restrict__ x = reinterpret_cast<const T*>(xin);
   const int64_t r0 = (int64_t)blockIdx.x * 32;
@@ -242,7 +244,7 @@ __global__ void to_feature_major_kernel(const void* xin, int64_t rows, int feat,
   for (int i = threadIdx.y; i < 32; i += 8) {
     const int64_t r = r0 + i;
     const int f = f0 + threadIdx.x;
-    tile[i][threadIdx.x] = (r < rows && f < feat) ? to_float<T>(x[r * feat + f]) : 0.f;
+    tile[i][threadIdx.x] = (r < rows && f < feat) ? to_float<T>(x[r * ldx + f]) : 0.f;
   }
   __syncthreads();
   for (int i = threadIdx.y; i < 32; i += 8) {
@@ -595,11 +597,17 @@ extern "C" size_t kfac_factor_linear_workspace_bytes(int64_t rows, int features,
   return CovWs(linear_pack_bytes(rows, features, append_ones), features + (append_ones ? 1 : 0), rows, 1).total;
 }
 
-extern "C" int kfac_factor_linear(const void* x, int dtype, int64_t rows, int features,
-                                  int append_ones, float scale, float* acc, void* ws, size_t ws_bytes,
-                                  void* stream) {
+extern "C" size_t kfac_factor_linear_strided_workspace_bytes(int64_t rows, int features, int64_t ld, int append_ones) {
+  (void)ld;   // the packed matrix and the split partials do not depend on the input's row stride
+  return kfac_factor_linear_workspace_bytes(rows, features, append_ones);
+}
+
+extern "C" int kfac_factor_linear_strided(const void* x, int dtype, int64_t rows, int features, int64_t ldx,
+                                          int append_ones, float scale, float* acc, void* ws, size_t ws_bytes,
+                                          void* stream) {
   KFAC_CHECK_ARG(x && acc, "null pointer");
   KFAC_CHECK_ARG(rows >= 0 && rows < (1ll << 31) && features > 0, "dims");
+  KFAC_CHECK_ARG(ldx >= features, "ld");
   const CovWs w(linear_pack_bytes(rows, features, append_ones), features + (append_ones ? 1 : 0), rows, 1);
   if (w.pack > 0 && ws && ws_bytes >= w.pack) {
     // tall activations (tokens x hidden): transpose once into a feature-major matrix
@@ -608,9 +616,9 @@ extern "C" int kfac_factor_linear(const void* x, int dtype, int64_t rows, int fe
     const int64_t ld = (rows + 3) / 4 * 4;
     const int ones = append_ones ? 1 : 0;
     dim3 grid(ceil_div(ld, 32), ceil_div(features + ones, 32));
-    if (dtype == KFAC_F32) to_feature_major_kernel<float><<<grid, dim3(32, 8), 0, st>>>(x, rows, features, ones, (float*)ws, ld);
-    else if (dtype == KFAC_F16) to_feature_major_kernel<__half><<<grid, dim3(32, 8), 0, st>>>(x, rows, features, ones, (float*)ws, ld);
-    else if (dtype == KFAC_BF16) to_feature_major_kernel<__nv_bfloat16><<<grid, dim3(32, 8), 0, st>>>(x, rows, features, ones, (float*)ws, ld);
+    if (dtype == KFAC_F32) to_feature_major_kernel<float><<<grid, dim3(32, 8), 0, st>>>(x, rows, features, ldx, ones, (float*)ws, ld);
+    else if (dtype == KFAC_F16) to_feature_major_kernel<__half><<<grid, dim3(32, 8), 0, st>>>(x, rows, features, ldx, ones, (float*)ws, ld);
+    else if (dtype == KFAC_BF16) to_feature_major_kernel<__nv_bfloat16><<<grid, dim3(32, 8), 0, st>>>(x, rows, features, ldx, ones, (float*)ws, ld);
     else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
     KFAC_LAUNCH_CHECK();
     CovArgs a{};
@@ -619,9 +627,15 @@ extern "C" int kfac_factor_linear(const void* x, int dtype, int64_t rows, int fe
     return launch_cov<true>(a, KFAC_F32, st);
   }
   CovArgs a{};
-  a.x = x; a.ld = features; a.batch_stride = 0; a.rows = (int)rows; a.batch = 1;
+  a.x = x; a.ld = ldx; a.batch_stride = 0; a.rows = (int)rows; a.batch = 1;
   a.feat = features; a.ones = append_ones ? 1 : 0; a.scale = scale; a.acc = acc; a.slab = w.slab(ws, ws_bytes);
   return launch_cov<false>(a, dtype, (cudaStream_t)stream);
+}
+
+extern "C" int kfac_factor_linear(const void* x, int dtype, int64_t rows, int features,
+                                  int append_ones, float scale, float* acc, void* ws, size_t ws_bytes,
+                                  void* stream) {
+  return kfac_factor_linear_strided(x, dtype, rows, features, features, append_ones, scale, acc, ws, ws_bytes, stream);
 }
 
 static bool conv_in_place(int C, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw) {

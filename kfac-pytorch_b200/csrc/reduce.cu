@@ -19,25 +19,25 @@ __device__ __forceinline__ double out_scale(float scale, const float* loss_scale
   return loss_scale ? (double)scale / (double)*loss_scale : (double)scale;
 }
 
-// out[b][f] = s * sum_t x[b][t][f] (f < feat), s * R (f == feat, ones), 0 up to ld.  The 8 warps of a CTA take the rows
-// t = warp, warp + 8, ...; their fp64 partials are added in warp order.
+// out[b][f] = s * sum_t x[b sb + t st + f] (f < feat), s * R (f == feat, ones), 0 up to ld.  The 8 warps of a CTA take
+// the rows t = warp, warp + 8, ...; their fp64 partials are added in warp order.
 template <typename T>
-__global__ void __launch_bounds__(256) reduce_linear_kernel(const T* __restrict__ x, int64_t R, int feat, int ones,
-                                                            float scale, const float* loss_scale, float* out,
-                                                            int64_t ld, int tiles) {
+__global__ void __launch_bounds__(256) reduce_linear_kernel(const T* __restrict__ x, int64_t R, int feat, int64_t sb,
+                                                            int64_t st, int ones, float scale, const float* loss_scale,
+                                                            float* out, int64_t ld, int tiles) {
   __shared__ double part[8][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t b = blockIdx.x / tiles;
   const int64_t f = (int64_t)(blockIdx.x % tiles) * 32 + lane;
   double acc = 0.0;
   if (f < feat) {
-    const T* __restrict__ p = x + b * R * feat + f;
+    const T* __restrict__ p = x + b * sb + f;
     for (int64_t t0 = warp; t0 < R; t0 += 8 * RUN) {
       float s = 0.f;
 #pragma unroll
       for (int k = 0; k < RUN; ++k) {
         const int64_t t = t0 + 8 * k;
-        if (t < R) s += to_float<T>(p[t * feat]);
+        if (t < R) s += to_float<T>(p[t * st]);
       }
       acc += (double)s;
     }
@@ -161,26 +161,38 @@ __global__ void __launch_bounds__(256) reduce_planes_kernel(const T* __restrict_
 
 using namespace kfac;
 
-extern "C" int kfac_reduce_rows_linear(const void* x, int dtype, int64_t B, int64_t R, int features, int append_ones,
-                                       float scale, const float* loss_scale, float* out, int ld_out, void* stream) {
+extern "C" int kfac_reduce_rows_linear_strided(const void* x, int dtype, int64_t B, int64_t R, int features,
+                                               int64_t example_stride, int64_t position_stride, int append_ones,
+                                               float scale, const float* loss_scale, float* out, int ld_out,
+                                               void* stream) {
   KFAC_CHECK_ARG(x && out, "null pointer");
   KFAC_CHECK_ARG(B > 0 && R > 0 && features > 0, "dims");
+  KFAC_CHECK_ARG(example_stride >= 0 && position_stride >= 0, "strides");
   const int ones = append_ones ? 1 : 0;
   KFAC_CHECK_ARG(ld_out >= features + ones, "ld_out");
   const int tiles = ceil_div(ld_out, 32);
   KFAC_CHECK_ARG(B * tiles < (1ll << 31), "grid");
   cudaStream_t s = (cudaStream_t)stream;
   const unsigned grid = (unsigned)(B * tiles);
+  const int64_t sb = example_stride, st = position_stride;
   if (dtype == KFAC_F32)
-    reduce_linear_kernel<float><<<grid, 256, 0, s>>>((const float*)x, R, features, ones, scale, loss_scale, out, ld_out, tiles);
+    reduce_linear_kernel<float><<<grid, 256, 0, s>>>((const float*)x, R, features, sb, st, ones, scale, loss_scale, out,
+                                                     ld_out, tiles);
   else if (dtype == KFAC_F16)
-    reduce_linear_kernel<__half><<<grid, 256, 0, s>>>((const __half*)x, R, features, ones, scale, loss_scale, out, ld_out, tiles);
+    reduce_linear_kernel<__half><<<grid, 256, 0, s>>>((const __half*)x, R, features, sb, st, ones, scale, loss_scale, out,
+                                                      ld_out, tiles);
   else if (dtype == KFAC_BF16)
-    reduce_linear_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, R, features, ones, scale, loss_scale,
-                                                              out, ld_out, tiles);
+    reduce_linear_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, R, features, sb, st, ones, scale,
+                                                             loss_scale, out, ld_out, tiles);
   else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   KFAC_LAUNCH_CHECK();
   return KFAC_OK;
+}
+
+extern "C" int kfac_reduce_rows_linear(const void* x, int dtype, int64_t B, int64_t R, int features, int append_ones,
+                                       float scale, const float* loss_scale, float* out, int ld_out, void* stream) {
+  return kfac_reduce_rows_linear_strided(x, dtype, B, R, features, R * features, features, append_ones, scale,
+                                         loss_scale, out, ld_out, stream);
 }
 
 extern "C" int kfac_reduce_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W, int kh, int kw,

@@ -16,6 +16,7 @@ from typing import Any, Callable
 import torch
 
 from kfac_b200 import _cabi
+from kfac_b200.attention import KFACMultiheadAttention
 
 
 class ModuleHelper:
@@ -529,6 +530,161 @@ class NormModuleHelper(ModuleHelper):
                                          _cabi.stream_ptr()), 'kfac_factor_norm')
 
 
+def _strided_rows(t: torch.Tensor, ordered: bool) -> tuple[torch.Tensor, int]:
+    """(rows tensor, row stride) of a (..., features) tensor whose rows are `features` unit-stride elements at one row
+    stride: the tensor itself, or -- when `ordered` is False, i.e. only sums over the rows are formed -- its
+    transpose(0, 1) (the contiguous batch-first input behind a sequence-first view).  Any other layout is made
+    contiguous."""
+    feat = t.size(-1)
+    for c in ((t,) if ordered or t.dim() != 3 else (t, t.transpose(0, 1))):
+        if c.stride(-1) != 1 and feat > 1:
+            continue
+        try:
+            r = c.view(-1, feat)
+        except RuntimeError:
+            continue
+        ld = r.stride(0) if r.size(0) > 1 else feat
+        if ld >= feat:
+            return r, ld
+    return t.contiguous().view(-1, feat), feat
+
+
+class AttentionProjectionHelper(LinearModuleHelper):
+    """One projection of a `torch.nn.MultiheadAttention` (an extension beyond the reference, opt-in through
+    `precondition_attention`), preconditioned as the `torch.nn.Linear` it is mathematically:
+
+        'q'    Linear(E, E) on query        rows [0, E) of in_proj_weight / in_proj_bias, or q_proj_weight
+        'k'    Linear(kdim, E) on key       rows [E, 2E), or k_proj_weight
+        'v'    Linear(vdim, E) on value     rows [2E, 3E), or v_proj_weight
+        'out'  Linear(E, E) on the concatenated head outputs: out_proj.weight / out_proj.bias
+
+    The gradients are row-slice views, contiguous like a Linear layer's, so the write-back runs in place.  The
+    statistics come from taps inside `kfac_b200.attention.KFACMultiheadAttention`, which see (L, B, features) tensors
+    in the sequence-first layout of torch's attention path: views of the batch-first input, column blocks of a packed
+    projection's gradient.  They are read in place through the strided native entry points.  Under K-FAC-reduce the
+    example dimension is the attention's batch dimension B (dimension 1 here); an unbatched call is one example."""
+
+    def __init__(self, attn: torch.nn.MultiheadAttention, which: str, reduce: bool = False):
+        super().__init__(attn, reduce=reduce)
+        self.attn = attn
+        self.which = which
+        E = attn.embed_dim
+        if which == 'out':
+            self.weight, self.bias, self.rows = attn.out_proj.weight, attn.out_proj.bias, None
+        else:
+            i = 'qkv'.index(which)
+            self.rows = (i * E, (i + 1) * E)
+            self.weight = attn.in_proj_weight if attn._qkv_same_embed_dim else getattr(attn, f'{which}_proj_weight')
+            self.bias = attn.in_proj_bias
+
+    def __repr__(self) -> str:
+        return f'{self.__class__.__name__}({self.which}, in_features={self.in_features}, out_features={self.attn.embed_dim})'
+
+    def parameters(self):
+        """The projection's own parameters (the whole packed in_proj_weight / in_proj_bias for q, k and v)."""
+        return iter([p for p in (self.weight, self.bias) if p is not None])
+
+    @property
+    def in_features(self) -> int:
+        return {'q': self.attn.embed_dim, 'k': self.attn.kdim, 'v': self.attn.vdim, 'out': self.attn.embed_dim}[self.which]
+
+    def has_bias(self) -> bool:
+        return self.bias is not None
+
+    @property
+    def a_factor_shape(self):
+        d = self.in_features + int(self.has_bias())
+        return (d, d)
+
+    @property
+    def g_factor_shape(self):
+        return (self.attn.embed_dim, self.attn.embed_dim)
+
+    def _slice(self, t: torch.Tensor | None, weight: bool) -> torch.Tensor | None:
+        if t is None or self.rows is None or (weight and not self.attn._qkv_same_embed_dim):
+            return t
+        return t[self.rows[0]:self.rows[1]]
+
+    def get_weight_grad(self):
+        return self._slice(self.weight.grad, True)
+
+    def get_bias_grad(self):
+        return self._slice(self.bias.grad, False)
+
+    def get_grad(self):
+        g = self.get_weight_grad()
+        return torch.cat([g, self.get_bias_grad().view(-1, 1)], 1) if self.has_bias() else g
+
+    def _positions(self, t):
+        """(B, R) = (t.size(1), t.size(0)) of an (L, B, features) tap under K-FAC-reduce with R > 1, else None."""
+        if not self.reduce or t.numel() == 0 or t.size(0) == 1:
+            return None
+        return (t.size(1), t.size(0))
+
+    def _write_reduced(self, t, side, scale, loss_scale, out_ptr, ld):
+        B, R = self._positions(t)
+        if t.stride(-1) != 1:
+            t = t.contiguous()
+        ones = int(self.has_bias()) if side == 'a' else 0
+        per = 1.0 / R if side == 'a' else 1.0 / math.sqrt(R)
+        _cabi.check(_cabi.load().kfac_reduce_rows_linear_strided(
+            t.data_ptr(), _dtype_code(t), B, R, t.size(-1), t.stride(1), t.stride(0), ones, scale * per, loss_scale,
+            out_ptr, ld, _cabi.stream_ptr()), 'kfac_reduce_rows_linear_strided')
+
+    def _accumulate(self, t, acc, ones, grad_scale, scratch):
+        r, ld = _strided_rows(t, ordered=False)
+        rows, feat = r.shape
+        if rows == 0:
+            return
+        lib = _cabi.load()
+        need = lib.kfac_factor_linear_strided_workspace_bytes(rows, feat, ld, ones)
+        ws = scratch.get(need, t.device) if (need and scratch is not None) else None
+        _cabi.check(lib.kfac_factor_linear_strided(r.data_ptr(), _dtype_code(r), rows, feat, ld, ones,
+                                                   1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
+                                                   ws.data_ptr() if ws is not None else None,
+                                                   need if ws is not None else 0, _cabi.stream_ptr()),
+                    'kfac_factor_linear_strided')
+
+    def accumulate_a(self, x, acc, scratch):
+        _cabi.require_device(x)
+        x = x.detach()
+        if self._positions(x) is not None:
+            _reduced_factor(lambda p, ld: self._write_reduced(x, 'a', 1.0, None, p, ld), x.size(1),
+                            x.size(-1) + int(self.has_bias()), 1.0 / x.size(1), acc, scratch, x.device)
+            return
+        self._accumulate(x, acc, int(self.has_bias()), 1.0, scratch)
+
+    def accumulate_g(self, g, acc, grad_scale, scratch=None):
+        _cabi.require_device(g)
+        g = g.detach()
+        if self._positions(g) is not None:
+            B = g.size(1)
+            _reduced_factor(lambda p, ld: self._write_reduced(g, 'g', 1.0, None, p, ld), B, g.size(-1),
+                            1.0 / (B * grad_scale * grad_scale), acc, scratch, g.device)
+            return
+        self._accumulate(g, acc, 0, grad_scale, scratch)
+
+    def num_rows_a(self, x):
+        pos = self._positions(x)
+        return pos[0] if pos is not None else x.numel() // x.size(-1)
+
+    num_rows_g = num_rows_a
+
+    def _write_rows(self, t, out, side, scale, loss_scale):
+        _cabi.require_device(t)
+        t = t.detach()
+        ones = int(self.has_bias()) if side == 'a' else 0
+        if self._positions(t) is not None:
+            self._write_reduced(t, side, scale, loss_scale, out.data_ptr(), _cabi.ld4(t.size(-1) + ones))
+            return
+        # the A and G rows of EKFAC are paired row by row: both in the (L, B) order of the taps
+        r, ld = _strided_rows(t, ordered=True)
+        rows, feat = r.shape
+        _cabi.check(_cabi.load().kfac_rows_linear_strided(r.data_ptr(), _dtype_code(r), rows, feat, ld, ones, scale,
+                                                          loss_scale, out.data_ptr(), _cabi.ld4(feat + ones),
+                                                          _cabi.stream_ptr()), 'kfac_rows_linear_strided')
+
+
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
 CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
 EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
@@ -738,7 +894,7 @@ def any_match(query: str, patterns: list[str]) -> bool:
 
 def register_modules(model: torch.nn.Module, skip_layers: list[str], precondition_embeddings: bool = False,
                      diagonal_g_layers: list[str] | None = None, precondition_norms: bool = False,
-                     kfac_approx: str = 'expand',
+                     kfac_approx: str = 'expand', precondition_attention: bool = False,
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
@@ -747,12 +903,24 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     module that matches is an error.  precondition_norms: also register BatchNorm1d/2d, LayerNorm and
     RMSNorm modules with affine parameters (not in the reference; `layer.norm`).  kfac_approx: 'expand'
     or 'reduce' (K-FAC-reduce statistics for the Linear and Conv2d layers; not in the reference).
+    precondition_attention: register every torch.nn.MultiheadAttention as four projections named
+    `{name}.q_proj`, `.k_proj`, `.v_proj` and `.out_proj`, keyed by their AttentionProjectionHelper
+    (not in the reference); the `out_proj` leaf of an attention is then never registered as a Linear.
     `layer.index` counts the other layers and the normalization layers separately."""
     diagonal_g_layers = diagonal_g_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     counts = [0, 0]
+    out_projs = ({id(m.out_proj) for m in model.modules() if isinstance(m, torch.nn.MultiheadAttention)}
+                 if precondition_attention else set())
     for name, module in model.named_modules():
-        if len(list(module.children())) != 0:
+        if precondition_attention and isinstance(module, torch.nn.MultiheadAttention):
+            for helper in _attention_projections(name, module, skip_layers, diagonal_g_layers, kfac_approx):
+                layer = KFACLayer(helper, **layer_kwargs)
+                layer.index = counts[0]
+                counts[0] += 1
+                layers[helper] = (f'{name}.{helper.which}_proj', layer)
+            continue
+        if len(list(module.children())) != 0 or id(module) in out_projs:
             continue
         if any_match(name, skip_layers) or any_match(module.__class__.__name__, skip_layers):
             continue
@@ -771,4 +939,47 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
         layer.index = counts[helper.norm]
         counts[helper.norm] += 1
         layers[module] = (name, layer)
+    # a projection weight that another registered module also owns would have its gradient preconditioned twice (the
+    # projections of one attention share in_proj_weight / in_proj_bias by design)
+    owners: dict[int, list[tuple[Any, str]]] = {}
+    for key, (name, _) in layers.items():
+        owner = key.attn if isinstance(key, AttentionProjectionHelper) else key
+        for p in key.parameters():
+            owners.setdefault(id(p), []).append((owner, name))
+    for key, (name, _) in layers.items():
+        if isinstance(key, AttentionProjectionHelper):
+            for p in key.parameters():
+                other = next((n for o, n in owners[id(p)] if o is not key.attn), None)
+                if other is not None:
+                    raise ValueError(f'attention projection "{name}" shares a weight with "{other}": two layers '
+                                     'would precondition one gradient; add one of them to skip_layers')
     return layers
+
+
+def _attention_projections(name: str, module: torch.nn.MultiheadAttention, skip_layers: list[str],
+                           diagonal_g_layers: list[str], kfac_approx: str) -> list[AttentionProjectionHelper]:
+    """The registered projections of one attention: none when skip_layers matches its name or class or one of its
+    parameters is frozen, else those whose name `{name}.{q,k,v,out}_proj` skip_layers does not match."""
+    cls = module.__class__.__name__
+    if any_match(name, skip_layers) or any_match(cls, skip_layers):
+        return []
+    if not all(p.requires_grad for p in module.parameters()):
+        return []
+    if type(module) not in (torch.nn.MultiheadAttention, KFACMultiheadAttention):
+        raise ValueError(f'precondition_attention: "{name}" is a {cls}, a subclass of torch.nn.MultiheadAttention '
+                         'whose forward cannot be tapped; add it to skip_layers')
+    for flag, what in ((module.bias_k is not None, 'add_bias_kv=True'), (module.add_zero_attn, 'add_zero_attn=True')):
+        if flag:
+            raise ValueError(f'precondition_attention does not support {what} (attention "{name}"); add it to '
+                             'skip_layers')
+    helpers = []
+    for which in ('q', 'k', 'v', 'out'):
+        pname = f'{name}.{which}_proj'
+        if any_match(pname, skip_layers):
+            continue
+        if any_match(name, diagonal_g_layers) or any_match(cls, diagonal_g_layers) or any_match(pname,
+                                                                                               diagonal_g_layers):
+            raise ValueError(f'diagonal_g_layers matches the attention projection "{pname}": attention projections '
+                             'cannot keep a diagonal G (add it to skip_layers or narrow the pattern)')
+        helpers.append(AttentionProjectionHelper(module, which, reduce=kfac_approx == 'reduce'))
+    return helpers

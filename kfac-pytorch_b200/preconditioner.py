@@ -17,6 +17,7 @@ from typing import Any, Callable
 import torch
 import torch.distributed as dist
 
+from kfac_b200 import attention
 from kfac_b200.assignment import KAISAAssignment
 from kfac_b200.base_preconditioner import BaseKFACPreconditioner
 from kfac_b200.distributed import ArenaCommunicator, get_rank, get_world_size
@@ -124,6 +125,20 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     exact per-channel blocks) keep their statistics.  Under EKFAC the reduced rows are the rows of S_batch (N = B),
     which makes it the per-example EKFAC of George et al.  Factor shapes do not change, so checkpoints move between the
     two settings.
+
+    `precondition_attention=True` registers every `torch.nn.MultiheadAttention` whose parameters all require grad, and
+    which `skip_layers` does not match by name or class, as four K-FAC layers `{name}.q_proj`, `.k_proj`, `.v_proj`
+    and `.out_proj`, each preconditioned exactly like the `torch.nn.Linear` it is mathematically (rows [0, E), [E, 2E)
+    and [2E, 3E) of `in_proj_weight` / `in_proj_bias` or the separate `q/k/v_proj_weight`, and `out_proj`); see
+    `kfac_b200.layers.AttentionProjectionHelper`.  A `skip_layers` pattern matching one projection name leaves that
+    projection's rows of the gradient untouched.  The `out_proj` leaf of an attention is never registered as a Linear
+    (torch's attention never calls its forward, so its hooks could not fire).  To see the projections, the constructor
+    sets the class of each registered attention to `kfac_b200.attention.KFACMultiheadAttention`, a subclass that adds
+    no state and overrides only `forward`: at the factor steps in training it runs a restatement of torch's training
+    path with the taps, and the stock forward otherwise.  Under `kfac_approx='reduce'` the example dimension is the
+    attention's batch dimension (an unbatched call is one example).  Refused with a ValueError: `add_bias_kv`,
+    `add_zero_attn`, subclasses of `torch.nn.MultiheadAttention`, a `diagonal_g_layers` pattern matching an attention or
+    a projection, and a projection weight shared with another registered module.
     """
 
     def __init__(
@@ -154,6 +169,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         diagonal_g_layers: list[str] | None = None,
         precondition_norms: bool = False,
         kfac_approx: str = 'expand',
+        precondition_attention: bool = False,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -238,7 +254,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         kfac_layers = register_modules(
             model, self.skip_layers, precondition_embeddings=precondition_embeddings,
             diagonal_g_layers=diagonal_g_layers, precondition_norms=precondition_norms, kfac_approx=kfac_approx,
-            method=compute_method,
+            precondition_attention=precondition_attention, method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
         # normalization layers are preconditioned locally on every rank: the placement never sees them
@@ -275,6 +291,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'diagonal_g_layers': diagonal_g_layers,
             'precondition_norms': precondition_norms,
             'kfac_approx': kfac_approx,
+            'precondition_attention': precondition_attention,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
@@ -282,3 +299,5 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             kl_clip=kl_clip, lr=lr, accumulation_steps=accumulation_steps,
             assignment=assignment, update_factors_in_hook=update_factors_in_hook,
             defaults=defaults, tdc=self.tdc, loglevel=loglevel)
+        for module in self._attention_taps:
+            attention.bind(module, self)
