@@ -279,8 +279,18 @@ int kfac_transpose(const float* src, int ld_src, float* dst, int ld_dst, int row
  *   EIGEN  : P = [(grad Qa) / (dg x da + damping)] Qa^T      (qa, qaT, da; dgda is not used)
  *   INVERSE: P = diag(1 / (dg + damping)) grad Ainv           (a_inv)
  * qg, qgT, g_inv, dgda, ldqg and ld_dgda are ignored.  This is the embedding item with the dense
- * factor on the A side. */
-enum kfac_item_kind { KFAC_ITEM_DENSE = 0, KFAC_ITEM_EMBEDDING = 1, KFAC_ITEM_DIAG_G = 2 };
+ * factor on the A side.
+ * Tied items (kind = KFAC_ITEM_TIED): one (V, d) weight used by an embedding (token frequencies f,
+ * output-gradient factor E) and by a bias-less diagonal-G head (input factor H, diagonal G h).  With
+ * M and mu from kfac_tied_whiten / kfac_tied_basis (M^T (E + tI) M = I, M^T (H + tI) M = diag(mu),
+ * t = tied_damping), the row v of P is (f_v + t)(E + tI) + (h_v + t)(H + tI) solved for row v of
+ * the gradient:
+ *   P = [(wgrad M) / ((f + t) 1^T + (h + t) mu^T)] M^T
+ * wgrad is (a = V, g = d), bgrad NULL, qg = M, qgT = M^T (ld = ldqg), da = f, dh = h (V floats each),
+ * dg = mu (d floats), P (V x ldp, ldp >= d).  `method` and `damping` of the call are not used; the
+ * two GEMMs join the grouped launches, the division is one more launch over all tied items (the
+ * engines' epilogues are left as they are), and the other items' results do not depend on tied items. */
+enum kfac_item_kind { KFAC_ITEM_DENSE = 0, KFAC_ITEM_EMBEDDING = 1, KFAC_ITEM_DIAG_G = 2, KFAC_ITEM_TIED = 3 };
 typedef struct kfac_precond_item {
   const void* wgrad; /* (g, a - has_bias) */
   const void* bgrad; /* (g) or NULL */
@@ -305,10 +315,41 @@ typedef struct kfac_precond_item {
   float* const* peer_P;
   int n_peers;
   int kind; /* kfac_item_kind; 0 (dense) for the positional initialisers written before it */
+  const float* dh;    /* KFAC_ITEM_TIED: the head's diagonal G (V floats); else ignored */
+  float tied_damping; /* KFAC_ITEM_TIED: the damping M and mu were formed with (> 0) */
 } kfac_precond_item;
 size_t kfac_precondition_workspace_bytes(const kfac_precond_item* items, int count);
 int kfac_precondition(const kfac_precond_item* items, int count, int method,
                       float damping, void* ws, size_t ws_bytes, void* stream);
+
+/* Tied embedding / LM-head pairs (an extension beyond the reference, opt-in): the d x d factors E
+ * (the embedding's G) and H (the head's A) are diagonalised together.  With E = Q diag(e) Q^T
+ * (kfac_eigh_batched, e >= 0) and s = (e + damping)^-1/2:
+ *   kfac_tied_whiten:  C = diag(s) (Q^T H Q + damping I) diag(s), written exactly symmetric
+ *                      ((X + X^T) / 2 before the scaling), dense with ld = d: the F of a
+ *                      kfac_eigh_batched item whose Q / QT are U / UT below.
+ *   kfac_tied_basis:   M = Q diag(s) U (U: the eigenvectors of C in its columns) and MT = M^T.
+ * Then M^T (E + damping I) M = I and M^T (H + damping I) M = diag(mu), mu the eigenvalues of C.
+ * Q^T H Q, the product by Q and M run on the grouped wgmma engine (3xTF32); products with d > 1024
+ * are split into chains of <= 512 whose partials are added in a fixed order.  No floating-point
+ * atomics: the same inputs give the same bits.  Both calls are batched over items; the fields a
+ * call does not name are ignored.  ws: kfac_tied_workspace_bytes(items, count) bytes. */
+typedef struct kfac_tied_item {
+  const float* Q;  /* d x d (ld): eigenvectors of E in the columns (kfac_eigh_item.Q) */
+  const float* QT; /* its transpose (ld) */
+  const float* e;  /* d eigenvalues of E */
+  const float* H;  /* d x d (ld = d), symmetric: whiten */
+  float* C;        /* out of whiten: d x d (ld = d) */
+  const float* UT; /* basis: d x d (ld), rows are the eigenvectors of C (kfac_eigh_item.QT) */
+  float* M;        /* out of basis: d x d (ld) */
+  float* MT;       /* out of basis: d x d (ld), the transpose of M */
+  int d, ld;       /* ld: a multiple of 4, >= d */
+} kfac_tied_item;
+size_t kfac_tied_workspace_bytes(const kfac_tied_item* items, int count);
+int kfac_tied_whiten(const kfac_tied_item* items, int count, float damping, void* ws,
+                     size_t ws_bytes, void* stream);
+int kfac_tied_basis(const kfac_tied_item* items, int count, float damping, void* ws,
+                    size_t ws_bytes, void* stream);
 
 /* K11: replaces BaseKFACPreconditioner._compute_grad_scale
  * (kfac/base_preconditioner.py:411-435) without host syncs:

@@ -21,7 +21,7 @@ KFAC_ERR_WORKSPACE, KFAC_ERR_NO_CONVERGE, KFAC_ERR_UNSUPPORTED = -4, -5, -6
 KFAC_EIGEN, KFAC_INVERSE = 1, 2
 KFAC_EKFAC_KEEP, KFAC_EKFAC_EMA, KFAC_EKFAC_RESET, KFAC_EKFAC_SEED = 0, 1, 2, 3
 
-KFAC_ITEM_DENSE, KFAC_ITEM_EMBEDDING, KFAC_ITEM_DIAG_G = 0, 1, 2
+KFAC_ITEM_DENSE, KFAC_ITEM_EMBEDDING, KFAC_ITEM_DIAG_G, KFAC_ITEM_TIED = 0, 1, 2, 3
 
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 INDEX_DTYPE_CODE = {torch.int32: 3, torch.int64: 4}
@@ -44,7 +44,13 @@ class PrecondItem(C.Structure):
                 ('a_inv', c_void_p), ('g_inv', c_void_p),
                 ('ldqa', c_int), ('ldqg', c_int), ('ld_dgda', c_int),
                 ('P', c_void_p), ('ldp', c_int),
-                ('peer_P', C.POINTER(c_void_p)), ('n_peers', c_int), ('kind', c_int)]
+                ('peer_P', C.POINTER(c_void_p)), ('n_peers', c_int), ('kind', c_int),
+                ('dh', c_void_p), ('tied_damping', c_float)]
+
+
+class TiedItem(C.Structure):
+    _fields_ = [('Q', c_void_p), ('QT', c_void_p), ('e', c_void_p), ('H', c_void_p), ('C', c_void_p),
+                ('UT', c_void_p), ('M', c_void_p), ('MT', c_void_p), ('d', c_int), ('ld', c_int)]
 
 
 KFAC_NORM_BATCH, KFAC_NORM_LAYER, KFAC_NORM_RMS = 0, 1, 2
@@ -114,6 +120,9 @@ SIGNATURES = {
     'kfac_transpose': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     'kfac_precondition_workspace_bytes': (c_size_t, [C.POINTER(PrecondItem), c_int]),
     'kfac_precondition': (c_int, [C.POINTER(PrecondItem), c_int, c_int, c_float, c_void_p, c_size_t, c_void_p]),
+    'kfac_tied_workspace_bytes': (c_size_t, [C.POINTER(TiedItem), c_int]),
+    'kfac_tied_whiten': (c_int, [C.POINTER(TiedItem), c_int, c_float, c_void_p, c_size_t, c_void_p]),
+    'kfac_tied_basis': (c_int, [C.POINTER(TiedItem), c_int, c_float, c_void_p, c_size_t, c_void_p]),
     'kfac_grad_workspace_bytes': (c_size_t, [c_int]),
     'kfac_grad_scale': (c_int, [C.POINTER(GradItem), c_int, c_float, c_float, c_void_p, c_size_t, c_void_p, c_void_p]),
     'kfac_grad_update': (c_int, [C.POINTER(GradItem), c_int, c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -126,12 +126,12 @@ def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignm
     Returns (inv_segments, grad_segments): ordered lists of _Segment.
     """
     inv: dict[tuple[int, int], _Segment] = {}
+    # the head of a tied pair has no placement of its own: the embedding carries the pair
+    layers = [(name, layer) for name, layer in layers if layer.tied_embedding is None]
     for name, layer in layers:
         if not assignment.is_grad_worker(name):
             continue
         group = assignment.grad_worker_group(name)
-        src_a = assignment.inv_worker(name, 'A')
-        src_g = assignment.inv_worker(name, 'G')
         a, g = layer.a_dim, layer.g_dim
 
         def seg(src):
@@ -140,6 +140,17 @@ def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignm
                 inv[key] = _Segment(src, group)
             return inv[key]
 
+        if layer.tied_head is not None:
+            # tied pair: M (K-major copy built by every receiver), mu and the snapshots f and h, from the rank that
+            # holds all four factors
+            s = seg(assignment.inv_worker(name, 'G'))
+            s.add(layer, 'tq', (g, g))
+            s.add(layer, 'tmu', (g,))
+            s.add(layer, 'da', (a,))
+            s.add(layer, 'dh', (a,))
+            continue
+        src_a = assignment.inv_worker(name, 'A')
+        src_g = assignment.inv_worker(name, 'G')
         if layer.diag_side:
             # embedding / diagonal-G layer: the snapshot of the diagonal factor (its own eigenvalues) and the data of
             # the dense one; never a V x d dgda
@@ -431,6 +442,18 @@ class BaseKFACPreconditioner:
         local = 0
         plan = []
         for name, l in ll:
+            if l.tied_embedding is not None:
+                continue
+            if l.tied_head is not None:
+                # tied pair: M^T on the gradient workers; Q_E, e, C and the eigenvectors U of C on the rank that forms
+                # the pair's data (C is dense with ld = d, the layout the eigensolver reads)
+                d = l.g_dim
+                if self._assignment.is_grad_worker(name):
+                    plan.append((l, '_tqT', (d, d)))
+                if rank == self._assignment.inv_worker(name, 'G'):
+                    plan += [(l, '_qg', (d, d)), (l, '_qgT', (d, d)), (l, '_dg', (d,)), (l, '_C', (d * d,)),
+                             (l, '_U', (d, d)), (l, '_UT', (d, d))]
+                continue
             mine_a = rank == self._assignment.inv_worker(name, 'A')
             mine_g = rank == self._assignment.inv_worker(name, 'G')
             if l.diag_side:
@@ -504,7 +527,7 @@ class BaseKFACPreconditioner:
                 and self._assignment.broadcast_gradients() and self._layers)
         group = None
         if want:
-            name0 = next(iter(self._layers.values()))[0]
+            name0 = next(n for n, l in self._layers.values() if l.tied_embedding is None)
             group = self._assignment.grad_receiver_group(name0)
             # pure functions of (group, backend): identical on every rank, no collective involved
             want = (dist.get_backend(group) == 'nccl' and 2 <= dist.get_world_size(group) <= 8)
@@ -985,8 +1008,32 @@ class BaseKFACPreconditioner:
         eig: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
         eig_diag: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
         post: list[tuple[KFACLayer, str]] = []
+        tied: list[KFACLayer] = []
         snapshots = False
         for name, layer in reversed(self._layer_list()):
+            if layer.tied_embedding is not None:
+                continue
+            if layer.tied_head is not None:
+                # tied pair: the snapshots f and h, E decomposed with the diagonal layers' dense factors, then the
+                # whitened H in a call of its own below.  Every rank keeps the damping the data is formed with
+                layer._tied_damping = damping
+                if rank != self._assignment.inv_worker(name, 'G'):
+                    continue
+                head, I = layer.tied_head, layer._inv
+                if not (layer._has_a and layer._has_g and head._has_a and head._has_g):
+                    raise RuntimeError('Cannot decompose the factors of a tied embedding / head pair before they have '
+                                       'been computed')
+                if self._diag_status is None:
+                    self._diag_status = torch.zeros(1, dtype=torch.int32, device=self._device)
+                if not snapshots:
+                    self._diag_status.zero_()
+                    snapshots = True
+                for view, key in ((layer._a_view, 'da'), (head._g_view, 'dh')):
+                    _cabi.check(lib.kfac_diag_snapshot(view.data_ptr(), I[key].data_ptr(), view.numel(),
+                                                       self._diag_status.data_ptr(), stream), 'kfac_diag_snapshot')
+                eig_diag.append((layer._g_view, I['_qg'], I['_qgT'], I['_dg'], layer.g_dim))
+                tied.append(layer)
+                continue
             mine_a = rank == self._assignment.inv_worker(name, 'A')
             mine_g = rank == self._assignment.inv_worker(name, 'G')
             if mine_a and not layer._has_a:
@@ -1059,7 +1106,7 @@ class BaseKFACPreconditioner:
         # embeddings and diagonal-G layers
         batches = [b for b in (eig, eig_diag) if b]
         if (batches or snapshots) and self._eig_status is None:
-            self._eig_status = torch.zeros(3, dtype=torch.int32).pin_memory()
+            self._eig_status = torch.zeros(4, dtype=torch.int32).pin_memory()
             self._eig_event = torch.cuda.Event()
         for slot, batch in enumerate(batches):
             items = (_cabi.EighItem * len(batch))()
@@ -1077,11 +1124,13 @@ class BaseKFACPreconditioner:
             # kfac/layers/eigen.py:310; here the error surfaces one call later instead of stalling the stream)
             _cabi.check(lib.kfac_eigh_status(ws.data_ptr(), self._eig_status[slot:].data_ptr(), stream),
                         'kfac_eigh_status')
+        if tied:
+            self._tied_inverses(tied, damping)
         if snapshots:
             # status word of the diagonal snapshots: same pinned path, no host sync
-            self._eig_status[2:].copy_(self._diag_status, non_blocking=True)
+            self._eig_status[2:3].copy_(self._diag_status, non_blocking=True)
         if batches or snapshots:
-            self._eig_slots = list(range(len(batches))) + ([2] if snapshots else [])
+            self._eig_slots = list(range(len(batches))) + ([2] if snapshots else []) + ([3] if tied else [])
             self._eig_event.record()
             self._eig_pending = True
         for layer, what in post:
@@ -1106,12 +1155,40 @@ class BaseKFACPreconditioner:
                                     group=seg.group)
             for layer, key, shape in seg.entries:
                 layer._inv_ready.add(key)
-                # a rank that RECEIVED an eigenbasis builds its K-major copy locally
-                if bcast and seg.src != rank and key in ('qa', 'qg'):
+                if key == 'tq':
+                    layer._inv_ready.add('_tqT')
+                # a rank that RECEIVED an eigenbasis (or a tied pair's M) builds its K-major copy locally
+                if bcast and seg.src != rank and key in ('qa', 'qg', 'tq'):
                     n, ld = shape[0], _cabi.ld4(shape[0])
                     _cabi.check(lib.kfac_transpose(layer._inv[key].data_ptr(), ld,
                                                    layer._inv['_' + key + 'T'].data_ptr(), ld, n, n, stream),
                                 'kfac_transpose')
+
+    def _tied_inverses(self, tied: list[KFACLayer], damping: float) -> None:
+        """M and mu of the tied pairs this rank forms, after the call that decomposed their E: C (whitened H), then
+        its eigendecomposition in a third call shared by all pairs (status slot 3), then M and M^T."""
+        lib = _cabi.load()
+        stream = _cabi.stream_ptr()
+        items = (_cabi.TiedItem * len(tied))()
+        eigs = (_cabi.EighItem * len(tied))()
+        ns = (C.c_int * len(tied))()
+        for i, layer in enumerate(tied):
+            I, d = layer._inv, layer.g_dim
+            items[i] = _cabi.TiedItem(I['_qg'].data_ptr(), I['_qgT'].data_ptr(), I['_dg'].data_ptr(),
+                                      layer.tied_head._a_view.data_ptr(), I['_C'].data_ptr(), I['_UT'].data_ptr(),
+                                      I['tq'].data_ptr(), I['_tqT'].data_ptr(), d, _cabi.ld4(d))
+            eigs[i] = _cabi.EighItem(I['_C'].data_ptr(), I['_U'].data_ptr(), I['_UT'].data_ptr(), I['tmu'].data_ptr(),
+                                     d, _cabi.ld4(d), None)
+            ns[i] = d
+        need = lib.kfac_tied_workspace_bytes(items, len(tied))
+        ws = self._gemm_scratch.get(need, self._device)
+        _cabi.check(lib.kfac_tied_whiten(items, len(tied), damping, ws.data_ptr(), need, stream), 'kfac_tied_whiten')
+        need_e = lib.kfac_eigh_workspace_bytes(ns, len(tied))
+        ws_e = self._eig_scratch.get(need_e, self._device)
+        _cabi.check(lib.kfac_eigh_batched(eigs, len(tied), ws_e.data_ptr(), need_e, 0, 0.0, stream), 'kfac_eigh_batched')
+        _cabi.check(lib.kfac_eigh_status(ws_e.data_ptr(), self._eig_status[3:].data_ptr(), stream), 'kfac_eigh_status')
+        ws = self._gemm_scratch.get(need, self._device)
+        _cabi.check(lib.kfac_tied_basis(items, len(tied), damping, ws.data_ptr(), need, stream), 'kfac_tied_basis')
 
     # EKFAC ----------------------------------------------------------------
     def _ekfac_update(self, new_basis: bool) -> None:
@@ -1177,7 +1254,8 @@ class BaseKFACPreconditioner:
 
     def _precondition(self) -> None:
         lib = _cabi.load()
-        todo = [(n, l) for n, l in reversed(self._layer_list()) if self._assignment.is_grad_worker(n)]
+        todo = [(n, l) for n, l in reversed(self._layer_list())
+                if l.tied_embedding is None and self._assignment.is_grad_worker(n)]
         eigen = None
         items = (_cabi.PrecondItem * max(1, len(todo)))()
         fused = self._peer_p_bases is not None
@@ -1187,7 +1265,16 @@ class BaseKFACPreconditioner:
             w, b = self._grad_ptrs(layer)
             I = layer._inv
             ready = layer._inv_ready
-            if layer.diag_side:
+            if layer.tied_head is not None:
+                # tied pair: M, M^T, mu, the snapshots f (da) and h (dh), and the damping they were formed with
+                if not {'tq', '_tqT', 'tmu', 'da', 'dh'} <= ready:
+                    raise RuntimeError('The second-order data of the tied embedding / head pair has not been computed')
+                items[i] = _cabi.PrecondItem(
+                    w.data_ptr(), None, _cabi.DTYPE_CODE[w.dtype], layer.g_dim, layer.a_dim, None, None,
+                    I['tq'].data_ptr(), I['_tqT'].data_ptr(), None, I['da'].data_ptr(), I['tmu'].data_ptr(), None, None,
+                    0, _cabi.ld4(layer.g_dim), 0, layer._p_store.data_ptr(), _cabi.ld4(layer.p_shape[1]), None, 0,
+                    _cabi.KFAC_ITEM_TIED, I['dh'].data_ptr(), layer._tied_damping)
+            elif layer.diag_side:
                 # embedding (d = 'a') or diagonal-G layer (d = 'g'): the diagonal factor's snapshot and the dense
                 # factor f's eigendecomposition (eigen) or inverse
                 d, f = layer.diag_side, layer.dense_side
@@ -1285,7 +1372,8 @@ class BaseKFACPreconditioner:
     # K11/K12 --------------------------------------------------------------
     def _scale_and_write_back(self) -> None:
         lib = _cabi.load()
-        ll = list(reversed(self._layer_list())) + self._norm_list()    # nu over all layers
+        # nu over all layers; the weight of a tied pair counts once (through its embedding)
+        ll = [(n, l) for n, l in reversed(self._layer_list()) if l.tied_embedding is None] + self._norm_list()
         items = (_cabi.GradItem * max(1, len(ll)))()
         for i, (_, layer) in enumerate(ll):
             w, b = self._grad_ptrs(layer)

@@ -249,11 +249,13 @@ extern "C" int kfac_transpose(const float* src, int ld_src, float* dst, int ld_d
   return KFAC_OK;
 }
 
+struct TiedScaleDev { float* T; const float* f; const float* h; const float* mu; float t; int n, ld; long long elem0; };
+
 // ---- precondition: stage-wise over ALL layers ------------------------------------------------------
 // workspace: [GatherDev table][grouped-GEMM tables][ones vector][per layer: GR (g x ld4 a), T1 (a x ld4 g),
 // T2 (g x ld4 a)][slabs].  A diagonal item (rows x n, see DiagItem) takes GR and T1 as rows x ld4(n) and no T2.
 struct PrecondLayout {
-  size_t off_gather, off_gemm, off_ones, off_tiles, off_slab, total;
+  size_t off_gather, off_tied, off_gemm, off_ones, off_tiles, off_slab, total;
   int ones_n;                                          // length of the ones vector (inverse method, diagonal items)
   std::vector<size_t> gr, t1, t2, slab_a, slab_g;     // byte offsets per layer (slab_*: 0 = no split)
   std::vector<int> splits_a, splits_g;
@@ -262,28 +264,33 @@ struct PrecondLayout {
 // An embedding item and a diagonal-G item are the same problem with the sides swapped: a gradient of `rows` x n
 // (V x d for an embedding, V x a for a diagonal-G layer), one dense factor of size n on its columns (G, resp. A:
 // basis q, its transpose qT, inverse inv, eigenvalues vcol) and one diagonal factor vrow on its rows.  P has the
-// gradient's layout, rows x n.
+// gradient's layout, rows x n.  A tied item is an embedding item whose basis q = M is not orthogonal and whose
+// epilogue reads a second row vector vrow2 = h and its own damping (KFAC_ITEM_TIED in the header).
 struct DiagItem {
   int rows, n;
   const float *q, *qT, *inv, *vrow, *vcol;
   int ldq;
+  const float* vrow2;
+  float damping;
 };
 
 static bool is_diag(const kfac_precond_item& it) { return it.kind != KFAC_ITEM_DENSE; }
 
 static DiagItem diag_view(const kfac_precond_item& it) {
-  if (it.kind == KFAC_ITEM_EMBEDDING) return DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg};
-  return DiagItem{it.g, it.a, it.qa, it.qaT, it.a_inv, it.dg, it.da, it.ldqa};
+  if (it.kind == KFAC_ITEM_EMBEDDING) return DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg, nullptr, 0.f};
+  if (it.kind == KFAC_ITEM_TIED) return DiagItem{it.a, it.g, it.qg, it.qgT, nullptr, it.da, it.dg, it.ldqg, it.dh, it.tied_damping};
+  return DiagItem{it.g, it.a, it.qa, it.qaT, it.a_inv, it.dg, it.da, it.ldqa, nullptr, 0.f};
 }
 
 static void precond_layout(const kfac_precond_item* items, int count, PrecondLayout& L) {
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
   L.off_gather = take(sizeof(GatherDev) * (size_t)std::max(1, count));
+  L.off_tied = take(sizeof(TiedScaleDev) * (size_t)std::max(1, count));
   L.off_gemm = take(grouped_gemm_ws_bytes(count));
   L.ones_n = 0;
   for (int i = 0; i < count; ++i)
-    if (is_diag(items[i])) L.ones_n = std::max(L.ones_n, diag_view(items[i]).n);
+    if (is_diag(items[i]) && items[i].kind != KFAC_ITEM_TIED) L.ones_n = std::max(L.ones_n, diag_view(items[i]).n);
   L.off_ones = L.ones_n ? take((size_t)L.ones_n * sizeof(float)) : off;
   L.off_tiles = off;
   L.gr.resize(count); L.t1.resize(count); L.t2.resize(count);
@@ -324,6 +331,20 @@ static void precond_layout(const kfac_precond_item* items, int count, PrecondLay
   L.total = off;
 }
 
+// T[v][j] /= (f[v] + t) + (h[v] + t) mu[j] for every tied item, one launch: the division of a tied item's first product,
+// kept out of the GEMM engines so that their epilogues (shared by every layer) stay as they are
+__global__ void __launch_bounds__(256) tied_scale_kernel(const TiedScaleDev* items, int count, long long total) {
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    int lo = 0, hi = count - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (items[mid].elem0 <= e) lo = mid; else hi = mid - 1; }
+    const TiedScaleDev& it = items[lo];
+    const long long idx = e - it.elem0;
+    const long long v = idx / it.ld;
+    const int j = (int)(idx % it.ld);
+    if (j < it.n) it.T[idx] = it.T[idx] / ((it.f[v] + it.t) + (it.h[v] + it.t) * it.mu[j]);
+  }
+}
+
 __global__ void fill_ones_kernel(float* out, int n) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = 1.f;
 }
@@ -354,17 +375,21 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
   long long total = 0;
   for (int i = 0; i < count; ++i) {
     const kfac_precond_item& it = items[i];
-    KFAC_CHECK_ARG(it.kind == KFAC_ITEM_DENSE || it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_G,
-                   "precond item kind");
+    KFAC_CHECK_ARG(it.kind == KFAC_ITEM_DENSE || it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_G ||
+                   it.kind == KFAC_ITEM_TIED, "precond item kind");
     KFAC_CHECK_ARG(it.n_peers >= 0 && it.n_peers <= 7 && (it.n_peers == 0 || it.peer_P), "precond peers");
     if (is_diag(it)) {
       const DiagItem D = diag_view(it);
       KFAC_CHECK_ARG(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= D.n && D.ldq >= D.n &&
-                     (it.kind != KFAC_ITEM_EMBEDDING || !it.bgrad), "precond diagonal item");
-      const bool ready = D.vrow && (method == KFAC_EIGEN ? (D.q && D.qT && D.vcol) : D.inv != nullptr);
+                     (it.kind == KFAC_ITEM_DIAG_G || !it.bgrad), "precond diagonal item");
+      KFAC_CHECK_ARG(it.kind != KFAC_ITEM_TIED || it.tied_damping > 0.f, "precond tied item damping");
+      const bool ready = D.vrow && (it.kind == KFAC_ITEM_TIED ? (D.q && D.qT && D.vcol && D.vrow2)
+                                    : method == KFAC_EIGEN ? (D.q && D.qT && D.vcol) : D.inv != nullptr);
       if (!ready) {
         set_error(it.kind == KFAC_ITEM_EMBEDDING
                       ? "precondition: the second-order data of an embedding layer has not been computed"
+                  : it.kind == KFAC_ITEM_TIED
+                      ? "precondition: the second-order data of a tied embedding / head pair has not been computed"
                       : "precondition: the second-order data of a diagonal-G layer has not been computed");
         return KFAC_ERR_NOT_READY;
       }
@@ -417,7 +442,9 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
     const int g = it.g, a = it.a;
     if (is_diag(it)) {                  // (1d) T[v, j] = (sum_k grad[v, k] Q[k, j]) / (vrow[v] vcol[j] + damping)   (rows x n, K = n)
       const DiagItem D = diag_view(it);
-      if (method == KFAC_EIGEN) {
+      if (it.kind == KFAC_ITEM_TIED) {  // (1t) T[v, j] = sum_k grad[v, k] M[k, j], divided by tied_scale_kernel below
+        plain(i, F(L.gr[i]), ld4(D.n), D.qT, D.ldq, F(L.t1[i]), ld4(D.n), D.rows, D.n, D.n);
+      } else if (method == KFAC_EIGEN) {
         plain(i, F(L.gr[i]), ld4(D.n), D.qT, D.ldq, F(L.t1[i]), ld4(D.n), D.rows, D.n, D.n);
         div_rows(i, D, D.vcol);
       } else {
@@ -429,6 +456,23 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
     if (L.splits_a[i] > 1) { st[i].splits = L.splits_a[i]; st[i].slab = F(L.slab_a[i]); st[i].slab_stride = (int64_t)a * ld4(g); }
   }
   if ((rc = run())) return rc;
+  {                                     // (1t') the tied items' division, elementwise over all of them in one launch
+    std::vector<TiedScaleDev> tied;
+    long long tied_total = 0;
+    for (int i = 0; i < count; ++i) {
+      if (items[i].kind != KFAC_ITEM_TIED) continue;
+      const DiagItem D = diag_view(items[i]);
+      tied.push_back(TiedScaleDev{F(L.t1[i]), D.vrow, D.vrow2, D.vcol, D.damping, D.n, ld4(D.n), tied_total});
+      tied_total += (long long)D.rows * ld4(D.n);
+    }
+    if (!tied.empty()) {
+      KFAC_CUDA(cudaMemcpyAsync(base + L.off_tied, tied.data(), sizeof(TiedScaleDev) * tied.size(),
+                                cudaMemcpyHostToDevice, s));
+      tied_scale_kernel<<<grid_for(tied_total), 256, 0, s>>>((const TiedScaleDev*)(base + L.off_tied), (int)tied.size(),
+                                                             tied_total);
+      KFAC_LAUNCH_CHECK();
+    }
+  }
   if (method == KFAC_EIGEN) {
     for (int i = 0; i < count; ++i) {   // (2) V2[g', a'] = (sum_k QgT[g', k] T^T[a', k]) * dgda[g', a']     (g x a, K = g)
       const kfac_precond_item& it = items[i];
@@ -454,7 +498,7 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
     int64_t p_rows = g, p_ld = ld4(a);
     if (is_diag(it)) {
       const DiagItem D = diag_view(it);
-      if (method == KFAC_EIGEN) {       // (4d) P[v, c] = sum_k T[v, k] Q[c, k]                              (rows x n, K = n)
+      if (method == KFAC_EIGEN || it.kind == KFAC_ITEM_TIED) {   // (4d) P[v, c] = sum_k T[v, k] Q[c, k]  (rows x n, K = n)
         plain(i, F(L.t1[i]), ld4(D.n), D.q, D.ldq, it.P, it.ldp, D.rows, D.n, D.n);
       } else {                          // (4d) P[v, c] = (sum_k grad[v, k] Inv[c, k]) / (vrow[v] + damping)  (rows x n, K = n)
         plain(i, F(L.gr[i]), ld4(D.n), D.inv, D.ldq, it.P, it.ldp, D.rows, D.n, D.n);

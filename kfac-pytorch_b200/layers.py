@@ -741,6 +741,11 @@ class KFACLayer:
         # normalization layer (precondition_norms): no A factor, G holds the C x k blocks, P is C x a_dim
         # (a_dim = 1 + has_bias); it is preconditioned locally on every rank, outside the work assignment
         self.norm = module.norm
+        # tied pair (precondition_tied_embeddings): the embedding holds its head in `tied_head` and carries the pair's
+        # placement, second-order data and P; the head holds the embedding in `tied_embedding` and keeps only its
+        # factors
+        self.tied_head: KFACLayer | None = None
+        self.tied_embedding: KFACLayer | None = None
         self.index = -1
         # arena views (bound by the preconditioner)
         self._a_view = self._g_view = None

@@ -36,21 +36,34 @@ def layer_work(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
                assignment_strategy: AssignmentStrategy) -> dict[str, dict[str, float]]:
     """Per-factor cost the KAISA placement balances: d^3 (COMPUTE) or d^2 (MEMORY) for a dense factor.  A diagonal
     factor (an embedding's A, a diagonal-G layer's G) is never decomposed and takes V floats, so its cost is V under
-    both strategies; a V^3 cost would let one vocabulary dominate the greedy placement."""
+    both strategies; a V^3 cost would let one vocabulary dominate the greedy placement.  A tied pair is one unit
+    under the embedding's name with the single factor 'G' (one rank holds E, H, f and h whatever colocate_factors
+    says), costed 2 cost(d) + 2 V; the head has no entry."""
     if assignment_strategy == AssignmentStrategy.COMPUTE:
         cost = lambda n: n ** 3  # noqa: E731
     elif assignment_strategy == AssignmentStrategy.MEMORY:
         cost = lambda n: n ** 2  # noqa: E731
     else:
         raise AssertionError(f'Unknown assignment_strategy={assignment_strategy}')
-    return {name: {'A': l.a_dim if l.diag_a else cost(l.a_dim), 'G': l.g_dim if l.diag_g else cost(l.g_dim)}
-            for name, l in layers.values()}
+    work = {}
+    for name, l in layers.values():
+        if l.tied_embedding is not None:
+            continue
+        if l.tied_head is not None:
+            work[name] = {'G': 2 * cost(l.g_dim) + 2 * l.a_dim}
+        else:
+            work[name] = {'A': l.a_dim if l.diag_a else cost(l.a_dim), 'G': l.g_dim if l.diag_g else cost(l.g_dim)}
+    return work
 
 
 def _check_diagonal_layers(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
-                           compute_method: ComputeMethod) -> None:
-    """Reject the registered diagonal layers (embeddings, diagonal-G layers) this preconditioner cannot handle."""
+                           compute_method: ComputeMethod, tied_embeddings: bool = False) -> None:
+    """Reject the registered diagonal layers (embeddings, diagonal-G layers) this preconditioner cannot handle.  With
+    `tied_embeddings`, an embedding whose weight is the weight of one bias-less diagonal-G Linear forms a tied pair
+    with it instead (`KFACLayer.tied_head` / `tied_embedding`)."""
     diag = [(module, name, l) for module, (name, l) in layers.items() if l.diag_side]
+    if tied_embeddings:
+        _tie_pairs(layers, compute_method)
     for module, name, l in diag:
         kind, keyword = ('embedding', 'precondition_embeddings') if l.diag_a else ('layer', 'diagonal_g_layers')
         if compute_method == ComputeMethod.EKFAC:
@@ -63,9 +76,45 @@ def _check_diagonal_layers(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
             raise ValueError(f'embedding "{name}" has scale_grad_by_freq=True: its weight gradient is then not the '
                              'one the K-FAC factors model (add it to skip_layers)')
         for other, (other_name, _) in layers.items():
+            if l.tied_head is not None or l.tied_embedding is not None:
+                break
             if other is not module and any(p is module.weight for p in other.parameters()):
                 raise ValueError(f'{kind} "{name}" shares its weight with "{other_name}": two layers would '
                                  f'precondition one gradient; add one of them to skip_layers')
+
+
+def _tie_pairs(layers: dict[torch.nn.Module, tuple[str, KFACLayer]], compute_method: ComputeMethod) -> None:
+    """Form the tied pairs of precondition_tied_embeddings: a registered embedding and the one other registered module
+    that owns its weight, which must be a bias-less torch.nn.Linear matched by diagonal_g_layers."""
+    for module, (name, l) in layers.items():
+        if not l.diag_a:
+            continue
+        owners = [(other, other_name, ol) for other, (other_name, ol) in layers.items()
+                  if other is not module and any(p is module.weight for p in other.parameters())]
+        if not owners:
+            continue
+        if len(owners) > 1:
+            names = ', '.join(f'"{n}"' for _, n, _ in owners)
+            raise ValueError(f'embedding "{name}" shares its weight with {names}: precondition_tied_embeddings pairs '
+                             'one embedding with one head; add all but one of them to skip_layers')
+        head, head_name, hl = owners[0]
+        if not isinstance(head, torch.nn.Linear) or head.weight is not module.weight:
+            raise ValueError(f'embedding "{name}" shares a weight with "{head_name}", which is not a torch.nn.Linear '
+                             'using it as its weight: precondition_tied_embeddings ties an embedding to a Linear head '
+                             'only; add one of them to skip_layers')
+        if not hl.diag_g:
+            raise ValueError(f'embedding "{name}" is tied to "{head_name}", which is not in diagonal_g_layers: '
+                             f'precondition_tied_embeddings needs the head\'s diagonal G; add "{head_name}" to '
+                             'diagonal_g_layers (or one of the two layers to skip_layers)')
+        if head.bias is not None:
+            raise ValueError(f'embedding "{name}" is tied to "{head_name}", which has a bias: '
+                             'precondition_tied_embeddings supports bias-less heads only; add one of the two layers '
+                             'to skip_layers')
+        if compute_method == ComputeMethod.EKFAC:
+            raise ValueError(f'precondition_tied_embeddings does not support compute_method=EKFAC (pair "{name}" / '
+                             f'"{head_name}"); add one of the two layers to skip_layers')
+        l.tied_head, hl.tied_embedding = hl, l
+    # a weight shared by two Linears (with or without an embedding) stays refused by the checks that follow
 
 
 class KFACPreconditioner(BaseKFACPreconditioner):
@@ -82,7 +131,8 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     kept as a vector; see `kfac_b200.layers.EmbeddingModuleHelper`.  The embedding's P is always formed from the
     eigenvalue vectors (`compute_eigenvalue_outer_product` does not apply to it, so no V x d matrix is stored),
     and its damping is the one of the step that preconditions.  It cannot be combined with EKFAC, sparse
-    gradients, `scale_grad_by_freq`, or a weight shared with another registered module (a tied LM head).
+    gradients, `scale_grad_by_freq`, or a weight shared with another registered module (a tied LM head; see
+    `precondition_tied_embeddings`).
 
     `diagonal_g_layers` takes regexes matched against module names and class names, like `skip_layers`.  A
     registered `torch.nn.Linear` that matches keeps its G factor as the vector diag(G) of `out_features` floats
@@ -139,6 +189,19 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     attention's batch dimension (an unbatched call is one example).  Refused with a ValueError: `add_bias_kv`,
     `add_zero_attn`, subclasses of `torch.nn.MultiheadAttention`, a `diagonal_g_layers` pattern matching an attention or
     a projection, and a projection weight shared with another registered module.
+
+    `precondition_tied_embeddings=True` preconditions a weight tied between a registered embedding
+    (`precondition_embeddings`) and a bias-less `torch.nn.Linear` head in `diagonal_g_layers` (GPT-2, nanoGPT), instead
+    of refusing it.  Both uses keep their statistics: the embedding's token frequencies f and G factor E, the head's A
+    factor H and diagonal G h.  With the uses treated as uncorrelated and the factor-wise damping t of the inverse
+    step, row v of the (V, d) gradient is preconditioned by
+        F_v = (f_v + t)(E + t I) + (h_v + t)(H + t I),    P_v = F_v^-1 grad_v,
+    solved exactly for all rows through the simultaneous diagonalisation M^T (E + t I) M = I,
+    M^T (H + t I) M = diag(mu):  P = [(grad M) / ((f + t) 1^T + (h + t) mu^T)] M^T.  The pair is one unit of the
+    placement (one rank decomposes E and the whitened H), P is stored and written back once, under every
+    compute_method; `state_dict()` keeps both members' entries with their untied shapes.  Refused with a ValueError:
+    a tied head outside `diagonal_g_layers`, a tied head with a bias, a weight owned by more than two registered
+    modules or by two Linears, and EKFAC.  With `skip_layers` matching either member there is no pair.
     """
 
     def __init__(
@@ -170,6 +233,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         precondition_norms: bool = False,
         kfac_approx: str = 'expand',
         precondition_attention: bool = False,
+        precondition_tied_embeddings: bool = False,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -260,7 +324,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         # normalization layers are preconditioned locally on every rank: the placement never sees them
         norm_layers = {m: v for m, v in kfac_layers.items() if v[1].norm}
         kfac_layers = {m: v for m, v in kfac_layers.items() if not v[1].norm}
-        _check_diagonal_layers(kfac_layers, compute_method)
+        _check_diagonal_layers(kfac_layers, compute_method, tied_embeddings=precondition_tied_embeddings)
         for name, kfac_layer in list(kfac_layers.values()) + list(norm_layers.values()):
             logger.log(loglevel, f'Registered name="{name}": {repr(kfac_layer)}')
 
@@ -292,6 +356,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'precondition_norms': precondition_norms,
             'kfac_approx': kfac_approx,
             'precondition_attention': precondition_attention,
+            'precondition_tied_embeddings': precondition_tied_embeddings,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
