@@ -86,11 +86,43 @@ int kfac_factor_conv2d_input(const void* x, int dtype, int batch, int C, int H,
                              int pw, int append_ones, float scale, float* acc,
                              void* ws, size_t ws_bytes, void* stream);
 
+/* Geometry of a Conv1d / Conv2d / Conv3d layer's input, every per-axis array in (D, H, W)
+ * order: a Conv1d is D = kd = 1, H = kh = 1; the Conv2d entries are D = kd = 1 with dilation 1
+ * and symmetric padding.  The output extent of an axis is
+ *     (in + pad_before + pad_after - dilation * (kernel - 1) - 1) / stride + 1,
+ * and the feature order of A is (C, kd, kh, kw) [+ ones], the order of weight.reshape(out, -1).
+ * Padding is zero padding (other padding modes are applied to x by the caller). */
+typedef struct kfac_conv_geometry {
+  int batch, C;
+  int in[3];
+  int kernel[3];
+  int stride[3];
+  int dilation[3];
+  int pad_before[3];
+  int pad_after[3];
+} kfac_conv_geometry;
+
+/* acc (d x d) += scale * X^T X, X the N-d dilated im2col of x (batch, C, D, H, W) in any dtype.
+ * The im2col is formed in fp32, feature-major, in chunks of whole examples: the largest chunk
+ * whose matrix and SYRK partials fit in ws_bytes (one example with an unsplit SYRK when only
+ * its matrix fits), each chunk's SYRK added to acc in chunk order, so a call is deterministic
+ * for a given ws_bytes.  The workspace query returns the bytes of the largest chunk whose
+ * matrix and SYRK partials together fit in max_bytes, or of one example when even that does
+ * not fit.  A kernel of all ones with unit stride and no padding reads x in place (no
+ * matrix).  Conv2d: kfac_factor_conv2d_input is this call with one chunk of the whole batch. */
+size_t kfac_factor_conv_input_workspace_bytes(const kfac_conv_geometry* geom, int append_ones,
+                                              size_t max_bytes);
+int kfac_factor_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom,
+                           int append_ones, float scale, float* acc, void* ws, size_t ws_bytes,
+                           void* stream);
+
 /* replaces Conv2dModuleHelper.get_g_factor (modules.py:180-192):
  * g is (batch, C, Ho, Wo); acc (C x C) += scale * sum_n Y_n Y_n^T.
  * ws (optional, kfac_factor_conv2d_gradout_workspace_bytes): maps whose rows are not
  * 16-byte multiples (7 x 7) are packed there for the tensor-core SYRK; without it they
- * take the SIMT kernel. */
+ * take the SIMT kernel.  Only the plane of S = Ho * Wo elements is used, so the output
+ * gradient of a Conv1d (S = Lo) or Conv3d (S = Do * Ho * Wo) layer is passed as (1, S); the
+ * same holds for kfac_rows_conv2d_gradout and kfac_reduce_rows_conv2d_gradout. */
 size_t kfac_factor_conv2d_gradout_workspace_bytes(int batch, int C, int Ho, int Wo);
 int kfac_factor_conv2d_gradout(const void* g, int dtype, int batch, int C,
                                int Ho, int Wo, float scale, float* acc,
@@ -395,6 +427,10 @@ int kfac_rows_linear_strided(const void* x, int dtype, int64_t rows, int feature
 int kfac_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W, int kh,
                            int kw, int sh, int sw, int ph, int pw, int append_ones, float scale,
                            float* out, int ld_out, void* stream);
+/* the rows of kfac_factor_conv_input: (batch * Do * Ho * Wo) x ld_out; the Conv2d entry above is
+ * this call with a depth-1, dilation-1 geometry */
+int kfac_rows_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom, int append_ones,
+                         float scale, float* out, int ld_out, void* stream);
 /* g (batch, C, Ho, Wo) -> rows (batch*Ho*Wo, C) */
 int kfac_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo,
                              float scale, const float* loss_scale, float* out, int ld_out,
@@ -432,6 +468,14 @@ int kfac_reduce_rows_conv2d_input(const void* x, int dtype, int batch, int C, in
 int kfac_reduce_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo,
                                     float scale, const float* loss_scale, float* out,
                                     int ld_out, void* stream);
+/* conv2d_input for an N-d geometry with dilation: the window sums of every (b, c) volume over
+ * the output lattice, feature order (C, kd, kh, kw) [+ ones], the ones column
+ * scale * Do * Ho * Wo.  kd * kh * kw <= 2048.  The Conv2d entry above is this call with a
+ * depth-1, dilation-1 geometry.  A single-row input (D = H = 1, kd = kh = 1, no depth or height
+ * padding: a Conv1d) spreads each window offset's sum over a CTA; the sums keep their order. */
+int kfac_reduce_rows_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom,
+                                int append_ones, float scale, float* out, int ld_out,
+                                void* stream);
 
 /* S_batch of every item, for all items together; no floating-point atomics, the same bits on
  * every run.  Launches: one grouped wgmma launch of the projections (x^2 epilogue), the K = N

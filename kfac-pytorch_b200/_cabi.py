@@ -21,10 +21,18 @@ KFAC_ERR_WORKSPACE, KFAC_ERR_NO_CONVERGE, KFAC_ERR_UNSUPPORTED = -4, -5, -6
 KFAC_EIGEN, KFAC_INVERSE = 1, 2
 KFAC_EKFAC_KEEP, KFAC_EKFAC_EMA, KFAC_EKFAC_RESET, KFAC_EKFAC_SEED = 0, 1, 2, 3
 
+KFAC_EIGH_MAX_N = 8192   # largest factor dimension the eigensolver takes
+
 KFAC_ITEM_DENSE, KFAC_ITEM_EMBEDDING, KFAC_ITEM_DIAG_G, KFAC_ITEM_TIED = 0, 1, 2, 3
 
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 INDEX_DTYPE_CODE = {torch.int32: 3, torch.int64: 4}
+
+
+class ConvGeometry(C.Structure):
+    """kfac_conv_geometry: every per-axis array in (D, H, W) order."""
+    _fields_ = [('batch', c_int), ('C', c_int), ('input', c_int * 3), ('kernel', c_int * 3), ('stride', c_int * 3),
+                ('dilation', c_int * 3), ('pad_before', c_int * 3), ('pad_after', c_int * 3)]
 
 
 class EmaItem(C.Structure):
@@ -90,6 +98,9 @@ SIGNATURES = {
                                            c_size_t, c_void_p]),
     'kfac_factor_conv2d_input_workspace_bytes': (c_size_t, [c_int] * 11),
     'kfac_factor_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'kfac_factor_conv_input_workspace_bytes': (c_size_t, [C.POINTER(ConvGeometry), c_int, c_size_t]),
+    'kfac_factor_conv_input': (c_int, [c_void_p, c_int, C.POINTER(ConvGeometry), c_int, c_float, c_void_p, c_void_p,
+                                       c_size_t, c_void_p]),
     'kfac_factor_conv2d_gradout_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
     'kfac_factor_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     'kfac_factor_ema': (c_int, [C.POINTER(EmaItem), c_int, c_float, c_void_p]),
@@ -130,6 +141,8 @@ SIGNATURES = {
     'kfac_rows_linear_strided': (c_int, [c_void_p, c_int, c_int64, c_int, c_int64, c_int, c_float, c_void_p, c_void_p,
                                          c_int, c_void_p]),
     'kfac_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
+    'kfac_rows_conv_input': (c_int, [c_void_p, c_int, C.POINTER(ConvGeometry), c_int, c_float, c_void_p, c_int,
+                                     c_void_p]),
     'kfac_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
                                          c_void_p]),
     'kfac_reduce_rows_linear': (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_float, c_void_p, c_void_p,
@@ -137,6 +150,8 @@ SIGNATURES = {
     'kfac_reduce_rows_linear_strided': (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int64, c_int64, c_int,
                                                 c_float, c_void_p, c_void_p, c_int, c_void_p]),
     'kfac_reduce_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
+    'kfac_reduce_rows_conv_input': (c_int, [c_void_p, c_int, C.POINTER(ConvGeometry), c_int, c_float, c_void_p, c_int,
+                                            c_void_p]),
     'kfac_reduce_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                                 c_void_p, c_int, c_void_p]),
     'kfac_ekfac_statistics_workspace_bytes': (c_size_t, [C.POINTER(EkfacStatItem), c_int]),

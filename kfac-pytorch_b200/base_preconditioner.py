@@ -695,6 +695,7 @@ class BaseKFACPreconditioner:
             self._a_block_reduced = False
         if not layer.diag_a:        # integer indices are counted as they are
             x = cast_for_factor(x, layer.factor_dtype)
+        x = layer.module.prepare_input(x)
         layer.module.accumulate_a(x, layer._a_batch_view, self._scratch)
         if layer.method == ComputeMethod.EKFAC:
             n = layer.module.num_rows_a(x)

@@ -40,6 +40,38 @@ void count_launch(int n);
 inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// A kfac_conv_geometry flattened for the kernels, with its output extents.  Only the padding before an axis enters the
+// input index; the padding after it only extends the output.
+struct ConvGeo {
+  int batch, C, D, H, W, kd, kh, kw, sd, sh, sw, dd, dh, dw, pd, ph, pw, Do, Ho, Wo;
+  __host__ __device__ int64_t spatial() const { return (int64_t)Do * Ho * Wo; }
+  __host__ __device__ int64_t features() const { return (int64_t)C * kd * kh * kw; }
+};
+
+// Conv2d's geometry: depth 1, dilation 1, symmetric padding
+inline ConvGeo conv2d_geo(int batch, int C, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw) {
+  return ConvGeo{batch, C, 1, H, W, 1, kh, kw, 1, sh, sw, 1, 1, 1, 0, ph, pw,
+                 1, (H + 2 * ph - kh) / sh + 1, (W + 2 * pw - kw) / sw + 1};
+}
+
+// KFAC_OK with *o filled, or KFAC_ERR_BAD_ARG for a malformed geometry or an empty output
+inline int resolve_conv_geometry(const kfac_conv_geometry* g, ConvGeo* o) {
+  KFAC_CHECK_ARG(g != nullptr, "null geometry");
+  KFAC_CHECK_ARG(g->batch > 0 && g->C > 0, "geometry");
+  int out[3];
+  for (int a = 0; a < 3; ++a) {
+    KFAC_CHECK_ARG(g->in[a] > 0 && g->kernel[a] > 0 && g->stride[a] > 0 && g->dilation[a] > 0 &&
+                       g->pad_before[a] >= 0 && g->pad_after[a] >= 0, "geometry");
+    const int64_t span = (int64_t)g->in[a] + g->pad_before[a] + g->pad_after[a] - (int64_t)g->dilation[a] * (g->kernel[a] - 1) - 1;
+    KFAC_CHECK_ARG(span >= 0 && span / g->stride[a] + 1 < (1ll << 31), "empty output");
+    out[a] = (int)(span / g->stride[a] + 1);
+  }
+  *o = ConvGeo{g->batch, g->C, g->in[0], g->in[1], g->in[2], g->kernel[0], g->kernel[1], g->kernel[2],
+               g->stride[0], g->stride[1], g->stride[2], g->dilation[0], g->dilation[1], g->dilation[2],
+               g->pad_before[0], g->pad_before[1], g->pad_before[2], out[0], out[1], out[2]};
+  return KFAC_OK;
+}
+
 template <typename T>
 __device__ __forceinline__ float to_float(T v);
 template <>

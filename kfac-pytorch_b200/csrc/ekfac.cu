@@ -22,7 +22,7 @@ namespace {
 // ------------------------------------------------------------------ row writers
 struct RowsArgs {
   const void* x; float* out;
-  int batch, C, H, W, kh, kw, sh, sw, ph, pw, Ho, Wo;
+  ConvGeo g;
   int ones;                  // append a constant feature (scaled like the others)
   int64_t ld;                // row stride of `out` (>= d, multiple of 4); columns [d, ld) are written as 0
   float scale; const float* loss_scale;   // every value is multiplied by scale / *loss_scale (loss_scale may be null)
@@ -32,36 +32,41 @@ __device__ __forceinline__ float row_scale(float scale, const float* loss_scale)
   return loss_scale ? scale / *loss_scale : scale;
 }
 
-// out[(n, ho, wo)][(c, i, j) | ones] of an NCHW input.  A CTA moves a 32 rows x 32 features tile through shared memory:
-// it reads along the rows (neighbouring output positions) and writes along the features, both coalesced.  The 1 x 1 /
-// stride-1 case is the gather of an NCHW tensor into rows (the conv G side uses it with kh = kw = 1).
+// out[(n, do, ho, wo)][(c, l, i, j) | ones] of an NCDHW input.  A CTA moves a 32 rows x 32 features tile through shared
+// memory: it reads along the rows (neighbouring output positions) and writes along the features, both coalesced.  The
+// 1 x 1 / stride-1 case is the gather of an NCHW tensor into rows (the conv G side uses it with kh = kw = 1).
 template <typename T>
 __global__ void __launch_bounds__(256) rows_im2col_kernel(RowsArgs a) {
   __shared__ float tile[32][33];
-  const int64_t rows = (int64_t)a.batch * a.Ho * a.Wo;
-  const int nfeat = a.C * a.kh * a.kw;
+  const ConvGeo& g = a.g;
+  const int64_t rows = (int64_t)g.batch * g.Do * g.Ho * g.Wo;
+  const int nfeat = g.C * g.kd * g.kh * g.kw;
   const int64_t r0 = (int64_t)blockIdx.x * 32;
   const int f0 = blockIdx.y * 32;
   const float s = row_scale(a.scale, a.loss_scale);
   const T* __restrict__ x = reinterpret_cast<const T*>(a.x);
   {
     const int64_t r = r0 + threadIdx.x;
-    int wo = 0, ho = 0, n = 0;
+    int wo = 0, ho = 0, dz = 0, n = 0;
     if (r < rows) {
       const unsigned ur = (unsigned)r;                     // rows < 2^31 (checked by the caller)
-      wo = (int)(ur % (unsigned)a.Wo);
-      const unsigned t = ur / (unsigned)a.Wo;
-      ho = (int)(t % (unsigned)a.Ho);
-      n = (int)(t / (unsigned)a.Ho);
+      wo = (int)(ur % (unsigned)g.Wo);
+      unsigned t = ur / (unsigned)g.Wo;
+      ho = (int)(t % (unsigned)g.Ho);
+      t /= (unsigned)g.Ho;
+      dz = (int)(t % (unsigned)g.Do);
+      n = (int)(t / (unsigned)g.Do);
     }
     for (int i = threadIdx.y; i < 32; i += 8) {
       const int f = f0 + i;
       float v = 0.f;
       if (r < rows) {
         if (f < nfeat) {
-          const int j = f % a.kw, ki = (f / a.kw) % a.kh, c = f / (a.kw * a.kh);
-          const int h = ho * a.sh + ki - a.ph, w = wo * a.sw + j - a.pw;
-          if (h >= 0 && h < a.H && w >= 0 && w < a.W) v = to_float<T>(x[(((int64_t)n * a.C + c) * a.H + h) * a.W + w]) * s;
+          const int j = f % g.kw, ki = (f / g.kw) % g.kh, fl = f / (g.kw * g.kh);
+          const int l = fl % g.kd, c = fl / g.kd;
+          const int z = dz * g.sd + l * g.dd - g.pd, h = ho * g.sh + ki * g.dh - g.ph, w = wo * g.sw + j * g.dw - g.pw;
+          if (z >= 0 && z < g.D && h >= 0 && h < g.H && w >= 0 && w < g.W)
+            v = to_float<T>(x[((((int64_t)n * g.C + c) * g.D + z) * g.H + h) * g.W + w]) * s;
         } else if (f == nfeat && a.ones) {
           v = s;
         }
@@ -93,7 +98,7 @@ __global__ void __launch_bounds__(256) rows_linear_kernel(const void* xin, int64
 }
 
 static int launch_rows_im2col(const RowsArgs& a, int dtype, cudaStream_t s) {
-  const int64_t rows = (int64_t)a.batch * a.Ho * a.Wo;
+  const int64_t rows = (int64_t)a.g.batch * a.g.spatial();
   KFAC_CHECK_ARG(rows < (1ll << 31), "rows overflow");
   const dim3 grid((unsigned)ceil_div(rows, 32), (unsigned)ceil_div(a.ld, 32)), block(32, 8);
   KFAC_CHECK_ARG(grid.y <= 65535, "more than 2^21 features");
@@ -309,11 +314,23 @@ extern "C" int kfac_rows_conv2d_input(const void* x, int dtype, int batch, int C
   KFAC_CHECK_ARG(x && out, "null pointer");
   KFAC_CHECK_ARG(batch > 0 && C > 0 && H > 0 && W > 0 && kh > 0 && kw > 0 && sh > 0 && sw > 0 && ph >= 0 && pw >= 0,
                  "geometry");
-  const int Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
-  KFAC_CHECK_ARG(Ho > 0 && Wo > 0, "empty output");
+  const ConvGeo g = conv2d_geo(batch, C, H, W, kh, kw, sh, sw, ph, pw);
+  KFAC_CHECK_ARG(g.Ho > 0 && g.Wo > 0, "empty output");
   const int ones = append_ones ? 1 : 0;
-  KFAC_CHECK_ARG((int64_t)ld_out >= (int64_t)C * kh * kw + ones && ld_out % 4 == 0, "ld_out");
-  RowsArgs a{x, out, batch, C, H, W, kh, kw, sh, sw, ph, pw, Ho, Wo, ones, ld_out, scale, nullptr};
+  KFAC_CHECK_ARG((int64_t)ld_out >= g.features() + ones && ld_out % 4 == 0, "ld_out");
+  RowsArgs a{x, out, g, ones, ld_out, scale, nullptr};
+  return launch_rows_im2col(a, dtype, (cudaStream_t)stream);
+}
+
+extern "C" int kfac_rows_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom, int append_ones,
+                                    float scale, float* out, int ld_out, void* stream) {
+  KFAC_CHECK_ARG(x && out, "null pointer");
+  ConvGeo g;
+  const int rc = resolve_conv_geometry(geom, &g);
+  if (rc) return rc;
+  const int ones = append_ones ? 1 : 0;
+  KFAC_CHECK_ARG((int64_t)ld_out >= g.features() + ones && ld_out % 4 == 0, "ld_out");
+  RowsArgs a{x, out, g, ones, ld_out, scale, nullptr};
   return launch_rows_im2col(a, dtype, (cudaStream_t)stream);
 }
 
@@ -322,7 +339,7 @@ extern "C" int kfac_rows_conv2d_gradout(const void* g, int dtype, int batch, int
   KFAC_CHECK_ARG(g && out, "null pointer");
   KFAC_CHECK_ARG(batch > 0 && C > 0 && Ho > 0 && Wo > 0, "geometry");
   KFAC_CHECK_ARG(ld_out >= C && ld_out % 4 == 0, "ld_out");
-  RowsArgs a{g, out, batch, C, Ho, Wo, 1, 1, 1, 1, 0, 0, Ho, Wo, 0, ld_out, scale, loss_scale};
+  RowsArgs a{g, out, conv2d_geo(batch, C, Ho, Wo, 1, 1, 1, 1, 0, 0), 0, ld_out, scale, loss_scale};
   return launch_rows_im2col(a, dtype, (cudaStream_t)stream);
 }
 

@@ -192,20 +192,21 @@ static int launch_cov(CovArgs a, int dtype, cudaStream_t s) {
   return a.splits > 1 ? cov_reduce(a, d, a.splits, s) : KFAC_OK;
 }
 
-// im2col into a FEATURE-major fp32 matrix: out[(c,i,j)][(n,ho,wo)]
+// N-d, dilated im2col into a FEATURE-major fp32 matrix: out[(c,l,i,j)][(n,do,ho,wo)]
 struct Im2colArgs {
   const void* x; float* out;
-  int batch, C, H, W, kh, kw, sh, sw, ph, pw, Ho, Wo;
+  ConvGeo g;
   int ones;        // append a feature row of ones
   int64_t ld;      // leading dimension of the feature-major output (>= rows, multiple of 4)
 };
 // grid (ceil(ld / 4 / 256), features [+ 1]): a thread writes 4 consecutive samples of one feature row with one 16-byte
-// store; the (image, ho, wo) decomposition is done once per thread in 32-bit arithmetic and advanced incrementally
+// store; the (image, do, ho, wo) decomposition is done once per thread in 32-bit arithmetic and advanced incrementally
 // (the element-wise version spent its time in 64-bit divisions: 480 us for a 231 MB matrix, now bandwidth bound)
 template <typename T>
 __global__ void __launch_bounds__(256) im2col_kernel(Im2colArgs a) {
-  const int64_t rows = (int64_t)a.batch * a.Ho * a.Wo;
-  const int nfeat = a.C * a.kh * a.kw;
+  const ConvGeo& g = a.g;
+  const int64_t rows = (int64_t)g.batch * g.Do * g.Ho * g.Wo;
+  const int nfeat = g.C * g.kd * g.kh * g.kw;
   const int f = blockIdx.y;
   const int64_t r4 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
   if (r4 >= a.ld) return;
@@ -215,18 +216,24 @@ __global__ void __launch_bounds__(256) im2col_kernel(Im2colArgs a) {
     for (int k = 0; k < 4; ++k) v[k] = (r4 + k < rows) ? 1.f : 0.f;
   } else if (r4 < rows) {
     const T* __restrict__ x = reinterpret_cast<const T*>(a.x);
-    const int j = f % a.kw, i = (f / a.kw) % a.kh, c = f / (a.kw * a.kh);
+    const int j = f % g.kw, i = (f / g.kw) % g.kh, fl = f / (g.kw * g.kh);
+    const int l = fl % g.kd, c = fl / g.kd;
+    // input offsets of this window tap at output position 0
+    const int z0 = l * g.dd - g.pd, h0 = i * g.dh - g.ph, w0 = j * g.dw - g.pw;
     const unsigned row = (unsigned)r4;                    // rows < 2^31 (checked by the caller)
-    int wo = (int)(row % (unsigned)a.Wo);
-    const unsigned t = row / (unsigned)a.Wo;
-    int ho = (int)(t % (unsigned)a.Ho), n = (int)(t / (unsigned)a.Ho);
+    int wo = (int)(row % (unsigned)g.Wo);
+    unsigned t = row / (unsigned)g.Wo;
+    int ho = (int)(t % (unsigned)g.Ho);
+    t /= (unsigned)g.Ho;
+    int dz = (int)(t % (unsigned)g.Do), n = (int)(t / (unsigned)g.Do);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (r4 + k < rows) {
-        const int h = ho * a.sh + i - a.ph, w = wo * a.sw + j - a.pw;
-        if (h >= 0 && h < a.H && w >= 0 && w < a.W) v[k] = to_float<T>(x[(((int64_t)n * a.C + c) * a.H + h) * a.W + w]);
+        const int z = dz * g.sd + z0, h = ho * g.sh + h0, w = wo * g.sw + w0;
+        if (z >= 0 && z < g.D && h >= 0 && h < g.H && w >= 0 && w < g.W)
+          v[k] = to_float<T>(x[((((int64_t)n * g.C + c) * g.D + z) * g.H + h) * g.W + w]);
       }
-      if (++wo == a.Wo) { wo = 0; if (++ho == a.Ho) { ho = 0; ++n; } }
+      if (++wo == g.Wo) { wo = 0; if (++ho == g.Ho) { ho = 0; if (++dz == g.Do) { dz = 0; ++n; } } }
     }
   }
   *reinterpret_cast<float4*>(a.out + (int64_t)f * a.ld + r4) = make_float4(v[0], v[1], v[2], v[3]);
@@ -638,20 +645,85 @@ extern "C" int kfac_factor_linear(const void* x, int dtype, int64_t rows, int fe
   return kfac_factor_linear_strided(x, dtype, rows, features, features, append_ones, scale, acc, ws, ws_bytes, stream);
 }
 
-static bool conv_in_place(int C, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw) {
-  // 1x1 / stride 1 reads the NCHW input in place -- unless its rows (H*W floats) are not 16-byte multiples
-  // (7 x 7 maps): TMA cannot address those, so they are packed like an im2col matrix
-  return kh == 1 && kw == 1 && sh == 1 && sw == 1 && ph == 0 && pw == 0 && (((int64_t)H * W) % 4 == 0 || C < 64);
+// A kernel of all ones with unit stride and an output the size of the input reads the NCDHW input in place: it already
+// is a feature-major (C x DHW) matrix per example -- unless its rows (DHW floats) are not 16-byte multiples (7 x 7
+// maps): TMA cannot address those, so they are packed like an im2col matrix
+static bool conv_in_place(const ConvGeo& g) {
+  return g.kd == 1 && g.kh == 1 && g.kw == 1 && g.sd == 1 && g.sh == 1 && g.sw == 1 && g.pd == 0 && g.ph == 0 &&
+         g.pw == 0 && g.Do == g.D && g.Ho == g.H && g.Wo == g.W &&
+         ((int64_t)g.D * g.H * g.W % 4 == 0 || g.C < 64);
 }
 
-static CovWs conv_input_ws(int batch, int C, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw,
-                           int append_ones) {
+// workspace of a chunk of n examples: [im2col matrix (none in place)] [SYRK partials]
+static CovWs conv_chunk_ws(const ConvGeo& g, int64_t n, int append_ones) {
   const int ones = append_ones ? 1 : 0;
-  if (conv_in_place(C, H, W, kh, kw, sh, sw, ph, pw)) return CovWs(0, C + ones, (int64_t)H * W, batch);
-  const int64_t Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
-  const int64_t rows = (int64_t)batch * Ho * Wo, ld = (rows + 3) / 4 * 4;
-  const int d = C * kh * kw + ones;
-  return CovWs((size_t)ld * d * sizeof(float), d, rows, 1);
+  if (conv_in_place(g)) return CovWs(0, g.C + ones, (int64_t)g.D * g.H * g.W, g.batch);
+  const int64_t rows = n * g.spatial(), ld = (rows + 3) / 4 * 4;
+  const int64_t d = g.features() + ones;
+  return CovWs((size_t)ld * (size_t)d * sizeof(float), (int)d, rows, 1);
+}
+
+// the largest chunk n in [1, batch] whose workspace (with its SYRK partials, or the matrix alone) fits in `bytes`, and
+// whose rows stay below 2^31; 0 when not even one example fits.  Both sizes grow with n.
+static int conv_chunk_for(const ConvGeo& g, int ones, size_t bytes, bool with_slab) {
+  auto fits = [&](int64_t n) {
+    const CovWs w = conv_chunk_ws(g, n, ones);
+    return n * g.spatial() < (1ll << 31) && (with_slab ? w.total : w.pack) <= bytes;
+  };
+  if (!fits(1)) return 0;
+  int64_t lo = 1, hi = g.batch;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) / 2;
+    if (fits(mid)) lo = mid; else hi = mid - 1;
+  }
+  return (int)lo;
+}
+
+// acc += scale * X^T X of the im2col X, formed `chunk` examples at a time into the workspace (see the header)
+static int conv_input_factor(const void* x, int dtype, const ConvGeo& g, int append_ones, int chunk, float scale,
+                             float* acc, void* ws, size_t ws_bytes, cudaStream_t s) {
+  const int ones = append_ones ? 1 : 0;
+  CovArgs a{};
+  a.ones = ones; a.scale = scale; a.acc = acc;
+  if (conv_in_place(g)) {
+    const CovWs w = conv_chunk_ws(g, g.batch, ones);
+    const int64_t plane = (int64_t)g.D * g.H * g.W;
+    KFAC_CHECK_ARG(plane < (1ll << 31), "rows overflow");
+    a.x = x; a.ld = plane; a.batch_stride = (int64_t)g.C * plane;
+    a.rows = (int)plane; a.batch = g.batch; a.feat = g.C; a.slab = w.slab(ws, ws_bytes);
+    return launch_cov<true>(a, dtype, s);
+  }
+  const CovWs w = conv_chunk_ws(g, chunk, ones);
+  if (!ws || ws_bytes < w.pack) {
+    set_error("conv_input: workspace too small (%zu < %zu)", ws_bytes, w.pack);
+    return KFAC_ERR_WORKSPACE;
+  }
+  KFAC_CHECK_ARG((int64_t)chunk * g.spatial() < (1ll << 31), "rows overflow");
+  KFAC_CHECK_ARG(g.features() + ones <= 65535, "conv_input: more than 65535 features");
+  size_t elem;
+  if (dtype == KFAC_F32) elem = 4;
+  else if (dtype == KFAC_F16 || dtype == KFAC_BF16) elem = 2;
+  else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
+  const int64_t example = (int64_t)g.C * g.D * g.H * g.W;
+  const int d = (int)g.features() + ones;
+  for (int b0 = 0; b0 < g.batch; b0 += chunk) {
+    Im2colArgs ia{(const char*)x + (size_t)b0 * example * elem, (float*)ws, g, ones, 0};
+    ia.g.batch = std::min(chunk, g.batch - b0);
+    const int64_t rows = (int64_t)ia.g.batch * g.spatial();
+    ia.ld = (rows + 3) / 4 * 4;
+    const dim3 grid((unsigned)ceil_div(ia.ld / 4, 256), (unsigned)d);
+    if (dtype == KFAC_F32) im2col_kernel<float><<<grid, 256, 0, s>>>(ia);
+    else if (dtype == KFAC_F16) im2col_kernel<__half><<<grid, 256, 0, s>>>(ia);
+    else im2col_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(ia);
+    KFAC_LAUNCH_CHECK();
+    // the ones row is materialised, so the SYRK sees d = C*kd*kh*kw + ones plain features
+    CovArgs c = a;
+    c.x = ws; c.ld = ia.ld; c.batch_stride = 0; c.rows = (int)rows; c.batch = 1; c.feat = d; c.ones = 0;
+    c.slab = w.slab(ws, ws_bytes);
+    const int rc = launch_cov<true>(c, KFAC_F32, s);
+    if (rc) return rc;
+  }
+  return KFAC_OK;
 }
 
 extern "C" size_t kfac_factor_conv2d_input_workspace_bytes(int batch, int C, int H, int W, int kh,
@@ -659,7 +731,7 @@ extern "C" size_t kfac_factor_conv2d_input_workspace_bytes(int batch, int C, int
                                                            int append_ones) {
   if (batch <= 0 || C <= 0 || H <= 0 || W <= 0 || kh <= 0 || kw <= 0 || sh <= 0 || sw <= 0 || ph < 0 || pw < 0) return 0;
   if ((H + 2 * ph - kh) / sh + 1 <= 0 || (W + 2 * pw - kw) / sw + 1 <= 0) return 0;
-  return conv_input_ws(batch, C, H, W, kh, kw, sh, sw, ph, pw, append_ones).total;
+  return conv_chunk_ws(conv2d_geo(batch, C, H, W, kh, kw, sh, sw, ph, pw), batch, append_ones).total;
 }
 
 extern "C" int kfac_factor_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W,
@@ -669,37 +741,39 @@ extern "C" int kfac_factor_conv2d_input(const void* x, int dtype, int batch, int
   KFAC_CHECK_ARG(x && acc, "null pointer");
   KFAC_CHECK_ARG(batch > 0 && C > 0 && H > 0 && W > 0 && kh > 0 && kw > 0 && sh > 0 && sw > 0 &&
                      ph >= 0 && pw >= 0, "geometry");
-  cudaStream_t s = (cudaStream_t)stream;
-  const int Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
-  KFAC_CHECK_ARG(Ho > 0 && Wo > 0, "empty output");
-  const CovWs w = conv_input_ws(batch, C, H, W, kh, kw, sh, sw, ph, pw, append_ones);
-  CovArgs a{};
-  a.ones = append_ones ? 1 : 0; a.scale = scale; a.acc = acc; a.slab = w.slab(ws, ws_bytes);
-  if (conv_in_place(C, H, W, kh, kw, sh, sw, ph, pw)) {
-    // 1x1 / stride 1: the NCHW input already is a feature-major (C x HW) matrix per image
-    a.x = x; a.ld = (int64_t)H * W; a.batch_stride = (int64_t)C * H * W;
-    a.rows = H * W; a.batch = batch; a.feat = C;
-    return launch_cov<true>(a, dtype, s);
+  const ConvGeo g = conv2d_geo(batch, C, H, W, kh, kw, sh, sw, ph, pw);
+  KFAC_CHECK_ARG(g.Ho > 0 && g.Wo > 0, "empty output");
+  return conv_input_factor(x, dtype, g, append_ones, batch, scale, acc, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+extern "C" size_t kfac_factor_conv_input_workspace_bytes(const kfac_conv_geometry* geom, int append_ones,
+                                                         size_t max_bytes) {
+  ConvGeo g;
+  if (resolve_conv_geometry(geom, &g) != KFAC_OK) return 0;
+  const int ones = append_ones ? 1 : 0;
+  if (conv_in_place(g)) return conv_chunk_ws(g, g.batch, ones).total;
+  // the largest chunk whose matrix and SYRK partials fit; else one example (beyond max_bytes when it alone does not fit)
+  const int n = std::max(1, conv_chunk_for(g, ones, max_bytes, true));
+  return conv_chunk_ws(g, n, ones).total;
+}
+
+extern "C" int kfac_factor_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom, int append_ones,
+                                      float scale, float* acc, void* ws, size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(x && acc, "null pointer");
+  ConvGeo g;
+  const int rc = resolve_conv_geometry(geom, &g);
+  if (rc) return rc;
+  const int ones = append_ones ? 1 : 0;
+  int chunk = g.batch;
+  if (!conv_in_place(g)) {
+    chunk = conv_chunk_for(g, ones, ws_bytes, true);
+    if (chunk == 0) chunk = conv_chunk_for(g, ones, ws_bytes, false);   // one matrix, unsplit SYRK
+    if (chunk == 0) {
+      set_error("conv_input: workspace too small for one example (%zu < %zu)", ws_bytes, conv_chunk_ws(g, 1, ones).pack);
+      return KFAC_ERR_WORKSPACE;
+    }
   }
-  if (!ws || ws_bytes < w.pack) {
-    set_error("conv2d_input: workspace too small (%zu < %zu)", ws_bytes, w.pack);
-    return KFAC_ERR_WORKSPACE;
-  }
-  const int64_t rows = (int64_t)batch * Ho * Wo;
-  KFAC_CHECK_ARG(rows < (1ll << 31), "rows overflow");
-  const int64_t ld = (rows + 3) / 4 * 4;
-  Im2colArgs ia{x, (float*)ws, batch, C, H, W, kh, kw, sh, sw, ph, pw, Ho, Wo, a.ones, ld};
-  KFAC_CHECK_ARG((int64_t)C * kh * kw + a.ones <= 65535, "conv2d_input: more than 65535 features");
-  const dim3 grid((unsigned)ceil_div(ld / 4, 256), (unsigned)(C * kh * kw + a.ones));
-  if (dtype == KFAC_F32) im2col_kernel<float><<<grid, 256, 0, s>>>(ia);
-  else if (dtype == KFAC_F16) im2col_kernel<__half><<<grid, 256, 0, s>>>(ia);
-  else if (dtype == KFAC_BF16) im2col_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(ia);
-  else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
-  KFAC_LAUNCH_CHECK();
-  // the ones row is materialised, so the SYRK sees d = C*kh*kw + ones plain features
-  a.x = ws; a.ld = ld; a.batch_stride = 0; a.rows = (int)rows; a.batch = 1; a.feat = C * kh * kw + a.ones;
-  a.ones = 0;
-  return launch_cov<true>(a, KFAC_F32, s);
+  return conv_input_factor(x, dtype, g, ones, chunk, scale, acc, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 static CovWs gradout_ws(int batch, int C, int Ho, int Wo) {
@@ -725,7 +799,7 @@ extern "C" int kfac_factor_conv2d_gradout(const void* g, int dtype, int batch, i
     const int64_t rows = (int64_t)batch * Ho * Wo;
     KFAC_CHECK_ARG(rows < (1ll << 31), "rows overflow");
     const int64_t ld = (rows + 3) / 4 * 4;
-    Im2colArgs ia{g, (float*)ws, batch, C, Ho, Wo, 1, 1, 1, 1, 0, 0, Ho, Wo, 0, ld};
+    Im2colArgs ia{g, (float*)ws, conv2d_geo(batch, C, Ho, Wo, 1, 1, 1, 1, 0, 0), 0, ld};
     KFAC_CHECK_ARG(C <= 65535, "conv2d_gradout: more than 65535 channels");
     const dim3 grid((unsigned)ceil_div(ld / 4, 256), (unsigned)C);
     if (dtype == KFAC_F32) im2col_kernel<float><<<grid, 256, 0, s>>>(ia);

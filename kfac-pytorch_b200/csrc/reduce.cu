@@ -2,7 +2,8 @@
 // positions of the example's expand rows (those the kfac_rows_* writers form), times scale / *loss_scale.
 //
 //   linear          (B, R, features) -> B x ld_out                              a CTA per (example, 32 columns)
-//   conv2d_input    NCHW -> B x ld_out, features (C, kh, kw) [+ ones]          a CTA per (example, channel) plane
+//   conv_input      NCDHW -> B x ld_out, features (C, kd, kh, kw) [+ ones]     a CTA per (example, channel) volume,
+//                                                                              or per (example, channel, tap) of a Conv1d
 //   conv2d_gradout  NCHW -> B x ld_out, features C                             a warp per (example, channel) plane
 //
 // Every input element is read from HBM once (the conv input's window sums re-read a plane row from L1 only).  Sums run
@@ -58,60 +59,85 @@ __global__ void __launch_bounds__(256) reduce_linear_kernel(const T* __restrict_
   out[b * ld + f] = v;
 }
 
-// Window sums of one (b, c) plane: out[b][(c, i, j)] = scale * sum_{ho, wo} xpad[ho sh + i - ph][wo sw + j - pw].
-// Separable: rowsum[h][j] = sum_wo x[h][wo sw + j - pw] for a chunk of rows (a thread per (h, j), so a row is read once
-// from HBM and re-read from L1 for the other j), then acc[i][j] += sum_ho rowsum[ho sh + i - ph][j] in row order (a
-// thread per (i, j), the same thread for every chunk).  Rows no window touches are not read.
-constexpr int CONV_SMEM = 2048;   // doubles of rowsum per chunk, and the most (i, j) pairs of a CTA
+// Window sums of one (b, c) volume:
+//   out[b][(c, l, i, j)] = scale * sum_{do, ho, wo} xpad[do sd + l dd - pd][ho sh + i dh - ph][wo sw + j dw - pw].
+// Separable: the volume is a sequence of D * H rows (z, h) of W elements.  rowsum[(z, h)][j] = sum_wo x[z][h][wo sw +
+// j dw - pw] for a chunk of rows (a thread per (row, j), so a row is read once from HBM and re-read from L1 for the other
+// j), then acc[l][i][j] += rowsum[(z, h)][j] over the chunk's rows on the lattice of (l, i), in row order (a thread per
+// (l, i, j), the same thread for every chunk).  Rows no window touches are not read.
+constexpr int CONV_SMEM = 2048;   // doubles of rowsum per chunk, and the most (l, i, j) taps of a CTA
+
+// the row index q of an axis is on the output lattice of window offset k: q = o s + k dil - p with 0 <= o < n_out
+__device__ __forceinline__ bool on_lattice(int q, int k, int s, int dil, int p, int n_out) {
+  const int t = q + p - k * dil;
+  return t >= 0 && t % s == 0 && t / s < n_out;
+}
+
+// fp32 sum of x[wo s] over one run [w0, w1), in order
+template <typename T>
+__device__ __forceinline__ float run_sum(const T* __restrict__ row, int w0, int w1, int s) {
+  float acc = 0.f;
+  for (int wo = w0; wo < w1; ++wo) acc += to_float<T>(row[wo * s]);
+  return acc;
+}
+
+// the output columns [lo, hi] whose tap j lies inside a row of W elements (hi < lo: none)
+__device__ __forceinline__ void tap_range(const ConvGeo& g, int j, int& lo, int& hi) {
+  const int off = j * g.dw - g.pw;   // input column of output column 0
+  lo = off < 0 ? (-off + g.sw - 1) / g.sw : 0;
+  hi = g.W - 1 - off < 0 ? -1 : min(g.Wo - 1, (g.W - 1 - off) / g.sw);
+}
+
+// the ones column and the zero padding of an example's row, written once per example
+__device__ __forceinline__ void ones_and_padding(const ConvGeo& g, int ones, double sc, float* o, int64_t ld) {
+  const int64_t d = g.features();
+  for (int64_t f = d + threadIdx.x; f < ld; f += blockDim.x)
+    o[f] = (f == d && ones) ? (float)((double)g.spatial() * sc) : 0.f;
+}
 
 template <typename T>
-__global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restrict__ x, int C, int H, int W, int kh,
-                                                                int kw, int sh, int sw, int ph, int pw, int Ho, int Wo,
-                                                                int ones, float scale, float* out, int64_t ld) {
+__global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restrict__ x, const ConvGeo g, int ones,
+                                                                float scale, float* out, int64_t ld) {
   __shared__ double rowsum[CONV_SMEM];
   __shared__ double pacc[CONV_SMEM];
   const int64_t plane = blockIdx.x;
-  const int64_t b = plane / C;
-  const int c = (int)(plane - b * C);
-  const T* __restrict__ xp = x + plane * H * W;
-  const int P = kh * kw;
-  const int HC = max(1, min(H, CONV_SMEM / kw));
+  const int64_t b = plane / g.C;
+  const int c = (int)(plane - b * g.C);
+  const int kw = g.kw;
+  const int NR = g.D * g.H;
+  const T* __restrict__ xp = x + plane * NR * g.W;
+  const int P = g.kd * g.kh * kw;
+  const int HC = max(1, min(NR, CONV_SMEM / kw));
   for (int p = threadIdx.x; p < P; p += blockDim.x) pacc[p] = 0.0;
-  for (int h0 = 0; h0 < H; h0 += HC) {
-    const int hc = min(HC, H - h0);
+  for (int r0 = 0; r0 < NR; r0 += HC) {
+    const int hc = min(HC, NR - r0);
     for (int e = threadIdx.x; e < hc * kw; e += blockDim.x) {
-      const int r = e / kw, j = e - r * kw, h = h0 + r;
-      // the rows of window offset i are h = ho sh + i - ph, 0 <= ho < Ho
-      bool used = false;
-      for (int i = 0; i < kh && !used; ++i) {
-        const int q = h + ph - i;
-        used = q >= 0 && q % sh == 0 && q / sh < Ho;
-      }
+      const int r = e / kw, j = e - r * kw, q = r0 + r, z = q / g.H, h = q - z * g.H;
+      bool used_z = false, used_h = false;
+      for (int l = 0; l < g.kd && !used_z; ++l) used_z = on_lattice(z, l, g.sd, g.dd, g.pd, g.Do);
+      for (int i = 0; i < g.kh && !used_h; ++i) used_h = on_lattice(h, i, g.sh, g.dh, g.ph, g.Ho);
       double acc = 0.0;
-      if (used) {
-        // wo with 0 <= wo sw + j - pw < W
-        const int lo = j < pw ? (pw - j + sw - 1) / sw : 0;
-        const int hi = W - 1 + pw - j < 0 ? -1 : min(Wo - 1, (W - 1 + pw - j) / sw);
-        const T* __restrict__ row = xp + (int64_t)h * W + j - pw;
-        for (int w0 = lo; w0 <= hi; w0 += RUN) {
-          float s = 0.f;
-          const int w1 = min(hi + 1, w0 + RUN);
-          for (int wo = w0; wo < w1; ++wo) s += to_float<T>(row[wo * sw]);
-          acc += (double)s;
-        }
+      if (used_z && used_h) {
+        int lo, hi;
+        tap_range(g, j, lo, hi);
+        const T* __restrict__ row = xp + (int64_t)q * g.W + j * g.dw - g.pw;
+        for (int w0 = lo; w0 <= hi; w0 += RUN) acc += (double)run_sum(row, w0, min(hi + 1, w0 + RUN), g.sw);
       }
       rowsum[e] = acc;
     }
     __syncthreads();
     for (int p = threadIdx.x; p < P; p += blockDim.x) {
-      const int i = p / kw, j = p - i * kw;
+      const int j = p % kw, i = (p / kw) % g.kh, l = p / (kw * g.kh);
       double acc = pacc[p];
-      // first row of the chunk on the lattice of i, then every sh-th row
-      int q = h0 + ph - i;
-      int r = q <= 0 ? -q : (sh - q % sh) % sh;
-      for (; r < hc; r += sh) {
-        if ((h0 + r + ph - i) / sh >= Ho) break;
-        acc += rowsum[r * kw + j];
+      for (int z = r0 / g.H; z <= (r0 + hc - 1) / g.H; ++z) {
+        if (!on_lattice(z, l, g.sd, g.dd, g.pd, g.Do)) continue;
+        const int hlo = max(0, r0 - z * g.H), hhi = min(g.H, r0 + hc - z * g.H);
+        // first row of the chunk on the lattice of i, then every sh-th row
+        const int q = hlo + g.ph - i * g.dh;
+        for (int h = hlo + (q <= 0 ? -q : (g.sh - q % g.sh) % g.sh); h < hhi; h += g.sh) {
+          if ((h + g.ph - i * g.dh) / g.sh >= g.Ho) break;
+          acc += rowsum[(z * g.H + h - r0) * kw + j];
+        }
       }
       pacc[p] = acc;
     }
@@ -120,11 +146,44 @@ __global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restr
   const double sc = (double)scale;
   float* o = out + b * ld;
   for (int p = threadIdx.x; p < P; p += blockDim.x) o[(int64_t)c * P + p] = (float)(pacc[p] * sc);
-  if (c == 0) {   // the ones column and the padding of the example's row
-    const int64_t d = (int64_t)C * P;
-    for (int64_t f = d + threadIdx.x; f < ld; f += blockDim.x)
-      o[f] = (f == d && ones) ? (float)((double)Ho * Wo * sc) : 0.f;
+  if (c == 0) ones_and_padding(g, ones, sc, o, ld);
+}
+
+// A single-row input (a Conv1d: D = H = 1, kd = kh = 1, no depth or height padding, Do = Ho = 1).  reduce_conv_input_kernel would give one thread
+// per tap j a whole signal; here a CTA per (b, c, j) forms the fp32 runs of the tap's sum in parallel and one thread
+// adds them in fp64 in run order -- the order of reduce_conv_input_kernel, so both give the same bits.
+template <typename T>
+__global__ void __launch_bounds__(256) reduce_conv_input_1d_kernel(const T* __restrict__ x, const ConvGeo g, int ones,
+                                                                   float scale, float* out, int64_t ld) {
+  __shared__ double runs[CONV_SMEM];
+  const int64_t plane = blockIdx.x;
+  const int64_t b = plane / g.C;
+  const int c = (int)(plane - b * g.C);
+  const int j = blockIdx.y;
+  int lo, hi;
+  tap_range(g, j, lo, hi);
+  const T* __restrict__ row = x + plane * g.W + j * g.dw - g.pw;
+  const int n = hi >= lo ? (hi - lo) / RUN + 1 : 0;
+  double acc = 0.0;
+  for (int k0 = 0; k0 < n; k0 += CONV_SMEM) {
+    const int kn = min(CONV_SMEM, n - k0);
+    for (int k = threadIdx.x; k < kn; k += blockDim.x) {
+      const int w0 = lo + (k0 + k) * RUN;
+      runs[k] = (double)run_sum(row, w0, min(hi + 1, w0 + RUN), g.sw);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0)
+      for (int k = 0; k < kn; ++k) acc += runs[k];
+    __syncthreads();
   }
+  const double sc = (double)scale;
+  float* o = out + b * ld;
+  if (threadIdx.x == 0) {
+    double t = 0.0;   // as pacc in reduce_conv_input_kernel: 0 + acc (a signed zero becomes +0 there too)
+    t += acc;
+    o[(int64_t)c * g.kw + j] = (float)(t * sc);
+  }
+  if (c == 0 && j == 0) ones_and_padding(g, ones, sc, o, ld);
 }
 
 // out[b][c] = s * sum of the (b, c) plane of S elements (c < C), 0 for c in [C, ld): a warp per (b, c) of B x ld
@@ -195,32 +254,56 @@ extern "C" int kfac_reduce_rows_linear(const void* x, int dtype, int64_t B, int6
                                          loss_scale, out, ld_out, stream);
 }
 
+static int reduce_conv_input(const void* x, int dtype, const ConvGeo& g, int append_ones, float scale, float* out,
+                             int ld_out, cudaStream_t s) {
+  KFAC_CHECK_ARG((int64_t)g.kd * g.kh * g.kw <= CONV_SMEM, "kernel window of more than 2048 taps");
+  const int ones = append_ones ? 1 : 0;
+  KFAC_CHECK_ARG((int64_t)ld_out >= g.features() + ones, "ld_out");
+  KFAC_CHECK_ARG((int64_t)g.batch * g.C < (1ll << 31), "grid");
+  const unsigned planes = (unsigned)((int64_t)g.batch * g.C);
+  // the single-row kernel sums row 0 only: no depth or height padding may move the one output row off it
+  if (g.D == 1 && g.H == 1 && g.kd == 1 && g.kh == 1 && g.pd == 0 && g.ph == 0 && g.Do == 1 && g.Ho == 1) {
+    const dim3 grid(planes, (unsigned)g.kw);
+    if (dtype == KFAC_F32)
+      reduce_conv_input_1d_kernel<float><<<grid, 256, 0, s>>>((const float*)x, g, ones, scale, out, ld_out);
+    else if (dtype == KFAC_F16)
+      reduce_conv_input_1d_kernel<__half><<<grid, 256, 0, s>>>((const __half*)x, g, ones, scale, out, ld_out);
+    else if (dtype == KFAC_BF16)
+      reduce_conv_input_1d_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones, scale, out,
+                                                                      ld_out);
+    else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
+  } else {
+    if (dtype == KFAC_F32)
+      reduce_conv_input_kernel<float><<<planes, 256, 0, s>>>((const float*)x, g, ones, scale, out, ld_out);
+    else if (dtype == KFAC_F16)
+      reduce_conv_input_kernel<__half><<<planes, 256, 0, s>>>((const __half*)x, g, ones, scale, out, ld_out);
+    else if (dtype == KFAC_BF16)
+      reduce_conv_input_kernel<__nv_bfloat16><<<planes, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones, scale, out,
+                                                                     ld_out);
+    else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
+  }
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
 extern "C" int kfac_reduce_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, int W, int kh, int kw,
                                              int sh, int sw, int ph, int pw, int append_ones, float scale, float* out,
                                              int ld_out, void* stream) {
   KFAC_CHECK_ARG(x && out, "null pointer");
   KFAC_CHECK_ARG(batch > 0 && C > 0 && H > 0 && W > 0 && kh > 0 && kw > 0 && sh > 0 && sw > 0 && ph >= 0 && pw >= 0,
                  "geometry");
-  const int Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
-  KFAC_CHECK_ARG(Ho > 0 && Wo > 0, "empty output");
-  KFAC_CHECK_ARG(kh * kw <= CONV_SMEM, "kernel window of more than 2048 taps");
-  const int ones = append_ones ? 1 : 0;
-  KFAC_CHECK_ARG((int64_t)ld_out >= (int64_t)C * kh * kw + ones, "ld_out");
-  KFAC_CHECK_ARG((int64_t)batch * C < (1ll << 31), "grid");
-  cudaStream_t s = (cudaStream_t)stream;
-  const unsigned grid = (unsigned)((int64_t)batch * C);
-  if (dtype == KFAC_F32)
-    reduce_conv_input_kernel<float><<<grid, 256, 0, s>>>((const float*)x, C, H, W, kh, kw, sh, sw, ph, pw, Ho, Wo, ones,
-                                                         scale, out, ld_out);
-  else if (dtype == KFAC_F16)
-    reduce_conv_input_kernel<__half><<<grid, 256, 0, s>>>((const __half*)x, C, H, W, kh, kw, sh, sw, ph, pw, Ho, Wo, ones,
-                                                          scale, out, ld_out);
-  else if (dtype == KFAC_BF16)
-    reduce_conv_input_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, C, H, W, kh, kw, sh, sw, ph, pw,
-                                                                 Ho, Wo, ones, scale, out, ld_out);
-  else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
-  KFAC_LAUNCH_CHECK();
-  return KFAC_OK;
+  const ConvGeo g = conv2d_geo(batch, C, H, W, kh, kw, sh, sw, ph, pw);
+  KFAC_CHECK_ARG(g.Ho > 0 && g.Wo > 0, "empty output");
+  return reduce_conv_input(x, dtype, g, append_ones, scale, out, ld_out, (cudaStream_t)stream);
+}
+
+extern "C" int kfac_reduce_rows_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom, int append_ones,
+                                           float scale, float* out, int ld_out, void* stream) {
+  KFAC_CHECK_ARG(x && out, "null pointer");
+  ConvGeo g;
+  const int rc = resolve_conv_geometry(geom, &g);
+  if (rc) return rc;
+  return reduce_conv_input(x, dtype, g, append_ones, scale, out, ld_out, (cudaStream_t)stream);
 }
 
 extern "C" int kfac_reduce_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo, float scale,

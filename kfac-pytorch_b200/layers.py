@@ -9,6 +9,7 @@ happens in libkfac_b200.so.
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 import re
 from typing import Any, Callable
@@ -66,6 +67,10 @@ class ModuleHelper:
         if self.has_bias():
             g = torch.cat([g, self.module.bias.grad.view(-1, 1)], 1)
         return g
+
+    def prepare_input(self, x: torch.Tensor) -> torch.Tensor:
+        """The tensor accumulate_a, num_rows_a and write_rows_a of one call read, formed once per call."""
+        return x
 
     # native accumulation of the factor statistics of one micro-batch
     def accumulate_a(self, x: torch.Tensor, acc: torch.Tensor, scratch) -> None:
@@ -357,6 +362,197 @@ class Conv2dModuleHelper(ModuleHelper):
         _cabi.check(_cabi.load().kfac_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, Ho, Wo,
                                                           1.0 / (float(Ho * Wo) * grad_scale), loss_scale,
                                                           out.data_ptr(), _cabi.ld4(Cc), _cabi.stream_ptr()),
+                    'kfac_rows_conv2d_gradout')
+
+
+# Largest im2col chunk of a Conv1d / Conv3d factor call: a video layer's im2col is tens of times its input (r2plus1d_18
+# layer1 on 8 x 16 x 112^2 clips: 401 k rows x 576 features, 0.93 GB), so the matrix is formed a few examples at a time
+CONV_ND_WORKSPACE_BYTES = 1 << 30
+# most taps (kd * kh * kw) of a kernel whose K-FAC-reduce window sums the native kernel forms
+REDUCE_MAX_TAPS = 2048
+
+
+class ConvNdModuleHelper(ModuleHelper):
+    """torch.nn.Conv1d / Conv3d (an extension beyond the reference, opt-in through `precondition_conv_nd`).
+
+    The statistics are those of a Conv2d layer (modules.py:170-192) on the N-d lattice: rows = B * S positions
+    (S = Lo or Do * Ho * Wo), the A and G rows scaled by 1/S, A's feature order (C_in, kd, kh, kw) [+ ones], the order
+    of weight.reshape(out, -1).  Unlike Conv2d the geometry is honoured exactly: dilation on every axis, and per-axis
+    (before, after) padding from `_reversed_padding_repeated_twice` (integers, 'valid', or 'same' with torch's
+    asymmetric split).  A `padding_mode` other than 'zeros' pads the input with F.pad as the module's forward does,
+    and the statistics are formed with zero padding 0.  An unbatched input is one example.  A Conv1d is the N-d case
+    D = kd = 1, H = kh = 1.  Under K-FAC-reduce R = S with the Conv2d constants.  The A-side methods read the tensor
+    prepare_input made of the call's input (batched, contiguous, padded for a non-'zeros' padding_mode)."""
+
+    def __init__(self, module: torch.nn.Module, reduce: bool = False):
+        super().__init__(module, reduce=reduce)
+        self.nd = len(module.kernel_size)
+        # output extents of the recent A calls: the G call checks its output gradient against them
+        self._extents: list[tuple[int, ...]] = []
+
+    def check(self, name: str) -> None:
+        """Raise for what this helper cannot precondition (called at registration)."""
+        m = self.module
+        what = None
+        taps = math.prod(m.kernel_size)
+        if m.groups != 1:
+            what = f'groups={m.groups} (grouped and depthwise convolutions are not supported)'
+        elif max(self.a_factor_shape[0], m.out_channels) > _cabi.KFAC_EIGH_MAX_N:
+            what = (f'factors of {self.a_factor_shape[0]} (A) and {m.out_channels} (G), beyond the eigensolver\'s '
+                    f'{_cabi.KFAC_EIGH_MAX_N}')
+        elif self.reduce and taps > REDUCE_MAX_TAPS:
+            what = (f'a kernel of {taps} taps, beyond the {REDUCE_MAX_TAPS} of the K-FAC-reduce window sums '
+                    "(kfac_approx='reduce')")
+        if what is not None:
+            raise ValueError(f'precondition_conv_nd: "{name}" ({m.__class__.__name__}) has {what}; add it to '
+                             'skip_layers')
+
+    @property
+    def a_factor_shape(self):
+        d = self.module.in_channels * math.prod(self.module.kernel_size) + int(self.has_bias())
+        return (d, d)
+
+    @property
+    def g_factor_shape(self):
+        return (self.module.out_channels, self.module.out_channels)
+
+    def _pads(self) -> tuple[list[int], list[int]]:
+        """Per-axis (before, after) zero padding of the statistics, each in (D, H, W) order."""
+        before, after = [0, 0, 0], [0, 0, 0]
+        if self.module.padding_mode == 'zeros':
+            rp = self.module._reversed_padding_repeated_twice
+            for k in range(self.nd):            # rp lists (before, after) from the last axis to the first
+                before[2 - k], after[2 - k] = rp[2 * k], rp[2 * k + 1]
+        return before, after
+
+    def _geometry(self, shape: torch.Size) -> tuple[_cabi.ConvGeometry, tuple[int, ...]]:
+        """Native geometry and output extents of an input of `shape` (batched, padded as by prepare_input)."""
+        m = self.module
+        lead = [1] * (3 - self.nd)
+        ins = lead + list(shape[2:])
+        ker, st, dil = (lead + list(v) for v in (m.kernel_size, m.stride, m.dilation))
+        before, after = self._pads()
+        out = [(ins[a] + before[a] + after[a] - dil[a] * (ker[a] - 1) - 1) // st[a] + 1 for a in range(3)]
+        geo = _cabi.ConvGeometry(shape[0], shape[1], (C.c_int * 3)(*ins), (C.c_int * 3)(*ker), (C.c_int * 3)(*st),
+                                 (C.c_int * 3)(*dil), (C.c_int * 3)(*before), (C.c_int * 3)(*after))
+        return geo, tuple(out[3 - self.nd:])
+
+    def _batched(self, t: torch.Tensor) -> torch.Tensor:
+        return t.unsqueeze(0) if t.dim() == self.nd + 1 else t
+
+    def prepare_input(self, x: torch.Tensor) -> torch.Tensor:
+        """The batched, contiguous input the statistics read, padded here for a non-'zeros' padding_mode (once per
+        call: EKFAC's row writer reads the same tensor)."""
+        _cabi.require_device(x)
+        self._input_geometry(x.shape)       # refuses an input with an empty output
+        x = self._batched(x.detach())
+        m = self.module
+        if m.padding_mode != 'zeros':
+            x = torch.nn.functional.pad(x, m._reversed_padding_repeated_twice, mode=m.padding_mode)
+        return x if x.is_contiguous() else x.contiguous()
+
+    def _input_geometry(self, x_shape: torch.Size):
+        """(geometry, S) of a raw (unpadded, possibly unbatched) input shape."""
+        shape = list(x_shape) if len(x_shape) == self.nd + 2 else [1] + list(x_shape)
+        if self.module.padding_mode != 'zeros':
+            rp = self.module._reversed_padding_repeated_twice
+            for k in range(self.nd):
+                shape[-1 - k] += rp[2 * k] + rp[2 * k + 1]
+        geo, out = self._geometry(torch.Size(shape))
+        if min(out) <= 0:
+            raise ValueError(f'{self.module.__class__.__name__}: input of shape {tuple(x_shape)} gives an empty output')
+        return geo, math.prod(out), out
+
+    def _prepared_geometry(self, x: torch.Tensor) -> tuple[_cabi.ConvGeometry, int]:
+        """(geometry, S) of a prepare_input tensor; its output extent is recorded for the G call's check."""
+        geo, out = self._geometry(x.shape)
+        if not self._extents or self._extents[-1] != out:
+            self._extents = (self._extents + [out])[-8:]
+        return geo, math.prod(out)
+
+    def _gradout(self, g: torch.Tensor) -> tuple[torch.Tensor, int, int, int]:
+        """(batched contiguous g, B, C, S); the extent must be one an A call of this window computed."""
+        _cabi.require_device(g)
+        g = self._batched(g.detach())
+        g = g if g.is_contiguous() else g.contiguous()
+        out = tuple(g.shape[2:])
+        if self._extents and out not in self._extents:
+            raise ValueError(f'{self.module.__class__.__name__}: output gradient extent {out} does not match the '
+                             f'output extent {self._extents[-1]} computed from the input and the padding')
+        return g, g.size(0), g.size(1), math.prod(out)
+
+    def _write_reduced_a(self, x, geo, S, out_ptr, ld):
+        _cabi.check(_cabi.load().kfac_reduce_rows_conv_input(x.data_ptr(), _dtype_code(x), C.byref(geo),
+                                                             int(self.has_bias()), 1.0 / (float(S) * S), out_ptr, ld,
+                                                             _cabi.stream_ptr()), 'kfac_reduce_rows_conv_input')
+
+    def _write_reduced_g(self, g, B, Cc, S, scale, loss_scale, out_ptr, ld):
+        _cabi.check(_cabi.load().kfac_reduce_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, 1, S,
+                                                                 scale / float(S) ** 1.5, loss_scale, out_ptr, ld,
+                                                                 _cabi.stream_ptr()),
+                    'kfac_reduce_rows_conv2d_gradout')
+
+    def accumulate_a(self, x, acc, scratch):
+        geo, S = self._prepared_geometry(x)
+        B = geo.batch
+        if self.reduce and S > 1:
+            _reduced_factor(lambda p, ld: self._write_reduced_a(x, geo, S, p, ld), B, self.a_factor_shape[0], 1.0 / B,
+                            acc, scratch, x.device)
+            return
+        # rows = B*S, features scaled by 1/S  ->  scale = 1/(B*S) * 1/S^2   (modules.py:170-178)
+        scale = 1.0 / (float(B) * float(S) ** 3)
+        lib = _cabi.load()
+        ones = int(self.has_bias())
+        need = lib.kfac_factor_conv_input_workspace_bytes(C.byref(geo), ones, CONV_ND_WORKSPACE_BYTES)
+        ws = scratch.get(need, x.device)
+        # ws_bytes = need, not the scratch buffer's size: the chunking, and so the bits, depend on it
+        _cabi.check(lib.kfac_factor_conv_input(x.data_ptr(), _dtype_code(x), C.byref(geo), ones, scale, acc.data_ptr(),
+                                               ws.data_ptr() if need else None, need, _cabi.stream_ptr()),
+                    'kfac_factor_conv_input')
+
+    def accumulate_g(self, g, acc, grad_scale, scratch=None):
+        g, B, Cc, S = self._gradout(g)
+        if self.reduce and S > 1:
+            _reduced_factor(lambda p, ld: self._write_reduced_g(g, B, Cc, S, 1.0, None, p, ld), B, Cc,
+                            1.0 / (B * grad_scale * grad_scale), acc, scratch, g.device)
+            return
+        scale = 1.0 / (float(B) * float(S) ** 3 * grad_scale * grad_scale)
+        lib = _cabi.load()
+        need = lib.kfac_factor_conv2d_gradout_workspace_bytes(B, Cc, 1, S) if scratch is not None else 0
+        ws = scratch.get(need, g.device) if need else None
+        _cabi.check(lib.kfac_factor_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, 1, S, scale, acc.data_ptr(),
+                                                   ws.data_ptr() if ws is not None else None, need,
+                                                   _cabi.stream_ptr()), 'kfac_factor_conv2d_gradout')
+
+    def num_rows_a(self, x):
+        geo, out = self._geometry(x.shape)
+        S = math.prod(out)
+        return geo.batch if self.reduce and S > 1 else geo.batch * S
+
+    def num_rows_g(self, g):
+        B = g.size(0) if g.dim() == self.nd + 2 else 1
+        S = math.prod(g.shape[-self.nd:])
+        return B if self.reduce and S > 1 else B * S
+
+    def write_rows_a(self, x, out):
+        geo, S = self._prepared_geometry(x)
+        ones = int(self.has_bias())
+        ld = _cabi.ld4(self.a_factor_shape[0])
+        if self.reduce and S > 1:
+            self._write_reduced_a(x, geo, S, out.data_ptr(), ld)
+            return
+        # rows scaled by 1/S, the ones column included (modules.py:170-178)
+        _cabi.check(_cabi.load().kfac_rows_conv_input(x.data_ptr(), _dtype_code(x), C.byref(geo), ones, 1.0 / S,
+                                                      out.data_ptr(), ld, _cabi.stream_ptr()), 'kfac_rows_conv_input')
+
+    def write_rows_g(self, g, out, grad_scale, loss_scale):
+        g, B, Cc, S = self._gradout(g)
+        if self.reduce and S > 1:
+            self._write_reduced_g(g, B, Cc, S, 1.0 / grad_scale, loss_scale, out.data_ptr(), _cabi.ld4(Cc))
+            return
+        _cabi.check(_cabi.load().kfac_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, 1, S,
+                                                          1.0 / (float(S) * grad_scale), loss_scale, out.data_ptr(),
+                                                          _cabi.ld4(Cc), _cabi.stream_ptr()),
                     'kfac_rows_conv2d_gradout')
 
 
@@ -687,19 +883,23 @@ class AttentionProjectionHelper(LinearModuleHelper):
 
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
 CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
+CONV_ND_TYPES: tuple[type, ...] = (torch.nn.Conv1d, torch.nn.Conv3d)
 EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
 # SyncBatchNorm (global statistics), BatchNorm3d, GroupNorm and InstanceNorm* are not among them
 NORM_TYPES: tuple[type, ...] = (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d, torch.nn.LayerNorm, torch.nn.RMSNorm)
 
 
 def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
-                      diagonal_g: bool = False, norms: bool = False, reduce: bool = False) -> ModuleHelper | None:
-    """reduce: K-FAC-reduce statistics for Linear (dense and diagonal-G) and Conv2d layers; embeddings and
-    normalization layers keep their own statistics."""
+                      diagonal_g: bool = False, norms: bool = False, reduce: bool = False,
+                      conv_nd: bool = False) -> ModuleHelper | None:
+    """reduce: K-FAC-reduce statistics for Linear (dense and diagonal-G), Conv2d and (with conv_nd) Conv1d / Conv3d
+    layers; embeddings and normalization layers keep their own statistics."""
     if isinstance(module, LINEAR_TYPES):
         return (DiagonalGLinearModuleHelper if diagonal_g else LinearModuleHelper)(module, reduce=reduce)
     if isinstance(module, CONV2D_TYPES):
         return Conv2dModuleHelper(module, reduce=reduce)
+    if conv_nd and isinstance(module, CONV_ND_TYPES):
+        return ConvNdModuleHelper(module, reduce=reduce)
     if embeddings and isinstance(module, EMBEDDING_TYPES):
         return EmbeddingModuleHelper(module)
     if norms and isinstance(module, NORM_TYPES) and getattr(module, 'weight', None) is not None:
@@ -900,7 +1100,7 @@ def any_match(query: str, patterns: list[str]) -> bool:
 def register_modules(model: torch.nn.Module, skip_layers: list[str], precondition_embeddings: bool = False,
                      diagonal_g_layers: list[str] | None = None, precondition_norms: bool = False,
                      kfac_approx: str = 'expand', precondition_attention: bool = False,
-                     **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
+                     precondition_conv_nd: bool = False, **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
     modules (not in the reference).  diagonal_g_layers: regexes on name and class name; a registered
@@ -911,7 +1111,8 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     precondition_attention: register every torch.nn.MultiheadAttention as four projections named
     `{name}.q_proj`, `.k_proj`, `.v_proj` and `.out_proj`, keyed by their AttentionProjectionHelper
     (not in the reference); the `out_proj` leaf of an attention is then never registered as a Linear.
-    `layer.index` counts the other layers and the normalization layers separately."""
+    precondition_conv_nd: also register torch.nn.Conv1d and Conv3d modules (not in the reference); grouped ones and
+    ones whose factors exceed the eigensolver are an error.  `layer.index` counts the other layers and the normalization layers separately."""
     diagonal_g_layers = diagonal_g_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     counts = [0, 0]
@@ -933,12 +1134,15 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
             continue
         diag_g = any_match(name, diagonal_g_layers) or any_match(module.__class__.__name__, diagonal_g_layers)
         helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g,
-                                   norms=precondition_norms, reduce=kfac_approx == 'reduce')
+                                   norms=precondition_norms, reduce=kfac_approx == 'reduce',
+                                   conv_nd=precondition_conv_nd)
         if helper is None:
             continue
         if diag_g and not helper.diagonal_g:
             raise ValueError(f'diagonal_g_layers matches "{name}" ({module.__class__.__name__}): only torch.nn.Linear '
                              'layers can keep a diagonal G (add it to skip_layers or narrow the pattern)')
+        if isinstance(helper, ConvNdModuleHelper):
+            helper.check(name)
         assert module not in layers
         layer = KFACLayer(helper, **layer_kwargs)
         layer.index = counts[helper.norm]

@@ -202,6 +202,19 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     compute_method; `state_dict()` keeps both members' entries with their untied shapes.  Refused with a ValueError:
     a tied head outside `diagonal_g_layers`, a tied head with a bias, a weight owned by more than two registered
     modules or by two Linears, and EKFAC.  With `skip_layers` matching either member there is no pair.
+
+    `precondition_conv_nd=True` also registers leaf `torch.nn.Conv1d` and `torch.nn.Conv3d` modules whose parameters
+    all require grad (audio and sequence encoders, TCNs, video and volumetric models), which the reference leaves to
+    the first-order optimizer.  Their statistics are those of a Conv2d layer on the N-d lattice (rows = B * S positions,
+    S = Lo or Do * Ho * Wo, A and G rows scaled by 1/S; A's features in the order (C_in, kd, kh, kw) [+ ones] of
+    `weight.reshape(out, -1)`), but unlike Conv2d the geometry is honoured exactly: dilation on every axis, integer,
+    'valid' or 'same' padding (asymmetric where torch pads so), and a `padding_mode` other than 'zeros' by padding the
+    input as the module's forward does.  An unbatched input is one example.  A Conv1d with dilation 1 and zero padding
+    has the factors of its Conv2d twin with kernel (1, k) on the unsqueezed input.  It works with `kfac_approx`
+    ('reduce': R = S), EKFAC, `grad_scaler`, `accumulation_steps` and `factor_dtype`; see
+    `kfac_b200.layers.ConvNdModuleHelper`.  Refused with a ValueError naming the layer: `groups != 1`, an A dimension
+    C_in * kd * kh * kw (+ bias) or `out_channels` above `KFAC_EIGH_MAX_N` (8192), and a `diagonal_g_layers` match.
+    Conv2d layers are unaffected by the keyword.
     """
 
     def __init__(
@@ -234,6 +247,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         kfac_approx: str = 'expand',
         precondition_attention: bool = False,
         precondition_tied_embeddings: bool = False,
+        precondition_conv_nd: bool = False,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -318,7 +332,8 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         kfac_layers = register_modules(
             model, self.skip_layers, precondition_embeddings=precondition_embeddings,
             diagonal_g_layers=diagonal_g_layers, precondition_norms=precondition_norms, kfac_approx=kfac_approx,
-            precondition_attention=precondition_attention, method=compute_method,
+            precondition_attention=precondition_attention, precondition_conv_nd=precondition_conv_nd,
+            method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
         # normalization layers are preconditioned locally on every rank: the placement never sees them
@@ -357,6 +372,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'kfac_approx': kfac_approx,
             'precondition_attention': precondition_attention,
             'precondition_tied_embeddings': precondition_tied_embeddings,
+            'precondition_conv_nd': precondition_conv_nd,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
