@@ -269,7 +269,13 @@ typedef struct kfac_eigh_item {
 size_t kfac_eigh_workspace_bytes(const int* n, int count);
 /* max_sweeps <= 0 -> default (24 sweeps of the n <= 128 Jacobi); tol is ignored.
  * The first int of the workspace is a device status word written by the call (0 = fine, bit 0 = an
- * iteration did not converge, bit 1 = a non-finite (or |x| > 1e15) factor entry, replaced by 0, or a non-finite eigenvalue): fetch it with kfac_eigh_status(). */
+ * iteration did not converge, bit 1 = a non-finite (or |x| > 1e15) factor entry, replaced by 0, or a non-finite eigenvalue): fetch it with kfac_eigh_status().
+ * Scale: a factor whose largest finite entry of magnitude at most 1e15 is m is solved as 2^-e F with 2^-e m in
+ * [1, 2), and its eigenvalues are multiplied by 2^e, unless m lies in [1/16, 1) or is 0 (then e = 0, the result it
+ * had before the normalisation).  So the accuracy does not depend on the magnitude of F, and replacing F by 2^k F
+ * gives the same Q (and QT) bits and 2^k d whenever the largest entries of both lie outside [1/16, 1), provided the
+ * entries of both are normal floats (or zero) and at most 1e15; eigenvalues that are subnormal floats may differ by one
+ * subnormal ulp. */
 int kfac_eigh_batched(const kfac_eigh_item* items, int count, void* ws,
                       size_t ws_bytes, int max_sweeps, float tol, void* stream);
 /* asynchronous copy of the status word of the last kfac_eigh_batched() on this workspace into

@@ -39,24 +39,52 @@ __global__ void __launch_bounds__(N * 8) jacobi_small_kernel(const SmallMat* mat
   float* cs = sm + 2 * N * (N + 1);       // c[N/2], s[N/2]
   int* pq = reinterpret_cast<int*>(cs + N);
   __shared__ int sh_big;
+  __shared__ unsigned int sh_amax;
+  __shared__ float sh_floor;
+  __shared__ int sh_big_signal;
   constexpr int T = N * 8;   // the 2x2-block update is latency bound: more threads = fewer serial LDS/STS
   const int tid = threadIdx.x;
   const SmallMat mt = mats[blockIdx.x];
   const int n = mt.n;
+  if (tid == 0) sh_amax = 0u;
+  __syncthreads();
   bool bad_in = false;
+  float amax = 0.f;
   for (int idx = tid; idx < N * N; idx += T) {
     const int i = idx / N, j = idx % N;
     float x = (i < n && j < n) ? mt.F[(int64_t)i * n + j] : 0.f;
-    if (!(fabsf(x) <= 1e15f)) { bad_in = true; x = 0.f; }      // same input rule as the direct solver (eigh_direct.cu)
+    if (!eigh_entry_ok(x)) { bad_in = true; x = 0.f; }
     M[i][j] = x;
     W[i][j] = (i == j) ? 1.f : 0.f;
+    amax = fmaxf(amax, fabsf(x));
   }
   if (bad_in) atomicOr(status, 2);
+  atomicMax(&sh_amax, __float_as_uint(amax));
   __syncthreads();
+  // normalise by an exact power of two (eigh_scale_exponent); the eigenvalues are scaled back on output
+  const int ex = eigh_scale_exponent(sh_amax);
+  if (ex != 0) {
+    for (int idx = tid; idx < N * N; idx += T) M[idx / N][idx % N] = ldexpf(M[idx / N][idx % N], -ex);
+    __syncthreads();
+  }
+  // noise level eps ||M||_F of the convergence test (fixed summation order: the same bits in every call)
+  for (int i = tid; i < N; i += T) {
+    float r = 0.f;
+    for (int j = 0; j < N; ++j) r = fmaf(M[i][j], M[i][j], r);
+    cs[i] = r;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float f = 0.f;
+    for (int i = 0; i < N; ++i) f += cs[i];
+    sh_floor = 0x1p-24f * sqrtf(f);
+  }
+  __syncthreads();
+  const float floor_apq = sh_floor;
   bool converged = false;
   for (int sweep = 0; sweep < max_sweeps; ++sweep) {
     int rotated_sweep = 0;
-    if (tid == 0) sh_big = 0;   // set when some |sin| >= 2e-3 in this sweep
+    if (tid == 0) { sh_big = 0; sh_big_signal = 0; }   // set when some |sin| >= 2e-3 in this sweep
     __syncthreads();
     for (int st = 0; st < N - 1; ++st) {
       int rotated = 0;
@@ -70,7 +98,10 @@ __global__ void __launch_bounds__(N * 8) jacobi_small_kernel(const SmallMat* mat
           const float t = copysignf(1.f, tau) / (fabsf(tau) + sqrtf(1.f + tau * tau));
           c = 1.f / sqrtf(1.f + t * t);   // IEEE sqrt/div: rsqrtf's bias makes column norms drift
           s = t * c;
-          if (s != 0.f) { rotated = 1; if (fabsf(s) >= 2e-3f) sh_big = 1; }
+          if (s != 0.f) {
+            rotated = 1;
+            if (fabsf(s) >= 2e-3f) { sh_big = 1; if (fabsf(apq) > floor_apq) sh_big_signal = 1; }
+          }
         }
         cs[tid] = c;
         cs[N / 2 + tid] = s;
@@ -106,9 +137,14 @@ __global__ void __launch_bounds__(N * 8) jacobi_small_kernel(const SmallMat* mat
       __syncthreads();
     }
     // all rotations tiny: the next sweep would only find second-order leftovers
-    const int big = sh_big;
+    const int big = sh_big, big_signal = sh_big_signal;
     __syncthreads();
     if (!rotated_sweep || !big) { converged = true; break; }
+    // in the null space of a rank-deficient factor app, aqq and apq are all rounding noise below eps ||M||_F: the
+    // relative test keeps rotating them by large angles at an ever smaller scale and the sweeps never end.  Those
+    // rotations are harmless, so a last sweep whose only large rotations are of noise counts as converged (the
+    // sweeps themselves are left as they are, so every factor gets the same bits as before).
+    if (sweep == max_sweeps - 1 && !big_signal) converged = true;
   }
   // M = W^T F W: rescale by the (rounding-drifted) column norms of W
   for (int j = tid; j < N; j += T) {
@@ -125,7 +161,7 @@ __global__ void __launch_bounds__(N * 8) jacobi_small_kernel(const SmallMat* mat
   }
   int bad = 0;
   for (int j = tid; j < n; j += T) {
-    const float dj = M[j][j] * cs[j] * cs[j];
+    const float dj = ldexpf(M[j][j] * cs[j] * cs[j], ex);
     if (!isfinite(dj)) bad = 2;
     mt.d[j] = fmaxf(dj, 0.f);      // clamp(min=0): kfac/layers/eigen.py:321,344
   }

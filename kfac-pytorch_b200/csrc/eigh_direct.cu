@@ -57,23 +57,37 @@ struct IoMat {
   const float* Z; float* ZT;             // eigenvectors of T (columns) -> their transpose, both np-strided
   float* Q; float* QT; int ldq;          // user outputs
   const float* dsrc; float* ddst;        // eigenvalues
+  unsigned int* amax;                    // bit pattern of max|accepted entry| (zeroed workspace int)
   int n, np;
 };
 
-// A (np x np, zero padded) <- F (n x n, ld n), grid (x, matrix).  Entries that are not finite, or so large that the squared
-// column norms of the reduction could overflow (|x| > 1e15), are replaced by 0 and reported in the status word (bit 1):
-// the solve then runs on finite data (no NaN reaches the index arithmetic of the divide and conquer) and the caller
-// sees the failure.
+// amax <- max |x| over the entries of F the input rule accepts (eigh_entry_ok), grid (x, matrix)
+__global__ void max_abs_kernel(const IoMat* mats) {
+  const IoMat mt = mats[blockIdx.y];
+  const int64_t total = (int64_t)mt.n * mt.n;
+  float m = 0.f;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const float x = mt.F[idx];
+    if (eigh_entry_ok(x)) m = fmaxf(m, fabsf(x));
+  }
+  const unsigned int bits = __reduce_max_sync(0xffffffffu, __float_as_uint(m));
+  if ((threadIdx.x & 31) == 0 && bits) atomicMax(mt.amax, bits);
+}
+
+// A (np x np, zero padded) <- 2^-e F (n x n, ld n), e = eigh_scale_exponent(amax), grid (x, matrix).  Entries the input
+// rule rejects are replaced by 0 and reported in the status word (bit 1): the solve then runs on finite data (no NaN
+// reaches the index arithmetic of the divide and conquer) and the caller sees the failure.
 __global__ void pad_copy_kernel(const IoMat* mats, int* status) {
   const IoMat mt = mats[blockIdx.y];
   const int n = mt.n, np = mt.np;
+  const int ex = eigh_scale_exponent(*mt.amax);
   const int64_t total = (int64_t)np * np;
   bool bad = false;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int i = (int)(idx / np), j = (int)(idx % np);
     float x = (i < n && j < n) ? mt.F[(int64_t)i * n + j] : 0.f;
-    if (!(fabsf(x) <= 1e15f)) { bad = true; x = 0.f; }
-    mt.A[idx] = x;
+    if (!eigh_entry_ok(x)) { bad = true; x = 0.f; }
+    mt.A[idx] = ldexpf(x, -ex);
   }
   if (bad && status) atomicOr(status, 2);
 }
@@ -96,7 +110,7 @@ __global__ void transpose_z_kernel(const IoMat* mats) {
 }
 
 // final outputs of every matrix from ZT (rows = eigenvectors): QT_user = ZT, Q_user = ZT^T (one read of the tile),
-// eigenvalues clamped at 0 (eigen.py:321,344); grid (tiles, tiles, matrix)
+// eigenvalues scaled back by 2^e and clamped at 0 (eigen.py:321,344); grid (tiles, tiles, matrix)
 __global__ void outputs_kernel(const IoMat* mats, int* status) {
   __shared__ float tile[32][33];
   const IoMat mt = mats[blockIdx.z];
@@ -116,7 +130,7 @@ __global__ void outputs_kernel(const IoMat* mats, int* status) {
   if (blockIdx.y == 0 && threadIdx.y == 0) {
     const int j = bx + threadIdx.x;
     if (j < n) {
-      const float v = mt.dsrc[j];
+      const float v = ldexpf(mt.dsrc[j], eigh_scale_exponent(*mt.amax));
       if (!isfinite(v) && status) atomicOr(status, 2);
       mt.ddst[j] = fmaxf(v, 0.f);
     }
@@ -140,7 +154,8 @@ struct MatLayout {
 
 struct Layout {
   std::vector<MatLayout> m;
-  size_t off_trd, off_jobs, off_dc, off_blocks, off_io, off_plan, plan_bytes, off_gws, gws_bytes, zero_begin, zero_end, total;
+  size_t off_trd, off_jobs, off_dc, off_blocks, off_io, off_plan, plan_bytes, off_gws, gws_bytes, off_amax, zero_begin, zero_end,
+      total;
   int nblocks;
 };
 
@@ -162,8 +177,9 @@ void make_layout(const int* n, int count, Layout& L) {
   const int grid = sytrd_max_grid();
   // everything that must start as zeros lies in ONE region (one memset per call): the reflector stores (their padding
   // is a GEMM reduction dimension), the panel, barrier and partial-scalar state of the tridiagonalisation, the two
-  // eigenvector buffers of the divide and conquer (off-diagonal blocks), S and the T factors
+  // eigenvector buffers of the divide and conquer (off-diagonal blocks), S and the T factors, the max|F| of every matrix
   L.zero_begin = off;
+  L.off_amax = take(sizeof(unsigned int) * count);
   for (int i = 0; i < count; ++i) {
     MatLayout& m = L.m[i];
     m.n = n[i]; m.np = round_up(n[i], TRD_T); m.nblk = m.np / TRD_T; m.nbt = ceil_div(n[i], BT);
@@ -349,11 +365,15 @@ int eigh_direct_run(const kfac_eigh_item* items, int count, void* ws, size_t ws_
     o.F = items[i].F; o.A = trd[i].A; o.n = m.n; o.np = m.np;
     o.Q = items[i].Q; o.QT = items[i].QT; o.ldq = items[i].ldq > 0 ? items[i].ldq : m.n;
     o.dsrc = trd[i].d; o.ddst = items[i].d;
+    o.amax = (unsigned int*)(base + L.off_amax) + i;
     o.Z = nullptr; o.ZT = nullptr;
   }
   IoMat* d_io = (IoMat*)(base + L.off_io);
   KFAC_CUDA(cudaMemcpyAsync(d_io, io.data(), sizeof(IoMat) * count, cudaMemcpyHostToDevice, s));
-  pad_copy_kernel<<<dim3(std::min(1024, ceil_div((int64_t)np_max * np_max, 256)), count), 256, 0, s>>>(d_io, status);
+  const dim3 io_grid(std::min(1024, ceil_div((int64_t)np_max * np_max, 256)), count);
+  max_abs_kernel<<<io_grid, 256, 0, s>>>(d_io);
+  KFAC_LAUNCH_CHECK();
+  pad_copy_kernel<<<io_grid, 256, 0, s>>>(d_io, status);
   KFAC_LAUNCH_CHECK();
   std::vector<TrdJob> jobs;
   make_schedule(ns.data(), count, G, jobs);

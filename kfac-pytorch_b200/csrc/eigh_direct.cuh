@@ -78,6 +78,26 @@ struct StreamPool {
 };
 StreamPool& stream_pool();
 
+// ---- input rule and normalisation shared by both size classes (eigh.cu, eigh_direct.cu)
+// Entries that are not finite, or so large that the squared column norms of the reduction could overflow
+// (|x| > 1e15), are replaced by 0 (and reported in the status word).
+__device__ __forceinline__ bool eigh_entry_ok(float x) { return fabsf(x) <= 1e15f; }
+
+// A factor whose largest accepted |entry| m lies outside [1/16, 1) is solved as 2^-e F with 2^-e m in [1, 2), and its
+// eigenvalues are multiplied back by 2^e; inside [1/16, 1) it is solved as it is (e = 0), as is a zero factor.  The
+// deflation tolerance of the divide and conquer is absolute (it assumes max|T| near 1, as LAPACK's sstedc scales T),
+// and the Householder norms underflow below |x| ~ 1e-19: a per-batch G factor of 1e-12 was solved badly.  A power of
+// two adds no rounding, so every 2^k F whose largest entry is outside [1/16, 1) gives the same Q bits and 2^k d.  The
+// band [1/16, 1) is left unscaled so that factors near the identity an EMA starts from (0.95^t I) keep the results
+// they had before this normalisation, which a training run amplifies.  `amax_bits` is the bit pattern of m
+// (non-negative floats order like their bit patterns, which lets atomicMax find it).
+__device__ __forceinline__ int eigh_scale_exponent(unsigned int amax_bits) {
+  const float m = __uint_as_float(amax_bits);
+  int e = 0;
+  if (m > 0.f) frexpf(m, &e);          // m in [2^(e-1), 2^e)
+  return (e >= -3 && e <= 0) ? 0 : e - 1;
+}
+
 size_t eigh_direct_workspace_bytes(const int* n, int count);
 // status: device int (bit 0: an iteration did not converge, bit 1: non-finite eigenvalue); may be nullptr
 int eigh_direct_run(const kfac_eigh_item* items, int count, void* ws, size_t ws_bytes, int* status, cudaStream_t s);

@@ -199,6 +199,8 @@ __global__ void __launch_bounds__(1024) dc_deflate_kernel(const DcMat* mats, con
   int* rotb = is + (int64_t)I_ROTB * n + mg.lo;
   int* cpos = is + (int64_t)I_CPOS * n + mg.lo;
   int* csrc = is + (int64_t)I_CSRC * n + mg.lo;
+  // LAPACK slaed2's deflation rule.  zmax (|z| <= 1) does not scale with T, so the tolerance is only right for a T of
+  // norm near 1: eigh_direct.cu hands over factors with max|F| in [1/16, 2) (eigh_scale_exponent), as sstedc scales T.
   const float tol = 8.f * EPS * fmaxf(dmax, zmax);
   if (tid == 0) {
     int k = 0, nd = 0, nrot = 0;
