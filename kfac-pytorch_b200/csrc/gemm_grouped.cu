@@ -67,11 +67,25 @@ struct GroupedPolicy {
     tc::tma_load_3d(a, &it.pr->tmA, bar, kc, it.m0, 0);
     tc::tma_load_3d(b, &it.pr->tmB, bar, kc, it.n0, 0);
   }
-  __device__ static void store(const Params&, const Item& it, int row, int col, float (&v)[2]) {
+  // The problem table is in global memory: read once per item, not after each of the 64 stores of a thread (which
+  // the compiler must assume may alias it).
+  struct Out {
+    float* D; int64_t ldd; int M, N, m0, n0;
+    float alpha; int epi; const float* E; int64_t lde; const float* dg; const float* da; float damping;
+    int mode, npeer; const GProb* pr;
+  };
+  __device__ static Out out(const Params&, const Item& it) {
     const GProb& p = *it.pr;
-    const int m = it.m0 + row, nb = it.n0 + col;
+    Out o;
+    o.D = p.D + (int64_t)it.sp * p.slab_stride; o.ldd = p.ldd; o.M = p.M; o.N = p.N; o.m0 = it.m0; o.n0 = it.n0;
+    o.alpha = p.alpha; o.epi = p.epi; o.E = p.E; o.lde = p.lde; o.dg = p.dg; o.da = p.da; o.damping = p.damping;
+    o.mode = p.mode; o.npeer = p.npeer; o.pr = it.pr;
+    return o;
+  }
+  __device__ static void store(const Params&, const Out& p, int row, int col, float (&v)[2]) {
+    const int m = p.m0 + row, nb = p.n0 + col;
     if (m >= p.M || nb >= p.N) return;
-    float* drow = p.D + (int64_t)it.sp * p.slab_stride + (int64_t)m * p.ldd + nb;
+    float* drow = p.D + (int64_t)m * p.ldd + nb;
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       float x = p.alpha * v[j];
@@ -96,13 +110,13 @@ struct GroupedPolicy {
       *reinterpret_cast<float2*>(drow) = make_float2(v[0], v[1]);
       // fused compute + broadcast: the same tile goes straight to the peers' copies of D (P2P over NVLink)
       for (int q = 0; q < p.npeer; ++q)
-        *reinterpret_cast<float2*>(p.peerD[q] + (int64_t)m * p.ldd + nb) = make_float2(v[0], v[1]);
+        *reinterpret_cast<float2*>(p.pr->peerD[q] + (int64_t)m * p.ldd + nb) = make_float2(v[0], v[1]);
     } else {
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
         if (nb + j >= p.N) continue;
         drow[j] = (p.mode == 1) ? drow[j] + v[j] : v[j];
-        for (int q = 0; q < p.npeer; ++q) p.peerD[q][(int64_t)m * p.ldd + nb + j] = v[j];
+        for (int q = 0; q < p.npeer; ++q) p.pr->peerD[q][(int64_t)m * p.ldd + nb + j] = v[j];
       }
     }
   }

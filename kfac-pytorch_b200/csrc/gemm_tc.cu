@@ -5,10 +5,10 @@
 //
 // One persistent CTA per SM, warp-specialised (tc_pipeline.cuh):
 //   warp 0      TMA producer   (cp.async.bulk.tensor 3-D tiles, SWIZZLE_128B)
-//   warps 1-3   splitter       (smem -> smem: lo = x - trunc_tf32(x))
-//   warps 4-11  two consumer warpgroups (12 x wgmma m64n128k8 per k-block each, then the
-//               fused epilogue from the accumulator registers -> HBM)
-// 3 smem stages x {A_hi, B_hi, A_lo, B_lo} x 16 KB = 192 KB.
+//   warps 1-3   splitter       (smem -> smem: B_lo = x - trunc_tf32(x))
+//   warps 4-11  two consumer warpgroups (A_hi / A_lo in registers, 12 x wgmma m64n128k8 per k-block
+//               each, then the fused epilogue from the accumulator registers -> HBM)
+// 4 smem stages x {A, B_hi, B_lo} x 16 KB = 192 KB.
 #include "common.cuh"
 #include "tc_pipeline.cuh"
 
@@ -50,6 +50,8 @@ struct GemmPolicy {
     return it.kb1 > it.kb0;
   }
   __device__ static int num_kb(const Params&, const Item& it) { return it.kb1 - it.kb0; }
+  using Out = Item;                // the parameters are kernel parameters already
+  __device__ static Out out(const Params&, const Item& it) { return it; }
   __device__ static void load(const Params& p, const Item& it, int kbi, uint8_t* a, uint8_t* b, uint64_t* bar) {
     const int kblocks = (p.K + TBK - 1) / TBK;
     const int kb = it.kb0 + kbi;

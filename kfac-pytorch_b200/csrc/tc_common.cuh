@@ -62,17 +62,20 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, tf32 operands (fp32 containers, 10-bit mantissa used), fp32
-// accumulators in registers; both operands K-major in shared memory.  scale_d == 0: D = A B^T.
+// accumulators in registers.  scale_d == 0: D = A B^T.  B K-major in shared memory; A from registers, a[] is this
+// thread's fragment (warp w, lane l: a[0] = A[16 w + l / 4][l % 4], a[1] = row + 8, a[2] = column + 4, a[3] = both).
 // Accumulator layout (per warpgroup): warp w, lane l, d[4 j + 2 h + i] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + i].
-__device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], uint64_t a_desc, uint64_t b_desc, int scale_d) {
+// The tensor core reads a[] asynchronously: the registers must keep their values until the wgmma_wait that
+// retires this product (hold them with wgmma_hold after that wait).
+__device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], const float* a, uint64_t b_desc, int scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
       "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
       "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1;\n\t}"
+      "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
@@ -81,9 +84,19 @@ __device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], uint64_t a_
         "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
         "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a_desc), "l"(b_desc), "r"(scale_d)
+      : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])),
+        "l"(b_desc), "r"(scale_d)
       : "memory");
 }
+
+// Keeps a register live, unchanged, up to this point (the compiler may not reuse it for another value before).
+__device__ __forceinline__ void wgmma_hold(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
+// Moves registers between warpgroups: every warp of a warpgroup executes the same call.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // --------------------------------------------------------------- descriptors
 // K-major operand tile, rows of 128 B (32 fp32), SWIZZLE_128B as written by TMA, 8-row groups 1024 B apart
