@@ -59,7 +59,7 @@ import logging
 import math
 import warnings
 from collections import defaultdict
-from typing import Any, Callable
+from typing import Any, Callable, NamedTuple
 
 import torch
 
@@ -118,6 +118,124 @@ class _Segment:
         self.numel += _storage_numel(shape)
 
 
+class Entry(NamedTuple):
+    """One second-order tensor of a layer, `layer._inv[key]`.  holder: 'A' / 'G' (that factor's inverse worker),
+    'grad' (every gradient worker of the layer) or 'all' (every rank).  A shipped entry is broadcast from its holder
+    to the layer's gradient-worker group; a receiver builds the K-major copy `kmajor` of it, if any."""
+    key: str
+    shape: tuple[int, ...]
+    holder: str
+    shipped: bool = False
+    kmajor: str | None = None
+
+
+class Layout(NamedTuple):
+    """What the preconditioner stores, computes and reads for one layer's second-order data (second_order_layout).
+    A holder is 'A' or 'G', a side 'a' or 'g'."""
+    entries: tuple[Entry, ...]
+    factors: tuple[tuple[str, tuple[tuple[KFACLayer, str], ...], str], ...]  # holder, (layer, side) read, error if unset
+    snapshots: tuple[tuple[str, KFACLayer, str, str], ...]     # holder, layer and side of a vector factor, key
+    decompositions: tuple[tuple[str, int, str, str | None, str], ...]  # side, eigensolver call, keys of Q, Q^T, eigenvalues
+    post: tuple[tuple[str, str, tuple[str, ...]], ...]         # holder, op ('dgda', 'inverse', 'tied'), keys it uses
+    needs: frozenset[str]            # keys the precondition checks are ready
+    unready: str                     # ... and its error when one is not
+    fields: tuple[tuple[str, str], ...]  # PrecondItem pointer field, key
+    item: dict[str, int]             # the item's kind and leading dimensions
+    eigen: bool                      # the item takes the eigen path of kfac_precondition
+    damped: bool = False             # the item carries the damping its data was formed with
+
+
+def second_order_layout(layer: KFACLayer) -> Layout:
+    """The one declaration of a layer's second-order data; the comm plan, the local arena, the inverse step and the
+    precondition items all follow from it.  Not defined for the head of a tied pair: its embedding carries the pair.
+
+    Eigensolver call 0 takes the dense layers' factors, call 1 the dense factors of diagonal layers and tied pairs,
+    so that the dense layers get the same schedule (and bits) with or without those.  The precondition runs on every
+    gradient worker and reads what they all hold: the shipped entries and those held by 'grad' or 'all'."""
+    a, g = layer.a_dim, layer.g_dim
+    E, ld4 = Entry, _cabi.ld4
+    head = layer.tied_head
+    if head is not None:
+        # M (built K-major by every receiver), mu and the snapshots f and h, formed on the rank that holds all four
+        # factors with Q_E, e, C (dense, ld = d, the layout the eigensolver reads) and the eigenvectors U of C
+        needs = ('tq', '_tqT', 'tmu', 'da', 'dh')
+        return Layout(
+            (E('tq', (g, g), 'G', True, '_tqT'), E('tmu', (g,), 'G', True), E('da', (a,), 'G', True),
+             E('dh', (a,), 'G', True), E('_tqT', (g, g), 'grad'), E('_qg', (g, g), 'G'), E('_qgT', (g, g), 'G'),
+             E('_dg', (g,), 'G'), E('_C', (g * g,), 'G'), E('_U', (g, g), 'G'), E('_UT', (g, g), 'G')),
+            (('G', ((layer, 'a'), (layer, 'g'), (head, 'a'), (head, 'g')),
+              'Cannot decompose the factors of a tied embedding / head pair before they have been computed'),),
+            (('G', layer, 'a', 'da'), ('G', head, 'g', 'dh')),
+            (('g', 1, '_qg', '_qgT', '_dg'),),
+            (('G', 'tied', ('_qg', '_qgT', '_dg', '_C', '_U', '_UT', 'tq', '_tqT', 'tmu')),),
+            frozenset(needs), 'The second-order data of the tied embedding / head pair has not been computed',
+            tuple(zip(('qg', 'qgT', 'dg', 'da', 'dh'), needs)),
+            dict(kind=_cabi.KFAC_ITEM_TIED, ldqa=0, ldqg=ld4(g), ld_dgda=0), eigen=False, damped=True)
+    factors = tuple((s.upper(), ((layer, s),), f'Cannot eigendecompose {s.upper()} before {s.upper()} has been computed')
+                    for s in 'ag')
+    snapshots, post = (), ()
+    if layer.diag_side:
+        # embedding (d = 'a') or diagonal-G layer (d = 'g'): the diagonal factor is its own eigendecomposition and
+        # ships as a snapshot; only the dense factor f is decomposed, and there is never a V x d dgda
+        d, f = layer.diag_side, layer.dense_side
+        D, F, n, nd = d.upper(), f.upper(), (a if f == 'a' else g), (a if d == 'a' else g)
+        snapshots = ((D, layer, d, 'd' + d),)
+        if layer.method == ComputeMethod.EIGEN:
+            entries = (E('d' + d, (nd,), D, True), E('q' + f, (n, n), F, True, f'_q{f}T'), E('d' + f, (n,), F, True),
+                       E(f'_q{f}T', (n, n), 'grad'))
+            decompositions = ((f, 1, 'q' + f, f'_q{f}T', 'd' + f),)
+            needs = {'d' + d, 'q' + f, 'd' + f}
+        else:
+            entries = (E('d' + d, (nd,), D, True), E(f + '_inv', (n, n), F, True), E('_q' + f, (n, n), F),
+                       E('_d' + f, (n,), F))
+            decompositions = ((f, 1, '_q' + f, None, '_d' + f),)
+            post = ((F, 'inverse', ('_q' + f, '_d' + f, f + '_inv')),)
+            needs = {'d' + d, f + '_inv'}
+        unready = f'The second-order data of the {"embedding" if d == "a" else "diagonal-G layer"} has not been computed'
+        item = dict(kind=_cabi.KFAC_ITEM_EMBEDDING if d == 'a' else _cabi.KFAC_ITEM_DIAG_G,
+                    ldqa=ld4(n) if f == 'a' else 0, ldqg=ld4(n) if f == 'g' else 0, ld_dgda=0)
+        eigen = layer.method == ComputeMethod.EIGEN
+    else:
+        eigen = layer.method in (ComputeMethod.EIGEN, ComputeMethod.EKFAC)
+        unready = 'Eigendecompositions for both A and G have not been computed'
+        if layer.method == ComputeMethod.EIGEN and layer.prediv_eigenvalues:
+            # A and G are colocated: their holder divides by the eigenvalue outer product before shipping
+            entries = (E('qa', (a, a), 'G', True, '_qaT'), E('qg', (g, g), 'G', True, '_qgT'),
+                       E('dgda', (g, a), 'G', True), E('_qaT', (a, a), 'grad'), E('_qgT', (g, g), 'grad'),
+                       E('_da', (a,), 'A'), E('_dg', (g,), 'G'))
+            decompositions = (('a', 0, 'qa', '_qaT', '_da'), ('g', 0, 'qg', '_qgT', '_dg'))
+            post = (('G', 'dgda', ('_dg', '_da', 'dgda')),)
+            needs = {'qa', 'qg', 'dgda'}
+        elif eigen:
+            # EKFAC ships the eigenvalues too: every rank seeds S with dg x da for a basis no window has been measured
+            # in, and forms its own dgda from S (_ekfac_update)
+            ekfac = layer.method == ComputeMethod.EKFAC
+            kT = 'all' if ekfac else 'grad'
+            entries = (E('qa', (a, a), 'A', True, '_qaT'), E('da', (a,), 'A', True),
+                       E('qg', (g, g), 'G', True, '_qgT'), E('dg', (g,), 'G', True),
+                       E('_qaT', (a, a), kT), E('_qgT', (g, g), kT)) + ((E('dgda', (g, a), 'all'),) if ekfac else ())
+            decompositions = (('a', 0, 'qa', '_qaT', 'da'), ('g', 0, 'qg', '_qgT', 'dg'))
+            needs = {'qa', 'qg', 'dgda'} if ekfac else {'qa', 'qg', 'da', 'dg'}
+        else:
+            entries = (E('a_inv', (a, a), 'A', True), E('g_inv', (g, g), 'G', True), E('_qa', (a, a), 'A'),
+                       E('_da', (a,), 'A'), E('_qg', (g, g), 'G'), E('_dg', (g,), 'G'))
+            decompositions = (('a', 0, '_qa', None, '_da'), ('g', 0, '_qg', None, '_dg'))
+            post = (('A', 'inverse', ('_qa', '_da', 'a_inv')), ('G', 'inverse', ('_qg', '_dg', 'g_inv')))
+            needs = {'a_inv', 'g_inv'}
+            unready = 'Cannot precondition gradient before A and G have been inverted'
+        item = dict(kind=_cabi.KFAC_ITEM_DENSE, ldqa=ld4(a), ldqg=ld4(g), ld_dgda=ld4(a))
+    fields = tuple((e.key.lstrip('_'), e.key) for e in entries if e.shipped or e.holder in ('grad', 'all'))
+    return Layout(entries, factors, snapshots, decompositions, post, frozenset(needs), unready, fields, item, eigen)
+
+
+def _holds(holder: str, name: str, assignment: WorkAssignment, rank: int) -> bool:
+    if holder == 'all':
+        return True
+    if holder == 'grad':
+        return assignment.is_grad_worker(name)
+    return rank == assignment.inv_worker(name, holder)
+
+
 def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignment):
     """Decide which second-order tensors this rank stores and how they are
     grouped into broadcast segments.  Pure host logic (unit-tested on CPU for
@@ -132,59 +250,13 @@ def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignm
         if not assignment.is_grad_worker(name):
             continue
         group = assignment.grad_worker_group(name)
-        a, g = layer.a_dim, layer.g_dim
-
-        def seg(src):
-            key = (id(group) if group is not None else 0, src)
-            if key not in inv:
-                inv[key] = _Segment(src, group)
-            return inv[key]
-
-        if layer.tied_head is not None:
-            # tied pair: M (K-major copy built by every receiver), mu and the snapshots f and h, from the rank that
-            # holds all four factors
-            s = seg(assignment.inv_worker(name, 'G'))
-            s.add(layer, 'tq', (g, g))
-            s.add(layer, 'tmu', (g,))
-            s.add(layer, 'da', (a,))
-            s.add(layer, 'dh', (a,))
-            continue
-        src_a = assignment.inv_worker(name, 'A')
-        src_g = assignment.inv_worker(name, 'G')
-        if layer.diag_side:
-            # embedding / diagonal-G layer: the snapshot of the diagonal factor (its own eigenvalues) and the data of
-            # the dense one; never a V x d dgda
-            d, f = layer.diag_side, layer.dense_side
-            dims, srcs = {'a': a, 'g': g}, {'a': src_a, 'g': src_g}
-            seg(srcs[d]).add(layer, 'd' + d, (dims[d],))
-            sf, n = seg(srcs[f]), dims[f]
-            if layer.method == ComputeMethod.EIGEN:
-                sf.add(layer, 'q' + f, (n, n))
-                sf.add(layer, 'd' + f, (n,))
-            else:
-                sf.add(layer, f + '_inv', (n, n))
-        elif layer.method == ComputeMethod.EIGEN:
-            if layer.prediv_eigenvalues:
-                s = seg(src_g)
-                s.add(layer, 'qa', (a, a))
-                s.add(layer, 'qg', (g, g))
-                s.add(layer, 'dgda', (g, a))
-            else:
-                sa, sg = seg(src_a), seg(src_g)
-                sa.add(layer, 'qa', (a, a))
-                sa.add(layer, 'da', (a,))
-                sg.add(layer, 'qg', (g, g))
-                sg.add(layer, 'dg', (g,))
-        elif layer.method == ComputeMethod.EKFAC:
-            # eigenvalues too: every rank seeds S with dg x da for a basis no window has been measured in
-            sa, sg = seg(src_a), seg(src_g)
-            sa.add(layer, 'qa', (a, a))
-            sa.add(layer, 'da', (a,))
-            sg.add(layer, 'qg', (g, g))
-            sg.add(layer, 'dg', (g,))
-        else:
-            seg(src_a).add(layer, 'a_inv', (a, a))
-            seg(src_g).add(layer, 'g_inv', (g, g))
+        for e in second_order_layout(layer).entries:
+            if e.shipped:
+                src = assignment.inv_worker(name, e.holder)
+                key = (id(group) if group is not None else 0, src)
+                if key not in inv:
+                    inv[key] = _Segment(src, group)
+                inv[key].add(layer, e.key, e.shape)
     grad: dict[int, _Segment] = {}
     for name, layer in layers:
         src = assignment.src_grad_worker(name)
@@ -199,6 +271,36 @@ def build_comm_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignm
             s.offset = off
             off += s.numel
     return inv_segments, grad_segments
+
+
+def build_local_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignment, rank: int):
+    """The second-order tensors `rank` keeps for itself (never communicated), in registration order: a list of
+    (layer, key, shape)."""
+    return [(layer, e.key, e.shape) for name, layer in layers if layer.tied_embedding is None
+            for e in second_order_layout(layer).entries if not e.shipped and _holds(e.holder, name, assignment, rank)]
+
+
+def build_inverse_plan(layers: list[tuple[str, KFACLayer]], assignment: WorkAssignment, rank: int):
+    """The work of `rank` at an inverse step, in launch order, in reverse registration order and A before G within a
+    layer: the snapshots of vector factors (layer, owner of the factor, its side, key), the matrices of the two
+    eigensolver calls (layer, side, Q, Q^T, eigenvalues) and the post-ops (layer, op, keys).  Raises if a factor it
+    reads has not been computed yet."""
+    snapshots, calls, post = [], ([], []), []
+    for name, layer in reversed(layers):
+        if layer.tied_embedding is not None:
+            continue
+        lay = second_order_layout(layer)
+        # the holders this rank is (a tied pair is placed by its G alone)
+        mine = {h for h, _, _ in lay.factors if rank == assignment.inv_worker(name, h)}
+        for holder, factors, error in lay.factors:
+            if holder in mine and not all(src._has_a if side == 'a' else src._has_g for src, side in factors):
+                raise RuntimeError(error)
+        snapshots += [(layer, src, side, key) for holder, src, side, key in lay.snapshots if holder in mine]
+        for side, call, q, qT, d in lay.decompositions:
+            if side.upper() in mine:
+                calls[call].append((layer, side, q, qT, d))
+        post += [(layer, op, keys) for holder, op, keys in lay.post if holder in mine]
+    return snapshots, calls, post
 
 
 def _release_peer_memory(peer_bases: list[int], own_ptr: int) -> None:
@@ -437,54 +539,10 @@ class BaseKFACPreconditioner:
                         layer._inv[key] = store
                         layer._inv_cols[key] = shape[-1]
                     off += _storage_numel(shape)
-        # local (never communicated) eigen scratch of the inverse worker
-        rank = get_rank()
-        local = 0
-        plan = []
-        for name, l in ll:
-            if l.tied_embedding is not None:
-                continue
-            if l.tied_head is not None:
-                # tied pair: M^T on the gradient workers; Q_E, e, C and the eigenvectors U of C on the rank that forms
-                # the pair's data (C is dense with ld = d, the layout the eigensolver reads)
-                d = l.g_dim
-                if self._assignment.is_grad_worker(name):
-                    plan.append((l, '_tqT', (d, d)))
-                if rank == self._assignment.inv_worker(name, 'G'):
-                    plan += [(l, '_qg', (d, d)), (l, '_qgT', (d, d)), (l, '_dg', (d,)), (l, '_C', (d * d,)),
-                             (l, '_U', (d, d)), (l, '_UT', (d, d))]
-                continue
-            mine_a = rank == self._assignment.inv_worker(name, 'A')
-            mine_g = rank == self._assignment.inv_worker(name, 'G')
-            if l.diag_side:
-                # embedding / diagonal-G layer: only the dense factor f is decomposed; its K-major basis for the GEMM
-                # engine, or the scratch of its inverse
-                f = l.dense_side
-                n = l.a_dim if f == 'a' else l.g_dim
-                if l.method == ComputeMethod.EIGEN:
-                    if self._assignment.is_grad_worker(name):
-                        plan.append((l, f'_q{f}T', (n, n)))
-                elif mine_a if f == 'a' else mine_g:
-                    plan += [(l, f'_q{f}', (n, n)), (l, f'_d{f}', (n,))]
-            elif l.method == ComputeMethod.EIGEN:
-                if self._assignment.is_grad_worker(name):
-                    # K-major (transposed) copies of the eigenbases for the GEMM engine
-                    plan += [(l, '_qaT', (l.a_dim, l.a_dim)), (l, '_qgT', (l.g_dim, l.g_dim))]
-                if l.prediv_eigenvalues:
-                    if mine_a:
-                        plan.append((l, '_da', (l.a_dim,)))
-                    if mine_g:
-                        plan.append((l, '_dg', (l.g_dim,)))
-            elif l.method == ComputeMethod.EKFAC:
-                # every rank forms its own dgda from S (never communicated)
-                plan += [(l, '_qaT', (l.a_dim, l.a_dim)), (l, '_qgT', (l.g_dim, l.g_dim)), (l, 'dgda', (l.g_dim, l.a_dim))]
-            else:
-                if mine_a:
-                    plan += [(l, '_qa', (l.a_dim, l.a_dim)), (l, '_da', (l.a_dim,))]
-                if mine_g:
-                    plan += [(l, '_qg', (l.g_dim, l.g_dim)), (l, '_dg', (l.g_dim,))]
-        for _, _, shape in plan:
-            local += _storage_numel(shape)
+        self._layouts = {l: second_order_layout(l) for _, l in ll if l.tied_embedding is None}
+        # local (never communicated) second-order data: K-major bases for the GEMM engine, eigen scratch
+        plan = build_local_plan(ll, self._assignment, get_rank())
+        local = sum(_storage_numel(shape) for _, _, shape in plan)
         self._local_arena = torch.zeros(max(local, 1), dtype=torch.float32, device=device)
         off = 0
         for l, key, shape in plan:
@@ -1006,115 +1064,44 @@ class BaseKFACPreconditioner:
         rank = get_rank()
         damping = float(self.damping)
         stream = _cabi.stream_ptr()
-        eig: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
-        eig_diag: list[tuple[torch.Tensor, torch.Tensor, torch.Tensor | None, torch.Tensor, int]] = []
-        post: list[tuple[KFACLayer, str]] = []
-        tied: list[KFACLayer] = []
-        snapshots = False
-        for name, layer in reversed(self._layer_list()):
-            if layer.tied_embedding is not None:
-                continue
-            if layer.tied_head is not None:
-                # tied pair: the snapshots f and h, E decomposed with the diagonal layers' dense factors, then the
-                # whitened H in a call of its own below.  Every rank keeps the damping the data is formed with
+        snapshots, calls, post = build_inverse_plan(self._layer_list(), self._assignment, rank)
+        # every rank keeps the damping a tied pair's data is formed with
+        for layer, lay in self._layouts.items():
+            if lay.damped:
                 layer._tied_damping = damping
-                if rank != self._assignment.inv_worker(name, 'G'):
-                    continue
-                head, I = layer.tied_head, layer._inv
-                if not (layer._has_a and layer._has_g and head._has_a and head._has_g):
-                    raise RuntimeError('Cannot decompose the factors of a tied embedding / head pair before they have '
-                                       'been computed')
-                if self._diag_status is None:
-                    self._diag_status = torch.zeros(1, dtype=torch.int32, device=self._device)
-                if not snapshots:
-                    self._diag_status.zero_()
-                    snapshots = True
-                for view, key in ((layer._a_view, 'da'), (head._g_view, 'dh')):
-                    _cabi.check(lib.kfac_diag_snapshot(view.data_ptr(), I[key].data_ptr(), view.numel(),
-                                                       self._diag_status.data_ptr(), stream), 'kfac_diag_snapshot')
-                eig_diag.append((layer._g_view, I['_qg'], I['_qgT'], I['_dg'], layer.g_dim))
-                tied.append(layer)
-                continue
-            mine_a = rank == self._assignment.inv_worker(name, 'A')
-            mine_g = rank == self._assignment.inv_worker(name, 'G')
-            if mine_a and not layer._has_a:
-                raise RuntimeError('Cannot eigendecompose A before A has been computed')
-            if mine_g and not layer._has_g:
-                raise RuntimeError('Cannot eigendecompose G before G has been computed')
-            I = layer._inv
-            if layer.diag_side:
-                # embedding / diagonal-G layer: the diagonal factor d is its own eigendecomposition; its snapshot is the
-                # one the precondition uses until the next inverse step, like the eigenvalues of a dense factor, and
-                # an entry that is not finite (or exceeds 1e15) is reported through the eigensolver's status path
-                d, f = layer.diag_side, layer.dense_side
-                mine = {'a': mine_a, 'g': mine_g}
-                if mine[d]:
-                    if self._diag_status is None:
-                        self._diag_status = torch.zeros(1, dtype=torch.int32, device=self._device)
-                    if not snapshots:
-                        self._diag_status.zero_()
-                        snapshots = True
-                    view = layer._a_view if d == 'a' else layer._g_view
-                    _cabi.check(lib.kfac_diag_snapshot(view.data_ptr(), I['d' + d].data_ptr(), view.numel(),
-                                                       self._diag_status.data_ptr(), stream), 'kfac_diag_snapshot')
-                F, n = (layer._a_view, layer.a_dim) if f == 'a' else (layer._g_view, layer.g_dim)
-                if mine[f] and layer.method == ComputeMethod.EIGEN:
-                    eig_diag.append((F, I['q' + f], I[f'_q{f}T'], I['d' + f], n))
-                elif mine[f]:
-                    eig_diag.append((F, I['_q' + f], None, I['_d' + f], n))
-                    post.append((layer, f + '_inv'))
-            elif layer.method == ComputeMethod.EIGEN:
-                if layer.prediv_eigenvalues:
-                    if mine_a:
-                        eig.append((layer._a_view, I['qa'], I['_qaT'], I['_da'], layer.a_dim))
-                    if mine_g:
-                        eig.append((layer._g_view, I['qg'], I['_qgT'], I['_dg'], layer.g_dim))
-                        post.append((layer, 'dgda'))
-                else:
-                    if mine_a:
-                        eig.append((layer._a_view, I['qa'], I['_qaT'], I['da'], layer.a_dim))
-                    if mine_g:
-                        eig.append((layer._g_view, I['qg'], I['_qgT'], I['dg'], layer.g_dim))
-            elif layer.method == ComputeMethod.EKFAC:
-                if mine_a:
-                    eig.append((layer._a_view, I['qa'], I['_qaT'], I['da'], layer.a_dim))
-                if mine_g:
-                    eig.append((layer._g_view, I['qg'], I['_qgT'], I['dg'], layer.g_dim))
-            else:
-                if mine_a:
-                    eig.append((layer._a_view, I['_qa'], None, I['_da'], layer.a_dim))
-                    post.append((layer, 'a_inv'))
-                if mine_g:
-                    eig.append((layer._g_view, I['_qg'], None, I['_dg'], layer.g_dim))
-                    post.append((layer, 'g_inv'))
-        # normalization layers: every rank snapshots its (all-reduced) blocks, which are their own decomposition; an
-        # entry that is not finite is reported like a diagonal factor's
+        # a vector factor (an embedding's A, a diagonal-G layer's G, a tied pair's f and h) is its own
+        # eigendecomposition: its snapshot is the one the precondition uses until the next inverse step, like the
+        # eigenvalues of a dense factor
+        snapshots = [(src._a_view if side == 'a' else src._g_view, layer._inv[key]) for layer, src, side, key in snapshots]
+        # normalization layers: every rank snapshots its (all-reduced) blocks, which are their own decomposition
         for name, layer in self._norm_list():
             if not layer._has_g:
                 raise RuntimeError(f'Cannot snapshot the blocks of the normalization layer "{name}" before they have '
                                    'been computed')
+            snapshots.append((layer._g_view, layer._inv['dg']))
+            layer._inv_ready.add('dg')
+        if snapshots:
+            # an entry that is not finite (or exceeds 1e15) is reported through the eigensolver's status path
             if self._diag_status is None:
                 self._diag_status = torch.zeros(1, dtype=torch.int32, device=self._device)
-            if not snapshots:
-                self._diag_status.zero_()
-                snapshots = True
-            _cabi.check(lib.kfac_diag_snapshot(layer._g_view.data_ptr(), layer._inv['dg'].data_ptr(),
-                                               layer._g_view.numel(), self._diag_status.data_ptr(), stream),
-                        'kfac_diag_snapshot')
-            layer._inv_ready.add('dg')
-        # the dense factors of diagonal layers are decomposed in a call of their own: the batched solver shares its
-        # CTAs among the matrices of a call, so the other layers get the same schedule (and bits) with or without
-        # embeddings and diagonal-G layers
-        batches = [b for b in (eig, eig_diag) if b]
+            self._diag_status.zero_()
+            for view, out in snapshots:
+                _cabi.check(lib.kfac_diag_snapshot(view.data_ptr(), out.data_ptr(), view.numel(),
+                                                   self._diag_status.data_ptr(), stream), 'kfac_diag_snapshot')
+        # a tied pair's whitened H is decomposed in a call of its own after the one of its E (_tied_inverses)
+        tied = [layer for layer, op, _ in post if op == 'tied']
+        batches = [b for b in calls if b]
         if (batches or snapshots) and self._eig_status is None:
             self._eig_status = torch.zeros(4, dtype=torch.int32).pin_memory()
             self._eig_event = torch.cuda.Event()
         for slot, batch in enumerate(batches):
             items = (_cabi.EighItem * len(batch))()
             ns = (C.c_int * len(batch))()
-            for i, (F, Q, QT, d, n) in enumerate(batch):
-                items[i] = _cabi.EighItem(F.data_ptr(), Q.data_ptr(), QT.data_ptr() if QT is not None else None,
-                                          d.data_ptr(), n, _cabi.ld4(n), None)
+            for i, (layer, side, q, qT, d) in enumerate(batch):
+                F, n = (layer._a_view, layer.a_dim) if side == 'a' else (layer._g_view, layer.g_dim)
+                I = layer._inv
+                items[i] = _cabi.EighItem(F.data_ptr(), I[q].data_ptr(), I[qT].data_ptr() if qT else None,
+                                          I[d].data_ptr(), n, _cabi.ld4(n), None)
                 ns[i] = n
             need = lib.kfac_eigh_workspace_bytes(ns, len(batch))
             ws = self._eig_scratch.get(need, self._device)
@@ -1134,19 +1121,20 @@ class BaseKFACPreconditioner:
             self._eig_slots = list(range(len(batches))) + ([2] if snapshots else []) + ([3] if tied else [])
             self._eig_event.record()
             self._eig_pending = True
-        for layer, what in post:
+        for layer, op, keys in post:
             I = layer._inv
-            if what == 'dgda':
-                _cabi.check(lib.kfac_dgda(I['_dg'].data_ptr(), I['_da'].data_ptr(), layer.g_dim,
-                                          layer.a_dim, damping, I['dgda'].data_ptr(),
-                                          _cabi.ld4(layer.a_dim), stream), 'kfac_dgda')
-            else:
-                q, d, n = (I['_qa'], I['_da'], layer.a_dim) if what == 'a_inv' else (I['_qg'], I['_dg'], layer.g_dim)
+            if op == 'dgda':
+                dg, da, dgda = keys
+                _cabi.check(lib.kfac_dgda(I[dg].data_ptr(), I[da].data_ptr(), layer.g_dim, layer.a_dim, damping,
+                                          I[dgda].data_ptr(), _cabi.ld4(layer.a_dim), stream), 'kfac_dgda')
+            elif op == 'inverse':
+                q, d, inv = keys
+                n = I[q].shape[0]
                 ld = _cabi.ld4(n)
                 need = n * ld * 4
                 ws = self._gemm_scratch.get(need, self._device)
-                _cabi.check(lib.kfac_inverse_from_eigh(q.data_ptr(), ld, d.data_ptr(), n, damping,
-                                                       I[what].data_ptr(), ld, ws.data_ptr(), need, stream),
+                _cabi.check(lib.kfac_inverse_from_eigh(I[q].data_ptr(), ld, I[d].data_ptr(), n, damping,
+                                                       I[inv].data_ptr(), ld, ws.data_ptr(), need, stream),
                             'kfac_inverse_from_eigh')
         # C2: one broadcast per (source, gradient-worker group)
         bcast = self._assignment.broadcast_inverses()
@@ -1155,15 +1143,16 @@ class BaseKFACPreconditioner:
                 self._tdc.broadcast(self._inv_arena.narrow(0, seg.offset, seg.numel), src=seg.src,
                                     group=seg.group)
             for layer, key, shape in seg.entries:
+                lay = self._layouts[layer]
+                kmajor = next(e.kmajor for e in lay.entries if e.key == key)
                 layer._inv_ready.add(key)
-                if key == 'tq':
-                    layer._inv_ready.add('_tqT')
+                if kmajor in lay.needs:
+                    layer._inv_ready.add(kmajor)
                 # a rank that RECEIVED an eigenbasis (or a tied pair's M) builds its K-major copy locally
-                if bcast and seg.src != rank and key in ('qa', 'qg', 'tq'):
+                if bcast and seg.src != rank and kmajor:
                     n, ld = shape[0], _cabi.ld4(shape[0])
-                    _cabi.check(lib.kfac_transpose(layer._inv[key].data_ptr(), ld,
-                                                   layer._inv['_' + key + 'T'].data_ptr(), ld, n, n, stream),
-                                'kfac_transpose')
+                    _cabi.check(lib.kfac_transpose(layer._inv[key].data_ptr(), ld, layer._inv[kmajor].data_ptr(), ld,
+                                                   n, n, stream), 'kfac_transpose')
 
     def _tied_inverses(self, tied: list[KFACLayer], damping: float) -> None:
         """M and mu of the tied pairs this rank forms, after the call that decomposed their E: C (whitened H), then
@@ -1257,73 +1246,23 @@ class BaseKFACPreconditioner:
         lib = _cabi.load()
         todo = [(n, l) for n, l in reversed(self._layer_list())
                 if l.tied_embedding is None and self._assignment.is_grad_worker(n)]
-        eigen = None
+        eigen = False
         items = (_cabi.PrecondItem * max(1, len(todo)))()
         fused = self._peer_p_bases is not None
         peer_arrays = []   # keep the ctypes pointer arrays alive during the call
         p_base = self._p_arena.data_ptr()
         for i, (name, layer) in enumerate(todo):
             w, b = self._grad_ptrs(layer)
+            lay = self._layouts[layer]
+            if not lay.needs <= layer._inv_ready:
+                raise RuntimeError(lay.unready)
             I = layer._inv
-            ready = layer._inv_ready
-            if layer.tied_head is not None:
-                # tied pair: M, M^T, mu, the snapshots f (da) and h (dh), and the damping they were formed with
-                if not {'tq', '_tqT', 'tmu', 'da', 'dh'} <= ready:
-                    raise RuntimeError('The second-order data of the tied embedding / head pair has not been computed')
-                items[i] = _cabi.PrecondItem(
-                    w.data_ptr(), None, _cabi.DTYPE_CODE[w.dtype], layer.g_dim, layer.a_dim, None, None,
-                    I['tq'].data_ptr(), I['_tqT'].data_ptr(), None, I['da'].data_ptr(), I['tmu'].data_ptr(), None, None,
-                    0, _cabi.ld4(layer.g_dim), 0, layer._p_store.data_ptr(), _cabi.ld4(layer.p_shape[1]), None, 0,
-                    _cabi.KFAC_ITEM_TIED, I['dh'].data_ptr(), layer._tied_damping)
-            elif layer.diag_side:
-                # embedding (d = 'a') or diagonal-G layer (d = 'g'): the diagonal factor's snapshot and the dense
-                # factor f's eigendecomposition (eigen) or inverse
-                d, f = layer.diag_side, layer.dense_side
-                eigen = layer.method == ComputeMethod.EIGEN
-                need = {'d' + d, 'q' + f, 'd' + f} if eigen else {'d' + d, f + '_inv'}
-                if not need <= ready:
-                    kind = 'embedding' if layer.diag_a else 'diagonal-G layer'
-                    raise RuntimeError(f'The second-order data of the {kind} has not been computed')
-                ptr = {k: I[k].data_ptr() for k in need}
-                if eigen:
-                    ptr[f'q{f}T'] = I[f'_q{f}T'].data_ptr()
-                n = layer.a_dim if f == 'a' else layer.g_dim
-                items[i] = _cabi.PrecondItem(
-                    w.data_ptr(), b.data_ptr() if b is not None else None, _cabi.DTYPE_CODE[w.dtype],
-                    layer.g_dim, layer.a_dim, ptr.get('qa'), ptr.get('qaT'), ptr.get('qg'), ptr.get('qgT'),
-                    None, ptr.get('da'), ptr.get('dg'), ptr.get('a_inv'), ptr.get('g_inv'),
-                    _cabi.ld4(n) if f == 'a' else 0, _cabi.ld4(n) if f == 'g' else 0, 0,
-                    layer._p_store.data_ptr(), _cabi.ld4(layer.p_shape[1]), None, 0,
-                    _cabi.KFAC_ITEM_EMBEDDING if layer.diag_a else _cabi.KFAC_ITEM_DIAG_G)
-            elif layer.method == ComputeMethod.EIGEN:
-                ok = ('qa' in ready and 'qg' in ready and
-                      ('dgda' in ready if layer.prediv_eigenvalues else ('da' in ready and 'dg' in ready)))
-                if not ok:
-                    raise RuntimeError('Eigendecompositions for both A and G have not been computed')
-                eigen = True
-            elif layer.method == ComputeMethod.EKFAC:
-                # the eigen precondition with dgda = 1 / (S + damping)
-                if not ('qa' in ready and 'qg' in ready and 'dgda' in ready):
-                    raise RuntimeError('Eigendecompositions for both A and G have not been computed')
-                eigen = True
-            else:
-                if not ('a_inv' in ready and 'g_inv' in ready):
-                    raise RuntimeError('Cannot precondition gradient before A and G have been inverted')
-                eigen = False
-
-            if not layer.diag_side:
-                def p(key):
-                    return I[key].data_ptr() if key in ready else None
-
-                eig_ok = 'qa' in ready and 'qg' in ready
-                items[i] = _cabi.PrecondItem(
-                    w.data_ptr(), b.data_ptr() if b is not None else None, _cabi.DTYPE_CODE[w.dtype],
-                    layer.g_dim, layer.a_dim,
-                    p('qa'), I['_qaT'].data_ptr() if eig_ok else None,
-                    p('qg'), I['_qgT'].data_ptr() if eig_ok else None,
-                    p('dgda'), p('da'), p('dg'), p('a_inv'), p('g_inv'),
-                    _cabi.ld4(layer.a_dim), _cabi.ld4(layer.g_dim), _cabi.ld4(layer.a_dim),
-                    layer._p_store.data_ptr(), _cabi.ld4(layer.a_dim), None, 0)
+            items[i] = _cabi.PrecondItem(
+                w.data_ptr(), b.data_ptr() if b is not None else None, _cabi.DTYPE_CODE[w.dtype], layer.g_dim,
+                layer.a_dim, P=layer._p_store.data_ptr(), ldp=_cabi.ld4(layer.p_shape[1]),
+                tied_damping=layer._tied_damping if lay.damped else 0.0, **lay.item,
+                **{field: I[key].data_ptr() for field, key in lay.fields})
+            eigen = eigen or lay.eigen
             if fused:
                 off = layer._p_store.data_ptr() - p_base
                 arr = (C.c_void_p * len(self._peer_p_bases))(*[b + off for b in self._peer_p_bases.values()])
