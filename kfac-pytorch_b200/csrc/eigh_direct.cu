@@ -219,7 +219,8 @@ double job_time(int n, int C) {
   return (double)n * (T0 + T1 * n + (BETA * (double)n * n + GAMMA * n + EPS) / C + DELTA * std::log2((double)C));
 }
 
-void make_schedule(const int* n, int count, int G, std::vector<TrdJob>& jobs) {
+// start: if given, the predicted start time of every job (same order as jobs)
+void make_schedule(const int* n, int count, int G, std::vector<TrdJob>& jobs, std::vector<double>* start = nullptr) {
   // smallest makespan M such that the CTA-time of all jobs (each sized to finish within M) fits into G * M
   auto ctas_for = [&](int ni, double M) {
     const int nb = (ni + TRD_T - 1) / TRD_T;
@@ -261,6 +262,68 @@ void make_schedule(const int* n, int count, int G, std::vector<TrdJob>& jobs) {
   std::stable_sort(placed.begin(), placed.end(), [](const Placed& a, const Placed& b) { return a.start < b.start; });
   jobs.clear();
   for (auto& p : placed) jobs.push_back(p.job);
+  if (start) {
+    start->clear();
+    for (auto& p : placed) start->push_back(p.start);
+  }
+}
+
+// ---- L2 residency plan of the tridiagonalisation -----------------------------------------------
+// Phase A of every column re-reads the whole active lower triangle of its matrix, and the block column J of tiles
+// stays active for min(n - 1, 64 (J + 1) - 1) columns.  The direct-solver matrices of a ResNet-50 batch hold ~280 MB of
+// lower tiles at once, far more than the 50 MB L2, so under LRU nearly every tile read comes from HBM.  The plan keeps
+// a trailing triangle (block columns J >= pin_j0) of selected matrices resident with evict_last and streams the rest
+// evict_first.  Block columns are taken greedily by decreasing lifetime (reads per pinned byte), so each matrix's
+// pinned set stays a contiguous trailing triangle, subject to: at every predicted instant (a job start of the
+// schedule's time model) the pinned bytes of the running jobs fit `budget`.  A matrix whose next block column does
+// not fit pins nothing more.  No L2 set-aside is used: the hints need no device-wide state.
+constexpr long long TRD_PIN_BUDGET = 8ll << 20;      // bytes; see NOTES.md (L2 residency sweep)
+long long g_pin_budget = -1;                          // test override (kfac_stage_sytrd_pin_budget); < 0: TRD_PIN_BUDGET
+
+void make_pin_plan(const int* n, int count, const std::vector<TrdJob>& jobs, const std::vector<double>& start,
+                   long long budget, std::vector<int>& pin_j0, std::vector<double>* t0 = nullptr,
+                   std::vector<double>* t1 = nullptr) {
+  pin_j0.resize(count);
+  std::vector<double> js(count, 0.0), je(count, 0.0);
+  for (size_t j = 0; j < jobs.size(); ++j) {
+    const int i = jobs[j].mat;
+    js[i] = start[j];
+    je[i] = start[j] + job_time(n[i], jobs[j].ncta);
+  }
+  for (int i = 0; i < count; ++i) pin_j0[i] = (n[i] + TRD_T - 1) / TRD_T;
+  if (t0) *t0 = js;
+  if (t1) *t1 = je;
+  if (budget <= 0) return;
+  // instants at which the set of running jobs can grow: the job starts
+  std::vector<double> inst(js);
+  std::sort(inst.begin(), inst.end());
+  inst.erase(std::unique(inst.begin(), inst.end()), inst.end());
+  std::vector<long long> load(inst.size(), 0);
+  struct Cand { int life, mat, J; };
+  std::vector<Cand> cand;
+  for (int i = 0; i < count; ++i) {
+    const int nblk = pin_j0[i];
+    for (int J = 0; J < nblk; ++J) cand.push_back({std::min(n[i] - 1, TRD_T * (J + 1) - 1), i, J});
+  }
+  // lifetime is strictly increasing in J within a matrix: each matrix's block columns come in decreasing J
+  std::sort(cand.begin(), cand.end(), [](const Cand& a, const Cand& b) {
+    if (a.life != b.life) return a.life > b.life;
+    return a.mat != b.mat ? a.mat < b.mat : a.J > b.J;
+  });
+  std::vector<char> closed(count, 0);
+  const long long tile_bytes = (long long)TRD_T * TRD_T * sizeof(float);
+  for (const Cand& c : cand) {
+    const int i = c.mat;
+    if (closed[i]) continue;
+    const long long bytes = (long long)((n[i] + TRD_T - 1) / TRD_T - c.J) * tile_bytes;   // tiles I >= J of column J
+    bool fits = true;
+    for (size_t k = 0; k < inst.size() && fits; ++k)
+      if (inst[k] >= js[i] && inst[k] < je[i] && load[k] + bytes > budget) fits = false;
+    if (!fits) { closed[i] = 1; continue; }
+    for (size_t k = 0; k < inst.size(); ++k)
+      if (inst[k] >= js[i] && inst[k] < je[i]) load[k] += bytes;
+    pin_j0[i] = c.J;
+  }
 }
 
 }  // namespace
@@ -376,7 +439,13 @@ int eigh_direct_run(const kfac_eigh_item* items, int count, void* ws, size_t ws_
   pad_copy_kernel<<<io_grid, 256, 0, s>>>(d_io, status);
   KFAC_LAUNCH_CHECK();
   std::vector<TrdJob> jobs;
-  make_schedule(ns.data(), count, G, jobs);
+  std::vector<double> start;
+  make_schedule(ns.data(), count, G, jobs, &start);
+  std::vector<int> pin_j0;
+  make_pin_plan(ns.data(), count, jobs, start, g_pin_budget >= 0 ? g_pin_budget : TRD_PIN_BUDGET, pin_j0);
+  bool any_pin = false;
+  for (int i = 0; i < count; ++i) any_pin |= pin_j0[i] < trd[i].nblk;
+  for (int i = 0; i < count; ++i) { trd[i].pin_j0 = pin_j0[i]; trd[i].stream_first = any_pin ? 1 : 0; }
   TrdMat* d_trd = (TrdMat*)(base + L.off_trd);
   TrdJob* d_jobs = (TrdJob*)(base + L.off_jobs);
   DcMat* d_dc = (DcMat*)(base + L.off_dc);
@@ -523,6 +592,7 @@ extern "C" int kfac_stage_sytrd(const float* F, int n, float* d, float* e, float
   t.e = (float*)(base + oE); t.Vp = (float*)(base + oVp); t.Wp = (float*)(base + oWp); t.part = (float*)(base + oPart);
   t.col = (float*)(base + oCol); t.cpart = (float*)(base + oC); t.bar = (unsigned int*)(base + oBar);
   t.n = n; t.np = np; t.nblk = nblk; t.ldv = np; t.Vb = nullptr;
+  t.pin_j0 = nblk; t.stream_first = 0;
   pad_copy_one_kernel<<<std::min(1024, ceil_div((int64_t)np * np, 256)), 256, 0, s>>>(F, n, t.A, np);
   KFAC_LAUNCH_CHECK();
   KFAC_CUDA(cudaMemsetAsync(t.VT, 0, (size_t)np * np * 4, s));
@@ -588,5 +658,28 @@ extern "C" int kfac_stage_schedule(const int* n, int count, int grid, int* mat, 
 }
 extern "C" int kfac_stage_sytrd_min_ctas(int n) { return kfac::sytrd_min_ctas(n); }
 
-namespace kfac { int sytrd_profile(int on, unsigned long long* out16); }
+// host-only: the L2 residency plan of the tridiagonalisation for the schedule of kfac_stage_schedule (same dims and
+// grid) under `budget` bytes (< 0: the default).  Per matrix: pin_j0 (first pinned block column; nblk = none) and the
+// predicted start / end of its job in seconds.  Returns count.
+extern "C" int kfac_stage_pin_plan(const int* n, int count, int grid, long long budget, int* pin_j0, double* t0,
+                                   double* t1) {
+  using namespace kfac;
+  if (!n || count <= 0 || grid <= 0) return 0;
+  std::vector<TrdJob> jobs;
+  std::vector<double> start, s0, s1;
+  std::vector<int> pin;
+  make_schedule(n, count, grid, jobs, &start);
+  make_pin_plan(n, count, jobs, start, budget >= 0 ? budget : TRD_PIN_BUDGET, pin, &s0, &s1);
+  for (int i = 0; i < count; ++i) { pin_j0[i] = pin[i]; t0[i] = s0[i]; t1[i] = s1[i]; }
+  return count;
+}
+// test-only: the residency budget (bytes) of the following kfac_eigh_batched calls; < 0 restores the default
+extern "C" void kfac_stage_sytrd_pin_budget(long long bytes) { kfac::g_pin_budget = bytes; }
+
+namespace kfac {
+int sytrd_profile(int on, unsigned long long* out16);
+int sytrd_job_times(unsigned long long* out, int max_jobs);
+}
 extern "C" int kfac_stage_sytrd_profile(int on, unsigned long long* out16) { return kfac::sytrd_profile(on, out16); }
+// %globaltimer (ns) at the start and end of job j of the last launch run with the profile switch on: out[2 j], out[2 j + 1]
+extern "C" int kfac_stage_sytrd_job_times(unsigned long long* out, int max_jobs) { return kfac::sytrd_job_times(out, max_jobs); }

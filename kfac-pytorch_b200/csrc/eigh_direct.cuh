@@ -31,6 +31,10 @@ struct TrdMat {
   float* cpart;    // 66 x ncta per-CTA partial scalars, transposed [scalar][cta]
   unsigned int* bar;  // group barrier counter (zeroed before launch)
   int n, np, nblk, ldv;
+  // L2 residency of the lower tiles (make_pin_plan, eigh_direct.cu): tiles of block columns J >= pin_j0 are loaded
+  // and stored evict_last (nblk: none).  The other tiles are streamed evict_first when the launch pins anything
+  // (stream_first), with the normal policy otherwise.  Hints only: the arithmetic does not depend on them.
+  int pin_j0, stream_first;
 };
 
 struct TrdJob { int mat, cta0, ncta; };

@@ -59,9 +59,46 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-// optional phase timing (CTA 0, thread 0 of every group accumulates clock64 deltas): set by kfac_stage_sytrd_profile
+// L2 eviction-priority hints for the lower tiles of A (TrdMat::pin_j0).  The loads are __ldcg with a cache policy
+// operand; the values loaded and stored are the same as without it.
+__device__ __forceinline__ uint64_t l2_policy(bool pinned, bool stream_first) {
+  uint64_t p;
+  if (pinned) asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  else if (stream_first) asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  else asm("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ float4 ldcg_hint(const float4* ptr, uint64_t pol) {
+  float4 r;
+  asm("ld.global.cg.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+      : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(ptr), "l"(pol));
+  return r;
+}
+__device__ __forceinline__ float ldcg_hint(const float* ptr, uint64_t pol) {
+  float r;
+  asm("ld.global.cg.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(r) : "l"(ptr), "l"(pol));
+  return r;
+}
+__device__ __forceinline__ void st_hint(float4* ptr, float4 v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"
+               ::"l"(ptr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
+// back to the normal priority: the 128-byte line at ptr (a pinned line must not outlive the tridiagonalisation)
+__device__ __forceinline__ void l2_unpin(const float* ptr) {
+  asm volatile("applypriority.global.L2::evict_normal [%0], 128;" ::"l"(ptr) : "memory");
+}
+
+// optional phase timing (CTA 0, thread 0 of every group accumulates clock64 deltas): set by kfac_stage_sytrd_profile,
+// which also records %globaltimer at the start and end of every job (on the job's first CTA)
 __device__ unsigned long long g_trd_prof[16];
 __device__ int g_trd_prof_on = 0;
+constexpr int MAX_TIMED_JOBS = 512;
+__device__ unsigned long long g_trd_jobtime[2 * MAX_TIMED_JOBS];
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 #define TRD_STAMP(i) do { if (prof) { const long long t__ = clock64(); if (tid == 0) atomicAdd(&g_trd_prof[i], (unsigned long long)(t__ - tprev)); tprev = t__; } } while (0)
 
 constexpr int MAXT = 256;                   // owned tiles per sub-group (list in shared memory)
@@ -168,6 +205,8 @@ __device__ void tridiagonalise(const TrdMat& mt, int cta, int ncta, float* smem)
   float* const col = mt.col;
   float* const cpart = mt.cpart;
   const float* __restrict__ A = mt.A;
+  const int pin_j0 = mt.pin_j0;
+  const bool sfirst = mt.stream_first != 0;
 
   if (n == 1) {
     if (cta == 0 && tid == 0) { mt.d[0] = mt.A[0]; mt.tau[0] = 0.f; mt.e[0] = 0.f; }
@@ -298,9 +337,10 @@ __device__ void tridiagonalise(const TrdMat& mt, int cta, int ncta, float* smem)
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           float4* p = reinterpret_cast<float4*>(&mt.A[(int64_t)(I * T + ty * 4 + i) * np + J * T + tx * 4]);
-          float4 a = __ldcg(p);
+          const uint64_t pol = l2_policy(J >= pin_j0, sfirst);
+          float4 a = ldcg_hint(p, pol);
           a.x -= acc[i][0].x; a.y -= acc[i][0].y; a.z -= acc[i][1].x; a.w -= acc[i][1].y;
-          *p = a;
+          st_hint(p, a, pol);
         }
       }
       P = 0;
@@ -332,14 +372,22 @@ __device__ void tridiagonalise(const TrdMat& mt, int cta, int ncta, float* smem)
       float* cs = stage + sg8 * (4 * T);             // column partial sums: [4 warps][64]
       const int st_tid = tid & 127;
       const int hl = lane & 15, h8 = (lane >> 4) * 8;
+      if (s1 % T == 0 && b0 - 1 >= pin_j0) {         // block column b0 - 1 has left the active set: unpin its lines
+        for (int ti = 0; ti < ntile8; ++ti) {
+          const int I = tlist8[ti].x, J = tlist8[ti].y;
+          if (J < b0 - 1) break;
+          if (J == b0 - 1) l2_unpin(A + (int64_t)(I * T + (st_tid >> 1)) * np + J * T + (st_tid & 1) * 32);
+        }
+      }
       for (int ti = 0; ti < ntile8; ++ti) {
         const int I = tlist8[ti].x, J = tlist8[ti].y;
         if (J < b0) break;                           // the active tiles are a prefix of the list
         const int rb = I * T + sw4 * 16 + h8, c0 = J * T + 4 * hl;
         const float* ap = A + (int64_t)rb * np + c0;
         float4 a[8];
+        const uint64_t pol = l2_policy(J >= pin_j0, sfirst);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) a[k] = __ldcg(reinterpret_cast<const float4*>(ap + (int64_t)k * np));
+        for (int k = 0; k < 8; ++k) a[k] = ldcg_hint(reinterpret_cast<const float4*>(ap + (int64_t)k * np), pol);
         const float4 rj = __ldcg(reinterpret_cast<const float4*>(col + c0));     // col has np >= c0 + 4 entries
         const int ri_r = rb + (lane & 7);
         const float ri = TRD_RAW(ri_r);
@@ -437,7 +485,7 @@ __device__ void tridiagonalise(const TrdMat& mt, int cta, int ncta, float* smem)
           const int r = k * 32 + warp;                 // finish: warp = row, lane = panel column
           if (k < nrb && r >= s1 && r < n) {           // uniform
             if (lane < P) { vr[q] = __ldcg(mt.Vp + r * NB + lane); wr[q] = __ldcg(mt.Wp + r * NB + lane); }
-            if (r > s1) ac[q] = __ldcg(A + (int64_t)r * np + s1);
+            if (r > s1) ac[q] = ldcg_hint(A + (int64_t)r * np + s1, l2_policy(b0 >= pin_j0, sfirst));
             rw[q] = TRD_RAW(r);
           }
         }
@@ -489,7 +537,7 @@ __device__ void tridiagonalise(const TrdMat& mt, int cta, int ncta, float* smem)
           for (int j = 0; j < 3; ++j) { const int X = b0 + lane + 32 * j; if (X < nblk) y1p += __ldcg(&mt.part[(int64_t)X * np + s1]); }
           for (int X = b0 + lane + 96; X < nblk; X += 32) y1p += __ldcg(&mt.part[(int64_t)X * np + s1]);    // n > 6144
           if (lane < P) { vrow = __ldcg(mt.Vp + s1 * NB + lane); wrow = __ldcg(mt.Wp + s1 * NB + lane); }
-          a11 = __ldcg(&A[(int64_t)s1 * np + s1]);
+          a11 = ldcg_hint(&A[(int64_t)s1 * np + s1], l2_policy(b0 >= pin_j0, sfirst));
         }
         if (warp < P) { sa = warp_sum(sa); sb = warp_sum(sb); }
         if (warp == 0) scv = warp_sum(scv);
@@ -568,6 +616,16 @@ __device__ void tridiagonalise(const TrdMat& mt, int cta, int ncta, float* smem)
 #undef TRD_RAW
 #undef TRD_VFIX
   }
+  // the block columns still active at the last column: unpin their lines
+  const int b0_last = (n - 1) / T;
+  if (max(b0_last, pin_j0) < nblk) {
+    const int st_tid = tid & 127;
+    for (int ti = 0; ti < ntile8; ++ti) {
+      const int I = tlist8[ti].x, J = tlist8[ti].y;
+      if (J < max(b0_last, pin_j0)) break;
+      l2_unpin(A + (int64_t)(I * T + (st_tid >> 1)) * np + J * T + (st_tid & 1) * 32);
+    }
+  }
   if (cta == 0 && tid == 0) { mt.e[n - 1] = 0.f; mt.tau[n - 1] = 0.f; }
 }
 
@@ -577,8 +635,11 @@ __global__ void __launch_bounds__(TRD_THREADS, 1) sytrd_kernel(const TrdMat* mat
     const TrdJob job = jobs[j];
     const int b = (int)blockIdx.x;
     if (b < job.cta0 || b >= job.cta0 + job.ncta) continue;
+    const bool stamp = g_trd_prof_on != 0 && b == job.cta0 && threadIdx.x == 0 && j < MAX_TIMED_JOBS;
+    if (stamp) g_trd_jobtime[2 * j] = globaltimer();
     tridiagonalise(mats[job.mat], b - job.cta0, job.ncta, trd_smem);
     __syncthreads();
+    if (stamp) g_trd_jobtime[2 * j + 1] = globaltimer();
   }
 }
 
@@ -621,6 +682,12 @@ int sytrd_profile(int on, unsigned long long* out16) {
   unsigned long long zero[16] = {0};
   KFAC_CUDA(cudaMemcpyToSymbol(g_trd_prof, zero, sizeof(zero)));
   KFAC_CUDA(cudaMemcpyToSymbol(g_trd_prof_on, &on, sizeof(int)));
+  return KFAC_OK;
+}
+
+int sytrd_job_times(unsigned long long* out, int max_jobs) {
+  const int m = std::min(max_jobs, MAX_TIMED_JOBS);
+  if (out && m > 0) KFAC_CUDA(cudaMemcpyFromSymbol(out, g_trd_jobtime, sizeof(unsigned long long) * 2 * m));
   return KFAC_OK;
 }
 
