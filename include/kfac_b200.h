@@ -116,6 +116,33 @@ int kfac_factor_conv_input(const void* x, int dtype, const kfac_conv_geometry* g
                            int append_ones, float scale, float* acc, void* ws, size_t ws_bytes,
                            void* stream);
 
+/* Geometry of a ConvTranspose1d / 2d / 3d layer's input (groups = 1) in torch's own parameters, every
+ * per-axis array in (D, H, W) order (a 1-d layer is D = kd = 1, H = kh = 1).  The output extent of
+ * an axis is
+ *     (in - 1) * stride - 2 * padding + dilation * (kernel - 1) + output_padding + 1,
+ * and output position o reads input (o + padding - k * dilation) / stride through tap k when stride
+ * divides it and the quotient lies in [0, in), zero otherwise.  With the weight (C_in, C_out, k...),
+ * A's feature order is (C_in, kd, kh, kw) [+ ones].  Every call refuses with KFAC_ERR_BAD_ARG an
+ * empty output, output_padding >= max(stride, dilation), and batch x output positions >= 2^31. */
+typedef struct kfac_conv_transpose_geometry {
+  int batch, C;
+  int in[3];
+  int kernel[3];
+  int stride[3];
+  int dilation[3];
+  int padding[3];
+  int output_padding[3];
+} kfac_conv_transpose_geometry;
+
+/* kfac_factor_conv_input for a transposed geometry: the same chunked fp32 im2col (the taps that
+ * fall between inputs are exact zeros) and the same SYRK, chunking and workspace query. */
+size_t kfac_factor_conv_transpose_input_workspace_bytes(const kfac_conv_transpose_geometry* geom,
+                                                        int append_ones, size_t max_bytes);
+int kfac_factor_conv_transpose_input(const void* x, int dtype,
+                                     const kfac_conv_transpose_geometry* geom, int append_ones,
+                                     float scale, float* acc, void* ws, size_t ws_bytes,
+                                     void* stream);
+
 /* replaces Conv2dModuleHelper.get_g_factor (modules.py:180-192):
  * g is (batch, C, Ho, Wo); acc (C x C) += scale * sum_n Y_n Y_n^T.
  * ws (optional, kfac_factor_conv2d_gradout_workspace_bytes): maps whose rows are not
@@ -355,6 +382,10 @@ typedef struct kfac_precond_item {
   int kind; /* kfac_item_kind; 0 (dense) for the positional initialisers written before it */
   const float* dh;    /* KFAC_ITEM_TIED: the head's diagonal G (V floats); else ignored */
   float tied_damping; /* KFAC_ITEM_TIED: the damping M and mu were formed with (> 0) */
+  /* layout of wgrad (dense items): 0 (the initialisers written before this field) = row-major
+   * (g, a - has_bias); T > 0 = a transposed convolution's (C_in, g, T) weight gradient, whose
+   * grad-matrix element (r, ci * T + t) lies at wgrad[(ci * g + r) * T + t].  P stays (g, a). */
+  int wgrad_taps;
 } kfac_precond_item;
 size_t kfac_precondition_workspace_bytes(const kfac_precond_item* items, int count);
 int kfac_precondition(const kfac_precond_item* items, int count, int method,
@@ -402,6 +433,7 @@ typedef struct kfac_grad_item {
   int grad_dtype;
   int g, a;
   int ldp; /* leading dimension of P */
+  int wgrad_taps; /* layout of wgrad, as for a precondition item (0 = row-major); the sums run in P's order */
 } kfac_grad_item;
 /* Both calls run as ONE launch over all layers and are bitwise reproducible (fixed assignment of elements
  * to threads, fixed-order reduction; no floating-point atomics): every data-parallel replica that
@@ -437,6 +469,10 @@ int kfac_rows_conv2d_input(const void* x, int dtype, int batch, int C, int H, in
  * this call with a depth-1, dilation-1 geometry */
 int kfac_rows_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom, int append_ones,
                          float scale, float* out, int ld_out, void* stream);
+/* the rows of kfac_factor_conv_transpose_input: (batch * Do * Ho * Wo) x ld_out */
+int kfac_rows_conv_transpose_input(const void* x, int dtype, const kfac_conv_transpose_geometry* geom,
+                                   int append_ones, float scale, float* out, int ld_out,
+                                   void* stream);
 /* g (batch, C, Ho, Wo) -> rows (batch*Ho*Wo, C) */
 int kfac_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo,
                              float scale, const float* loss_scale, float* out, int ld_out,
@@ -482,6 +518,12 @@ int kfac_reduce_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, 
 int kfac_reduce_rows_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom,
                                 int append_ones, float scale, float* out, int ld_out,
                                 void* stream);
+/* conv_input for a transposed geometry: the sum over the output positions of tap (l, i, j) is the
+ * sum of x over the box of inputs whose outputs i * stride - padding + k * dilation lie inside the
+ * output on every axis, formed by the same kernels (and the same single-row path). */
+int kfac_reduce_rows_conv_transpose_input(const void* x, int dtype,
+                                          const kfac_conv_transpose_geometry* geom, int append_ones,
+                                          float scale, float* out, int ld_out, void* stream);
 
 /* S_batch of every item, for all items together; no floating-point atomics, the same bits on
  * every run.  Launches: one grouped wgmma launch of the projections (x^2 epilogue), the K = N

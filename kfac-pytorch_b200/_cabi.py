@@ -35,6 +35,13 @@ class ConvGeometry(C.Structure):
                 ('dilation', c_int * 3), ('pad_before', c_int * 3), ('pad_after', c_int * 3)]
 
 
+class ConvTransposeGeometry(C.Structure):
+    """kfac_conv_transpose_geometry: torch's parameters of a transposed convolution, every per-axis array in (D, H, W)
+    order."""
+    _fields_ = [('batch', c_int), ('C', c_int), ('input', c_int * 3), ('kernel', c_int * 3), ('stride', c_int * 3),
+                ('dilation', c_int * 3), ('padding', c_int * 3), ('output_padding', c_int * 3)]
+
+
 class EmaItem(C.Structure):
     _fields_ = [('factor', c_void_p), ('batch', c_void_p), ('d', c_int),
                 ('first', c_int), ('inv_count', c_float)]
@@ -53,7 +60,7 @@ class PrecondItem(C.Structure):
                 ('ldqa', c_int), ('ldqg', c_int), ('ld_dgda', c_int),
                 ('P', c_void_p), ('ldp', c_int),
                 ('peer_P', C.POINTER(c_void_p)), ('n_peers', c_int), ('kind', c_int),
-                ('dh', c_void_p), ('tied_damping', c_float)]
+                ('dh', c_void_p), ('tied_damping', c_float), ('wgrad_taps', c_int)]
 
 
 class TiedItem(C.Structure):
@@ -71,7 +78,7 @@ class NormItem(C.Structure):
 
 class GradItem(C.Structure):
     _fields_ = [('P', c_void_p), ('wgrad', c_void_p), ('bgrad', c_void_p),
-                ('grad_dtype', c_int), ('g', c_int), ('a', c_int), ('ldp', c_int)]
+                ('grad_dtype', c_int), ('g', c_int), ('a', c_int), ('ldp', c_int), ('wgrad_taps', c_int)]
 
 
 class EkfacStatItem(C.Structure):
@@ -101,6 +108,9 @@ SIGNATURES = {
     'kfac_factor_conv_input_workspace_bytes': (c_size_t, [C.POINTER(ConvGeometry), c_int, c_size_t]),
     'kfac_factor_conv_input': (c_int, [c_void_p, c_int, C.POINTER(ConvGeometry), c_int, c_float, c_void_p, c_void_p,
                                        c_size_t, c_void_p]),
+    'kfac_factor_conv_transpose_input_workspace_bytes': (c_size_t, [C.POINTER(ConvTransposeGeometry), c_int, c_size_t]),
+    'kfac_factor_conv_transpose_input': (c_int, [c_void_p, c_int, C.POINTER(ConvTransposeGeometry), c_int, c_float,
+                                                 c_void_p, c_void_p, c_size_t, c_void_p]),
     'kfac_factor_conv2d_gradout_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
     'kfac_factor_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     'kfac_factor_ema': (c_int, [C.POINTER(EmaItem), c_int, c_float, c_void_p]),
@@ -143,6 +153,8 @@ SIGNATURES = {
     'kfac_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
     'kfac_rows_conv_input': (c_int, [c_void_p, c_int, C.POINTER(ConvGeometry), c_int, c_float, c_void_p, c_int,
                                      c_void_p]),
+    'kfac_rows_conv_transpose_input': (c_int, [c_void_p, c_int, C.POINTER(ConvTransposeGeometry), c_int, c_float,
+                                               c_void_p, c_int, c_void_p]),
     'kfac_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
                                          c_void_p]),
     'kfac_reduce_rows_linear': (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_float, c_void_p, c_void_p,
@@ -152,6 +164,8 @@ SIGNATURES = {
     'kfac_reduce_rows_conv2d_input': (c_int, [c_void_p, c_int] + [c_int] * 11 + [c_float, c_void_p, c_int, c_void_p]),
     'kfac_reduce_rows_conv_input': (c_int, [c_void_p, c_int, C.POINTER(ConvGeometry), c_int, c_float, c_void_p, c_int,
                                             c_void_p]),
+    'kfac_reduce_rows_conv_transpose_input': (c_int, [c_void_p, c_int, C.POINTER(ConvTransposeGeometry), c_int,
+                                                      c_float, c_void_p, c_int, c_void_p]),
     'kfac_reduce_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                                 c_void_p, c_int, c_void_p]),
     'kfac_ekfac_statistics_workspace_bytes': (c_size_t, [C.POINTER(EkfacStatItem), c_int]),

@@ -224,6 +224,8 @@ def second_order_layout(layer: KFACLayer) -> Layout:
             needs = {'a_inv', 'g_inv'}
             unready = 'Cannot precondition gradient before A and G have been inverted'
         item = dict(kind=_cabi.KFAC_ITEM_DENSE, ldqa=ld4(a), ldqg=ld4(g), ld_dgda=ld4(a))
+        if layer.module.wgrad_taps:     # a transposed convolution's (C_in, g, T) weight gradient
+            item['wgrad_taps'] = layer.module.wgrad_taps
     fields = tuple((e.key.lstrip('_'), e.key) for e in entries if e.shipped or e.holder in ('grad', 'all'))
     return Layout(entries, factors, snapshots, decompositions, post, frozenset(needs), unready, fields, item, eigen)
 
@@ -410,7 +412,10 @@ class BaseKFACPreconditioner:
             if isinstance(module, AttentionProjectionHelper):
                 self._attention_taps.setdefault(module.attn, {})[module.which[0]] = module
                 continue
-            module.register_forward_pre_hook(self._save_input)
+            if layer.module.call_kwargs:
+                module.register_forward_pre_hook(self._save_input_with_kwargs, with_kwargs=True)
+            else:
+                module.register_forward_pre_hook(self._save_input)
             if layer.diag_a:
                 # the input of an embedding (the indices) never requires grad: a full backward hook would fire through
                 # the output with a warning on every backward pass, so the output tensor is hooked directly
@@ -722,6 +727,17 @@ class BaseKFACPreconditioner:
         if self.steps % self.factor_update_steps != 0:
             return
         self._accumulate_input(*self._layers[module], input_[0])
+
+    def _save_input_with_kwargs(self, module: torch.nn.Module, args: tuple, kwargs: dict) -> None:
+        """Forward pre-hook of a layer whose statistics depend on more of the call than its input: the output_size a
+        transposed convolution takes positionally or as a keyword."""
+        if not module.training:
+            return
+        if self.steps % self.factor_update_steps != 0:
+            return
+        name, layer = self._layers[module]
+        layer.module.bind_call(args, kwargs)
+        self._accumulate_input(name, layer, args[0])
 
     def _active_attention_taps(self, module: torch.nn.Module) -> dict[str, AttentionProjectionHelper] | None:
         """The registered projections of an attention module at a factor step (its forward taps them), else None."""
@@ -1318,10 +1334,12 @@ class BaseKFACPreconditioner:
         for i, (_, layer) in enumerate(ll):
             w, b = self._grad_ptrs(layer)
             rows, cols = layer.p_shape          # an embedding is a bias-less (V, d) layer here
+            lay = self._layouts.get(layer)      # (normalization layers have none)
             # ld4(cols) in the P arena, cols for a normalization layer's P
             items[i] = _cabi.GradItem(layer._p_store.data_ptr(), w.data_ptr(),
                                       b.data_ptr() if b is not None else None,
-                                      _cabi.DTYPE_CODE[w.dtype], rows, cols, layer._p_store.stride(0))
+                                      _cabi.DTYPE_CODE[w.dtype], rows, cols, layer._p_store.stride(0),
+                                      lay.item.get('wgrad_taps', 0) if lay is not None else 0)
         stream = _cabi.stream_ptr()
         kl_clip = self.kl_clip
         scale_ptr = None

@@ -72,6 +72,87 @@ inline int resolve_conv_geometry(const kfac_conv_geometry* g, ConvGeo* o) {
   return KFAC_OK;
 }
 
+// A kfac_conv_transpose_geometry as a ConvGeo: (D, H, W) the input extents, (pd, ph, pw) torch's padding, (Do, Ho, Wo)
+// the output extents (in - 1) s - 2 p + d (k - 1) + op + 1.  KFAC_ERR_BAD_ARG for a malformed geometry, an empty
+// output, an output padding of at least max(s, d) (torch refuses it) or batch x output positions of 2^31 or more.
+inline int resolve_conv_transpose_geometry(const kfac_conv_transpose_geometry* g, ConvGeo* o) {
+  KFAC_CHECK_ARG(g != nullptr, "null geometry");
+  KFAC_CHECK_ARG(g->batch > 0 && g->C > 0, "geometry");
+  int out[3];
+  int64_t rows = g->batch;
+  for (int a = 0; a < 3; ++a) {
+    KFAC_CHECK_ARG(g->in[a] > 0 && g->kernel[a] > 0 && g->stride[a] > 0 && g->dilation[a] > 0 && g->padding[a] >= 0 &&
+                       g->output_padding[a] >= 0, "geometry");
+    KFAC_CHECK_ARG(g->output_padding[a] < (g->stride[a] > g->dilation[a] ? g->stride[a] : g->dilation[a]),
+                   "output padding of at least max(stride, dilation)");
+    const int64_t n = ((int64_t)g->in[a] - 1) * g->stride[a] - 2 * (int64_t)g->padding[a] +
+                      (int64_t)g->dilation[a] * (g->kernel[a] - 1) + g->output_padding[a] + 1;
+    KFAC_CHECK_ARG(n > 0, "empty output");
+    rows *= n;
+    KFAC_CHECK_ARG(rows < (1ll << 31), "rows overflow");
+    out[a] = (int)n;
+  }
+  *o = ConvGeo{g->batch, g->C, g->in[0], g->in[1], g->in[2], g->kernel[0], g->kernel[1], g->kernel[2],
+               g->stride[0], g->stride[1], g->stride[2], g->dilation[0], g->dilation[1], g->dilation[2],
+               g->padding[0], g->padding[1], g->padding[2], out[0], out[1], out[2]};
+  return KFAC_OK;
+}
+
+// The tap -> input index map of one axis (stride s, dilation d, padding p; L inputs, n_out outputs).  A convolution
+// gathers: output o reads input o s + k d - p through tap k.  A transposed convolution scatters: input i feeds output
+// i s - p + k d, so output o reads input (o + p - k d) / s when s divides it.  Both read a tap's inputs in the order of
+// their outputs.  The kernels take it as a template parameter; the direct instantiations give the results they gave.
+template <bool TRANSPOSED>
+struct TapMap;
+
+template <>
+struct TapMap<false> {
+  // the input that output o reads through tap k, or -1 in the padding
+  __device__ __forceinline__ static int input(int o, int k, int s, int d, int p, int L) {
+    const int i = o * s + k * d - p;
+    return i >= 0 && i < L ? i : -1;
+  }
+  // input q is read through tap k by an output in [0, n_out)
+  __device__ __forceinline__ static bool feeds(int q, int k, int s, int d, int p, int n_out) {
+    const int t = q + p - k * d;
+    return t >= 0 && t % s == 0 && t / s < n_out;
+  }
+  // the inputs read through tap k, in output order: first + m step for m in [0, count)
+  __device__ __forceinline__ static void span(int L, int k, int s, int d, int p, int n_out, int& first, int& step,
+                                              int& count) {
+    const int off = k * d - p;   // input of output 0
+    const int lo = off < 0 ? (-off + s - 1) / s : 0;
+    const int hi = L - 1 - off < 0 ? -1 : min(n_out - 1, (L - 1 - off) / s);
+    first = off + lo * s;
+    step = s;
+    count = hi >= lo ? hi - lo + 1 : 0;
+  }
+};
+
+template <>
+struct TapMap<true> {
+  __device__ __forceinline__ static int input(int o, int k, int s, int d, int p, int L) {
+    const int t = o + p - k * d;
+    if (t < 0) return -1;
+    const int i = (int)((unsigned)t / (unsigned)s);
+    return i * s == t && i < L ? i : -1;
+  }
+  __device__ __forceinline__ static bool feeds(int q, int k, int s, int d, int p, int n_out) {
+    const int o = q * s - p + k * d;
+    return o >= 0 && o < n_out;
+  }
+  // the box of inputs i in [0, L) whose output i s - p + k d lies in [0, n_out), step 1
+  __device__ __forceinline__ static void span(int L, int k, int s, int d, int p, int n_out, int& first, int& step,
+                                              int& count) {
+    const int off = k * d - p;   // output of input 0
+    const int lo = off < 0 ? (-off + s - 1) / s : 0;
+    const int hi = n_out - 1 - off < 0 ? -1 : min(L - 1, (n_out - 1 - off) / s);
+    first = lo;
+    step = 1;
+    count = hi >= lo ? hi - lo + 1 : 0;
+  }
+};
+
 template <typename T>
 __device__ __forceinline__ float to_float(T v);
 template <>

@@ -35,8 +35,10 @@ __device__ __forceinline__ float row_scale(float scale, const float* loss_scale)
 // out[(n, do, ho, wo)][(c, l, i, j) | ones] of an NCDHW input.  A CTA moves a 32 rows x 32 features tile through shared
 // memory: it reads along the rows (neighbouring output positions) and writes along the features, both coalesced.  The
 // 1 x 1 / stride-1 case is the gather of an NCHW tensor into rows (the conv G side uses it with kh = kw = 1).
-template <typename T>
+// TRANSPOSED: the index map of a transposed convolution (TapMap).
+template <typename T, bool TRANSPOSED>
 __global__ void __launch_bounds__(256) rows_im2col_kernel(RowsArgs a) {
+  using Tap = TapMap<TRANSPOSED>;
   __shared__ float tile[32][33];
   const ConvGeo& g = a.g;
   const int64_t rows = (int64_t)g.batch * g.Do * g.Ho * g.Wo;
@@ -64,9 +66,9 @@ __global__ void __launch_bounds__(256) rows_im2col_kernel(RowsArgs a) {
         if (f < nfeat) {
           const int j = f % g.kw, ki = (f / g.kw) % g.kh, fl = f / (g.kw * g.kh);
           const int l = fl % g.kd, c = fl / g.kd;
-          const int z = dz * g.sd + l * g.dd - g.pd, h = ho * g.sh + ki * g.dh - g.ph, w = wo * g.sw + j * g.dw - g.pw;
-          if (z >= 0 && z < g.D && h >= 0 && h < g.H && w >= 0 && w < g.W)
-            v = to_float<T>(x[((((int64_t)n * g.C + c) * g.D + z) * g.H + h) * g.W + w]) * s;
+          const int z = Tap::input(dz, l, g.sd, g.dd, g.pd, g.D), h = Tap::input(ho, ki, g.sh, g.dh, g.ph, g.H),
+                    w = Tap::input(wo, j, g.sw, g.dw, g.pw, g.W);
+          if ((z | h | w) >= 0) v = to_float<T>(x[((((int64_t)n * g.C + c) * g.D + z) * g.H + h) * g.W + w]) * s;
         } else if (f == nfeat && a.ones) {
           v = s;
         }
@@ -97,14 +99,15 @@ __global__ void __launch_bounds__(256) rows_linear_kernel(const void* xin, int64
   }
 }
 
+template <bool TRANSPOSED = false>
 static int launch_rows_im2col(const RowsArgs& a, int dtype, cudaStream_t s) {
   const int64_t rows = (int64_t)a.g.batch * a.g.spatial();
   KFAC_CHECK_ARG(rows < (1ll << 31), "rows overflow");
   const dim3 grid((unsigned)ceil_div(rows, 32), (unsigned)ceil_div(a.ld, 32)), block(32, 8);
   KFAC_CHECK_ARG(grid.y <= 65535, "more than 2^21 features");
-  if (dtype == KFAC_F32) rows_im2col_kernel<float><<<grid, block, 0, s>>>(a);
-  else if (dtype == KFAC_F16) rows_im2col_kernel<__half><<<grid, block, 0, s>>>(a);
-  else if (dtype == KFAC_BF16) rows_im2col_kernel<__nv_bfloat16><<<grid, block, 0, s>>>(a);
+  if (dtype == KFAC_F32) rows_im2col_kernel<float, TRANSPOSED><<<grid, block, 0, s>>>(a);
+  else if (dtype == KFAC_F16) rows_im2col_kernel<__half, TRANSPOSED><<<grid, block, 0, s>>>(a);
+  else if (dtype == KFAC_BF16) rows_im2col_kernel<__nv_bfloat16, TRANSPOSED><<<grid, block, 0, s>>>(a);
   else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   KFAC_LAUNCH_CHECK();
   return KFAC_OK;
@@ -332,6 +335,18 @@ extern "C" int kfac_rows_conv_input(const void* x, int dtype, const kfac_conv_ge
   KFAC_CHECK_ARG((int64_t)ld_out >= g.features() + ones && ld_out % 4 == 0, "ld_out");
   RowsArgs a{x, out, g, ones, ld_out, scale, nullptr};
   return launch_rows_im2col(a, dtype, (cudaStream_t)stream);
+}
+
+extern "C" int kfac_rows_conv_transpose_input(const void* x, int dtype, const kfac_conv_transpose_geometry* geom,
+                                              int append_ones, float scale, float* out, int ld_out, void* stream) {
+  KFAC_CHECK_ARG(x && out, "null pointer");
+  ConvGeo g;
+  const int rc = resolve_conv_transpose_geometry(geom, &g);
+  if (rc) return rc;
+  const int ones = append_ones ? 1 : 0;
+  KFAC_CHECK_ARG((int64_t)ld_out >= g.features() + ones && ld_out % 4 == 0, "ld_out");
+  RowsArgs a{x, out, g, ones, ld_out, scale, nullptr};
+  return launch_rows_im2col<true>(a, dtype, (cudaStream_t)stream);
 }
 
 extern "C" int kfac_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo, float scale,

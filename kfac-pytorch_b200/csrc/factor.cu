@@ -201,9 +201,11 @@ struct Im2colArgs {
 };
 // grid (ceil(ld / 4 / 256), features [+ 1]): a thread writes 4 consecutive samples of one feature row with one 16-byte
 // store; the (image, do, ho, wo) decomposition is done once per thread in 32-bit arithmetic and advanced incrementally
-// (the element-wise version spent its time in 64-bit divisions: 480 us for a 231 MB matrix, now bandwidth bound)
-template <typename T>
+// (the element-wise version spent its time in 64-bit divisions: 480 us for a 231 MB matrix, now bandwidth bound).
+// TRANSPOSED: the index map of a transposed convolution (TapMap); a tap between two inputs is an exact zero.
+template <typename T, bool TRANSPOSED = false>
 __global__ void __launch_bounds__(256) im2col_kernel(Im2colArgs a) {
+  using Tap = TapMap<TRANSPOSED>;
   const ConvGeo& g = a.g;
   const int64_t rows = (int64_t)g.batch * g.Do * g.Ho * g.Wo;
   const int nfeat = g.C * g.kd * g.kh * g.kw;
@@ -218,8 +220,6 @@ __global__ void __launch_bounds__(256) im2col_kernel(Im2colArgs a) {
     const T* __restrict__ x = reinterpret_cast<const T*>(a.x);
     const int j = f % g.kw, i = (f / g.kw) % g.kh, fl = f / (g.kw * g.kh);
     const int l = fl % g.kd, c = fl / g.kd;
-    // input offsets of this window tap at output position 0
-    const int z0 = l * g.dd - g.pd, h0 = i * g.dh - g.ph, w0 = j * g.dw - g.pw;
     const unsigned row = (unsigned)r4;                    // rows < 2^31 (checked by the caller)
     int wo = (int)(row % (unsigned)g.Wo);
     unsigned t = row / (unsigned)g.Wo;
@@ -229,9 +229,9 @@ __global__ void __launch_bounds__(256) im2col_kernel(Im2colArgs a) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (r4 + k < rows) {
-        const int z = dz * g.sd + z0, h = ho * g.sh + h0, w = wo * g.sw + w0;
-        if (z >= 0 && z < g.D && h >= 0 && h < g.H && w >= 0 && w < g.W)
-          v[k] = to_float<T>(x[((((int64_t)n * g.C + c) * g.D + z) * g.H + h) * g.W + w]);
+        const int z = Tap::input(dz, l, g.sd, g.dd, g.pd, g.D), h = Tap::input(ho, i, g.sh, g.dh, g.ph, g.H),
+                  w = Tap::input(wo, j, g.sw, g.dw, g.pw, g.W);
+        if ((z | h | w) >= 0) v[k] = to_float<T>(x[((((int64_t)n * g.C + c) * g.D + z) * g.H + h) * g.W + w]);
       }
       if (++wo == g.Wo) { wo = 0; if (++ho == g.Ho) { ho = 0; if (++dz == g.Do) { dz = 0; ++n; } } }
     }
@@ -679,7 +679,10 @@ static int conv_chunk_for(const ConvGeo& g, int ones, size_t bytes, bool with_sl
   return (int)lo;
 }
 
-// acc += scale * X^T X of the im2col X, formed `chunk` examples at a time into the workspace (see the header)
+// acc += scale * X^T X of the im2col X, formed `chunk` examples at a time into the workspace (see the header).  A
+// kernel of ones with unit stride and no padding has the identity index map in both directions, so conv_in_place
+// holds for a transposed geometry as well.
+template <bool TRANSPOSED = false>
 static int conv_input_factor(const void* x, int dtype, const ConvGeo& g, int append_ones, int chunk, float scale,
                              float* acc, void* ws, size_t ws_bytes, cudaStream_t s) {
   const int ones = append_ones ? 1 : 0;
@@ -712,9 +715,9 @@ static int conv_input_factor(const void* x, int dtype, const ConvGeo& g, int app
     const int64_t rows = (int64_t)ia.g.batch * g.spatial();
     ia.ld = (rows + 3) / 4 * 4;
     const dim3 grid((unsigned)ceil_div(ia.ld / 4, 256), (unsigned)d);
-    if (dtype == KFAC_F32) im2col_kernel<float><<<grid, 256, 0, s>>>(ia);
-    else if (dtype == KFAC_F16) im2col_kernel<__half><<<grid, 256, 0, s>>>(ia);
-    else im2col_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(ia);
+    if (dtype == KFAC_F32) im2col_kernel<float, TRANSPOSED><<<grid, 256, 0, s>>>(ia);
+    else if (dtype == KFAC_F16) im2col_kernel<__half, TRANSPOSED><<<grid, 256, 0, s>>>(ia);
+    else im2col_kernel<__nv_bfloat16, TRANSPOSED><<<grid, 256, 0, s>>>(ia);
     KFAC_LAUNCH_CHECK();
     // the ones row is materialised, so the SYRK sees d = C*kd*kh*kw + ones plain features
     CovArgs c = a;
@@ -746,10 +749,8 @@ extern "C" int kfac_factor_conv2d_input(const void* x, int dtype, int batch, int
   return conv_input_factor(x, dtype, g, append_ones, batch, scale, acc, ws, ws_bytes, (cudaStream_t)stream);
 }
 
-extern "C" size_t kfac_factor_conv_input_workspace_bytes(const kfac_conv_geometry* geom, int append_ones,
-                                                         size_t max_bytes) {
-  ConvGeo g;
-  if (resolve_conv_geometry(geom, &g) != KFAC_OK) return 0;
+// the workspace query of the chunked factor calls
+static size_t conv_chunked_ws_bytes(const ConvGeo& g, int append_ones, size_t max_bytes) {
   const int ones = append_ones ? 1 : 0;
   if (conv_in_place(g)) return conv_chunk_ws(g, g.batch, ones).total;
   // the largest chunk whose matrix and SYRK partials fit; else one example (beyond max_bytes when it alone does not fit)
@@ -757,12 +758,10 @@ extern "C" size_t kfac_factor_conv_input_workspace_bytes(const kfac_conv_geometr
   return conv_chunk_ws(g, n, ones).total;
 }
 
-extern "C" int kfac_factor_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom, int append_ones,
-                                      float scale, float* acc, void* ws, size_t ws_bytes, void* stream) {
-  KFAC_CHECK_ARG(x && acc, "null pointer");
-  ConvGeo g;
-  const int rc = resolve_conv_geometry(geom, &g);
-  if (rc) return rc;
+// the chunked factor calls: the chunk is the largest that ws_bytes holds
+template <bool TRANSPOSED>
+static int conv_chunked_factor(const void* x, int dtype, const ConvGeo& g, int append_ones, float scale, float* acc,
+                               void* ws, size_t ws_bytes, cudaStream_t s) {
   const int ones = append_ones ? 1 : 0;
   int chunk = g.batch;
   if (!conv_in_place(g)) {
@@ -773,7 +772,40 @@ extern "C" int kfac_factor_conv_input(const void* x, int dtype, const kfac_conv_
       return KFAC_ERR_WORKSPACE;
     }
   }
-  return conv_input_factor(x, dtype, g, ones, chunk, scale, acc, ws, ws_bytes, (cudaStream_t)stream);
+  return conv_input_factor<TRANSPOSED>(x, dtype, g, ones, chunk, scale, acc, ws, ws_bytes, s);
+}
+
+extern "C" size_t kfac_factor_conv_input_workspace_bytes(const kfac_conv_geometry* geom, int append_ones,
+                                                         size_t max_bytes) {
+  ConvGeo g;
+  if (resolve_conv_geometry(geom, &g) != KFAC_OK) return 0;
+  return conv_chunked_ws_bytes(g, append_ones, max_bytes);
+}
+
+extern "C" int kfac_factor_conv_input(const void* x, int dtype, const kfac_conv_geometry* geom, int append_ones,
+                                      float scale, float* acc, void* ws, size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(x && acc, "null pointer");
+  ConvGeo g;
+  const int rc = resolve_conv_geometry(geom, &g);
+  if (rc) return rc;
+  return conv_chunked_factor<false>(x, dtype, g, append_ones, scale, acc, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+extern "C" size_t kfac_factor_conv_transpose_input_workspace_bytes(const kfac_conv_transpose_geometry* geom,
+                                                                   int append_ones, size_t max_bytes) {
+  ConvGeo g;
+  if (resolve_conv_transpose_geometry(geom, &g) != KFAC_OK) return 0;
+  return conv_chunked_ws_bytes(g, append_ones, max_bytes);
+}
+
+extern "C" int kfac_factor_conv_transpose_input(const void* x, int dtype, const kfac_conv_transpose_geometry* geom,
+                                                int append_ones, float scale, float* acc, void* ws, size_t ws_bytes,
+                                                void* stream) {
+  KFAC_CHECK_ARG(x && acc, "null pointer");
+  ConvGeo g;
+  const int rc = resolve_conv_transpose_geometry(geom, &g);
+  if (rc) return rc;
+  return conv_chunked_factor<true>(x, dtype, g, append_ones, scale, acc, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 static CovWs gradout_ws(int batch, int C, int Ho, int Wo) {

@@ -26,8 +26,16 @@ __global__ void gather_grad_kernel(const void* w, const void* b, int dtype, int 
   }
 }
 
+// Offset in wgrad of element (r, c) of the (g, aw) weight-gradient matrix: row-major (taps = 0), or a transposed
+// convolution's (C_in, g, taps) weight with c = ci * taps + t (kfac_precond_item.wgrad_taps)
+__device__ __forceinline__ long long wgrad_offset(long long r, int c, int g, int aw, int taps) {
+  if (taps == 0) return r * aw + c;
+  const int ci = c / taps;
+  return ((long long)ci * g + r) * taps + (c - ci * taps);
+}
+
 // all layers in one launch: item i owns the elements [elem0, elem0 + g * ldo) of the concatenated space
-struct GatherDev { const void* w; const void* b; int dtype, g, a, ldo; float* out; long long elem0; };
+struct GatherDev { const void* w; const void* b; int dtype, g, a, ldo; float* out; long long elem0; int taps; };
 __global__ void __launch_bounds__(256) gather_all_kernel(const GatherDev* items, int count, long long total) {
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     int lo = 0, hi = count - 1;
@@ -38,7 +46,7 @@ __global__ void __launch_bounds__(256) gather_all_kernel(const GatherDev* items,
     const int j = (int)(idx % it.ldo);
     const int aw = it.b ? it.a - 1 : it.a;
     float v = 0.f;
-    if (j < aw) v = load_as_float(it.w, it.dtype, i * aw + j);
+    if (j < aw) v = load_as_float(it.w, it.dtype, wgrad_offset(i, j, it.g, aw, it.taps));
     else if (j < it.a) v = load_as_float(it.b, it.dtype, i);
     it.out[idx] = v;
   }
@@ -46,7 +54,7 @@ __global__ void __launch_bounds__(256) gather_all_kernel(const GatherDev* items,
 
 // ---- kl-clip scale and write-back: ONE launch each over all layers, deterministic ---------------
 // device copy of a kfac_grad_item + the offset of its g*a elements in the concatenated element space
-struct GradDev { const float* P; void* w; void* b; int dtype, g, a, ldp; long long elem0; };
+struct GradDev { const float* P; void* w; void* b; int dtype, g, a, ldp; long long elem0; int taps; };
 constexpr int VG_BLOCKS = 592;          // 4 per SM; partial sums are combined in a fixed order
 
 __device__ __forceinline__ int find_item(const GradDev* items, int count, long long e) {
@@ -67,7 +75,8 @@ __global__ void __launch_bounds__(256) vg_all_kernel(const GradDev* items, int c
     const long long i = loc / it.a;
     const int j = (int)(loc % it.a);
     const int aw = it.b ? it.a - 1 : it.a;
-    const float gr = (j < aw) ? load_as_float(it.w, it.dtype, i * aw + j) : load_as_float(it.b, it.dtype, i);
+    const float gr = (j < aw) ? load_as_float(it.w, it.dtype, wgrad_offset(i, j, it.g, aw, it.taps))
+                              : load_as_float(it.b, it.dtype, i);
     acc += (double)it.P[i * it.ldp + j] * (double)gr;
   }
 #pragma unroll
@@ -101,7 +110,7 @@ __global__ void __launch_bounds__(256) update_all_kernel(const GradDev* items, i
     const int j = (int)(loc % it.a);
     const int aw = it.b ? it.a - 1 : it.a;
     const float v = s * it.P[i * it.ldp + j];
-    if (j < aw) store_from_float(it.w, it.dtype, i * aw + j, v);
+    if (j < aw) store_from_float(it.w, it.dtype, wgrad_offset(i, j, it.g, aw, it.taps), v);
     else store_from_float(it.b, it.dtype, i, v);
   }
 }
@@ -394,7 +403,7 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
         return KFAC_ERR_NOT_READY;
       }
       // [wgrad | bgrad] as a (rows, n) layer: an embedding's V x d weight gradient, or a diagonal-G layer's own
-      gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, D.rows, D.n, ld4(D.n), F(L.gr[i]), total};
+      gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, D.rows, D.n, ld4(D.n), F(L.gr[i]), total, 0};
       total += (long long)D.rows * ld4(D.n);
       continue;
     }
@@ -409,7 +418,9 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
       return KFAC_ERR_NOT_READY;
     }
     KFAC_CHECK_ARG(it.ldqa >= it.a && it.ldqg >= it.g, "second-order leading dims");
-    gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, it.g, it.a, ld4(it.a), F(L.gr[i]), total};
+    KFAC_CHECK_ARG(it.wgrad_taps >= 0 && (it.wgrad_taps == 0 || (it.a - (it.bgrad ? 1 : 0)) % it.wgrad_taps == 0),
+                   "precond item wgrad_taps");
+    gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, it.g, it.a, ld4(it.a), F(L.gr[i]), total, it.wgrad_taps};
     total += (long long)it.g * ld4(it.a);
   }
   KFAC_CUDA(cudaMemcpyAsync(base + L.off_gather, gat.data(), sizeof(GatherDev) * count, cudaMemcpyHostToDevice, s));
@@ -534,7 +545,9 @@ static int upload_grad_items(const kfac_grad_item* items, int count, void* ws, s
   for (int i = 0; i < count; ++i) {
     const kfac_grad_item& it = items[i];
     KFAC_CHECK_ARG(it.P && it.wgrad && it.g > 0 && it.a > 0 && it.ldp >= it.a, "grad item");
-    dev[i] = GradDev{it.P, it.wgrad, it.bgrad, it.grad_dtype, it.g, it.a, it.ldp, total};
+    KFAC_CHECK_ARG(it.wgrad_taps >= 0 && (it.wgrad_taps == 0 || (it.a - (it.bgrad ? 1 : 0)) % it.wgrad_taps == 0),
+                   "grad item wgrad_taps");
+    dev[i] = GradDev{it.P, it.wgrad, it.bgrad, it.grad_dtype, it.g, it.a, it.ldp, total, it.wgrad_taps};
     total += (long long)it.g * it.a;
   }
   KFAC_CUDA(cudaMemcpyAsync(ws, dev.data(), sizeof(GradDev) * count, cudaMemcpyHostToDevice, s));   // pageable: staged

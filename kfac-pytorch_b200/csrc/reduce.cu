@@ -60,32 +60,21 @@ __global__ void __launch_bounds__(256) reduce_linear_kernel(const T* __restrict_
 }
 
 // Window sums of one (b, c) volume:
-//   out[b][(c, l, i, j)] = scale * sum_{do, ho, wo} xpad[do sd + l dd - pd][ho sh + i dh - ph][wo sw + j dw - pw].
-// Separable: the volume is a sequence of D * H rows (z, h) of W elements.  rowsum[(z, h)][j] = sum_wo x[z][h][wo sw +
-// j dw - pw] for a chunk of rows (a thread per (row, j), so a row is read once from HBM and re-read from L1 for the other
-// j), then acc[l][i][j] += rowsum[(z, h)][j] over the chunk's rows on the lattice of (l, i), in row order (a thread per
-// (l, i, j), the same thread for every chunk).  Rows no window touches are not read.
+//   out[b][(c, l, i, j)] = scale * sum over the output positions (do, ho, wo) of the input read through tap (l, i, j)
+// (TapMap: a convolution's window, or a transposed convolution's scatter; for the latter the inputs of one tap form a
+// box).  Separable: the volume is a sequence of D * H rows (z, h) of W elements.  rowsum[(z, h)][j] = the sum over the
+// inputs of row (z, h) that tap j reads (TapMap::span) for a chunk of rows (a thread per (row, j), so a row is read
+// once from HBM and re-read from L1 for the other j), then acc[l][i][j] += rowsum[(z, h)][j] over the chunk's rows that
+// taps l and i read, in row order (a thread per (l, i, j), the same thread for every chunk).  Rows no tap reads are not
+// read.
 constexpr int CONV_SMEM = 2048;   // doubles of rowsum per chunk, and the most (l, i, j) taps of a CTA
 
-// the row index q of an axis is on the output lattice of window offset k: q = o s + k dil - p with 0 <= o < n_out
-__device__ __forceinline__ bool on_lattice(int q, int k, int s, int dil, int p, int n_out) {
-  const int t = q + p - k * dil;
-  return t >= 0 && t % s == 0 && t / s < n_out;
-}
-
-// fp32 sum of x[wo s] over one run [w0, w1), in order
+// fp32 sum of row[m step] over one run [m0, m1), in order
 template <typename T>
-__device__ __forceinline__ float run_sum(const T* __restrict__ row, int w0, int w1, int s) {
+__device__ __forceinline__ float run_sum(const T* __restrict__ row, int m0, int m1, int step) {
   float acc = 0.f;
-  for (int wo = w0; wo < w1; ++wo) acc += to_float<T>(row[wo * s]);
+  for (int m = m0; m < m1; ++m) acc += to_float<T>(row[m * step]);
   return acc;
-}
-
-// the output columns [lo, hi] whose tap j lies inside a row of W elements (hi < lo: none)
-__device__ __forceinline__ void tap_range(const ConvGeo& g, int j, int& lo, int& hi) {
-  const int off = j * g.dw - g.pw;   // input column of output column 0
-  lo = off < 0 ? (-off + g.sw - 1) / g.sw : 0;
-  hi = g.W - 1 - off < 0 ? -1 : min(g.Wo - 1, (g.W - 1 - off) / g.sw);
 }
 
 // the ones column and the zero padding of an example's row, written once per example
@@ -95,9 +84,10 @@ __device__ __forceinline__ void ones_and_padding(const ConvGeo& g, int ones, dou
     o[f] = (f == d && ones) ? (float)((double)g.spatial() * sc) : 0.f;
 }
 
-template <typename T>
+template <typename T, bool TRANSPOSED>
 __global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restrict__ x, const ConvGeo g, int ones,
                                                                 float scale, float* out, int64_t ld) {
+  using Tap = TapMap<TRANSPOSED>;
   __shared__ double rowsum[CONV_SMEM];
   __shared__ double pacc[CONV_SMEM];
   const int64_t plane = blockIdx.x;
@@ -114,30 +104,29 @@ __global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restr
     for (int e = threadIdx.x; e < hc * kw; e += blockDim.x) {
       const int r = e / kw, j = e - r * kw, q = r0 + r, z = q / g.H, h = q - z * g.H;
       bool used_z = false, used_h = false;
-      for (int l = 0; l < g.kd && !used_z; ++l) used_z = on_lattice(z, l, g.sd, g.dd, g.pd, g.Do);
-      for (int i = 0; i < g.kh && !used_h; ++i) used_h = on_lattice(h, i, g.sh, g.dh, g.ph, g.Ho);
+      for (int l = 0; l < g.kd && !used_z; ++l) used_z = Tap::feeds(z, l, g.sd, g.dd, g.pd, g.Do);
+      for (int i = 0; i < g.kh && !used_h; ++i) used_h = Tap::feeds(h, i, g.sh, g.dh, g.ph, g.Ho);
       double acc = 0.0;
       if (used_z && used_h) {
-        int lo, hi;
-        tap_range(g, j, lo, hi);
-        const T* __restrict__ row = xp + (int64_t)q * g.W + j * g.dw - g.pw;
-        for (int w0 = lo; w0 <= hi; w0 += RUN) acc += (double)run_sum(row, w0, min(hi + 1, w0 + RUN), g.sw);
+        int first, step, n;
+        Tap::span(g.W, j, g.sw, g.dw, g.pw, g.Wo, first, step, n);
+        const T* __restrict__ row = xp + (int64_t)q * g.W + first;
+        for (int m0 = 0; m0 < n; m0 += RUN) acc += (double)run_sum(row, m0, min(n, m0 + RUN), step);
       }
       rowsum[e] = acc;
     }
     __syncthreads();
     for (int p = threadIdx.x; p < P; p += blockDim.x) {
       const int j = p % kw, i = (p / kw) % g.kh, l = p / (kw * g.kh);
+      int first, step, n;
+      Tap::span(g.H, i, g.sh, g.dh, g.ph, g.Ho, first, step, n);
       double acc = pacc[p];
       for (int z = r0 / g.H; z <= (r0 + hc - 1) / g.H; ++z) {
-        if (!on_lattice(z, l, g.sd, g.dd, g.pd, g.Do)) continue;
+        if (!Tap::feeds(z, l, g.sd, g.dd, g.pd, g.Do)) continue;
         const int hlo = max(0, r0 - z * g.H), hhi = min(g.H, r0 + hc - z * g.H);
-        // first row of the chunk on the lattice of i, then every sh-th row
-        const int q = hlo + g.ph - i * g.dh;
-        for (int h = hlo + (q <= 0 ? -q : (g.sh - q % g.sh) % g.sh); h < hhi; h += g.sh) {
-          if ((h + g.ph - i * g.dh) / g.sh >= g.Ho) break;
-          acc += rowsum[(z * g.H + h - r0) * kw + j];
-        }
+        // the rows of tap i's span inside the chunk
+        int m = hlo > first ? (hlo - first + step - 1) / step : 0;
+        for (int h = first + m * step; m < n && h < hhi; ++m, h += step) acc += rowsum[(z * g.H + h - r0) * kw + j];
       }
       pacc[p] = acc;
     }
@@ -149,10 +138,11 @@ __global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restr
   if (c == 0) ones_and_padding(g, ones, sc, o, ld);
 }
 
-// A single-row input (a Conv1d: D = H = 1, kd = kh = 1, no depth or height padding, Do = Ho = 1).  reduce_conv_input_kernel would give one thread
-// per tap j a whole signal; here a CTA per (b, c, j) forms the fp32 runs of the tap's sum in parallel and one thread
-// adds them in fp64 in run order -- the order of reduce_conv_input_kernel, so both give the same bits.
-template <typename T>
+// A single-row input (D = H = 1, kd = kh = 1, no depth or height padding, Do = Ho = 1: a Conv1d or ConvTranspose1d).
+// reduce_conv_input_kernel would give one thread per tap j a whole signal; here a CTA per (b, c, j) forms the fp32 runs
+// of the tap's sum in parallel and one thread adds them in fp64 in run order -- the order of reduce_conv_input_kernel,
+// so both give the same bits.
+template <typename T, bool TRANSPOSED>
 __global__ void __launch_bounds__(256) reduce_conv_input_1d_kernel(const T* __restrict__ x, const ConvGeo g, int ones,
                                                                    float scale, float* out, int64_t ld) {
   __shared__ double runs[CONV_SMEM];
@@ -160,16 +150,16 @@ __global__ void __launch_bounds__(256) reduce_conv_input_1d_kernel(const T* __re
   const int64_t b = plane / g.C;
   const int c = (int)(plane - b * g.C);
   const int j = blockIdx.y;
-  int lo, hi;
-  tap_range(g, j, lo, hi);
-  const T* __restrict__ row = x + plane * g.W + j * g.dw - g.pw;
-  const int n = hi >= lo ? (hi - lo) / RUN + 1 : 0;
+  int first, step, cnt;
+  TapMap<TRANSPOSED>::span(g.W, j, g.sw, g.dw, g.pw, g.Wo, first, step, cnt);
+  const T* __restrict__ row = x + plane * g.W + first;
+  const int n = (cnt + RUN - 1) / RUN;
   double acc = 0.0;
   for (int k0 = 0; k0 < n; k0 += CONV_SMEM) {
     const int kn = min(CONV_SMEM, n - k0);
     for (int k = threadIdx.x; k < kn; k += blockDim.x) {
-      const int w0 = lo + (k0 + k) * RUN;
-      runs[k] = (double)run_sum(row, w0, min(hi + 1, w0 + RUN), g.sw);
+      const int m0 = (k0 + k) * RUN;
+      runs[k] = (double)run_sum(row, m0, min(cnt, m0 + RUN), step);
     }
     __syncthreads();
     if (threadIdx.x == 0)
@@ -254,6 +244,7 @@ extern "C" int kfac_reduce_rows_linear(const void* x, int dtype, int64_t B, int6
                                          loss_scale, out, ld_out, stream);
 }
 
+template <bool TRANSPOSED = false>
 static int reduce_conv_input(const void* x, int dtype, const ConvGeo& g, int append_ones, float scale, float* out,
                              int ld_out, cudaStream_t s) {
   KFAC_CHECK_ARG((int64_t)g.kd * g.kh * g.kw <= CONV_SMEM, "kernel window of more than 2048 taps");
@@ -261,25 +252,29 @@ static int reduce_conv_input(const void* x, int dtype, const ConvGeo& g, int app
   KFAC_CHECK_ARG((int64_t)ld_out >= g.features() + ones, "ld_out");
   KFAC_CHECK_ARG((int64_t)g.batch * g.C < (1ll << 31), "grid");
   const unsigned planes = (unsigned)((int64_t)g.batch * g.C);
-  // the single-row kernel sums row 0 only: no depth or height padding may move the one output row off it
+  // the single-row kernel sums row 0 only: no depth or height padding may move the one output row off it (for a
+  // transposed geometry with these extents the output row is row 0 as well)
   if (g.D == 1 && g.H == 1 && g.kd == 1 && g.kh == 1 && g.pd == 0 && g.ph == 0 && g.Do == 1 && g.Ho == 1) {
     const dim3 grid(planes, (unsigned)g.kw);
     if (dtype == KFAC_F32)
-      reduce_conv_input_1d_kernel<float><<<grid, 256, 0, s>>>((const float*)x, g, ones, scale, out, ld_out);
+      reduce_conv_input_1d_kernel<float, TRANSPOSED><<<grid, 256, 0, s>>>((const float*)x, g, ones, scale, out,
+                                                                          ld_out);
     else if (dtype == KFAC_F16)
-      reduce_conv_input_1d_kernel<__half><<<grid, 256, 0, s>>>((const __half*)x, g, ones, scale, out, ld_out);
+      reduce_conv_input_1d_kernel<__half, TRANSPOSED><<<grid, 256, 0, s>>>((const __half*)x, g, ones, scale, out,
+                                                                           ld_out);
     else if (dtype == KFAC_BF16)
-      reduce_conv_input_1d_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones, scale, out,
-                                                                      ld_out);
+      reduce_conv_input_1d_kernel<__nv_bfloat16, TRANSPOSED><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones,
+                                                                                  scale, out, ld_out);
     else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   } else {
     if (dtype == KFAC_F32)
-      reduce_conv_input_kernel<float><<<planes, 256, 0, s>>>((const float*)x, g, ones, scale, out, ld_out);
+      reduce_conv_input_kernel<float, TRANSPOSED><<<planes, 256, 0, s>>>((const float*)x, g, ones, scale, out, ld_out);
     else if (dtype == KFAC_F16)
-      reduce_conv_input_kernel<__half><<<planes, 256, 0, s>>>((const __half*)x, g, ones, scale, out, ld_out);
+      reduce_conv_input_kernel<__half, TRANSPOSED><<<planes, 256, 0, s>>>((const __half*)x, g, ones, scale, out,
+                                                                          ld_out);
     else if (dtype == KFAC_BF16)
-      reduce_conv_input_kernel<__nv_bfloat16><<<planes, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones, scale, out,
-                                                                     ld_out);
+      reduce_conv_input_kernel<__nv_bfloat16, TRANSPOSED><<<planes, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones,
+                                                                                 scale, out, ld_out);
     else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   }
   KFAC_LAUNCH_CHECK();
@@ -304,6 +299,16 @@ extern "C" int kfac_reduce_rows_conv_input(const void* x, int dtype, const kfac_
   const int rc = resolve_conv_geometry(geom, &g);
   if (rc) return rc;
   return reduce_conv_input(x, dtype, g, append_ones, scale, out, ld_out, (cudaStream_t)stream);
+}
+
+extern "C" int kfac_reduce_rows_conv_transpose_input(const void* x, int dtype, const kfac_conv_transpose_geometry* geom,
+                                                     int append_ones, float scale, float* out, int ld_out,
+                                                     void* stream) {
+  KFAC_CHECK_ARG(x && out, "null pointer");
+  ConvGeo g;
+  const int rc = resolve_conv_transpose_geometry(geom, &g);
+  if (rc) return rc;
+  return reduce_conv_input<true>(x, dtype, g, append_ones, scale, out, ld_out, (cudaStream_t)stream);
 }
 
 extern "C" int kfac_reduce_rows_conv2d_gradout(const void* g, int dtype, int batch, int C, int Ho, int Wo, float scale,

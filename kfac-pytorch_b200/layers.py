@@ -26,6 +26,10 @@ class ModuleHelper:
     diagonal_a = False      # True: A is diagonal and kept as a vector (embeddings)
     diagonal_g = False      # True: G is approximated by its diagonal and kept as a vector (diagonal_g_layers)
     norm = False            # True: exact per-channel Fisher blocks instead of two factors (precondition_norms)
+    call_kwargs = False     # True: the A hook passes every call's arguments to bind_call (output_size)
+    # 0: the weight gradient is the row-major (g, a - has_bias) gradient matrix; T > 0: it is (C_in, g, T), a transposed
+    # convolution's, with grad-matrix element (r, ci * T + t) at [ci, r, t] (kfac_precond_item.wgrad_taps)
+    wgrad_taps = 0
 
     def __init__(self, module: torch.nn.Module, reduce: bool = False):
         self.module = module
@@ -384,6 +388,10 @@ class ConvNdModuleHelper(ModuleHelper):
     D = kd = 1, H = kh = 1.  Under K-FAC-reduce R = S with the Conv2d constants.  The A-side methods read the tensor
     prepare_input made of the call's input (batched, contiguous, padded for a non-'zeros' padding_mode)."""
 
+    keyword = 'precondition_conv_nd'
+    # the native input-side entries: kfac_factor_{entry}, kfac_rows_{entry}, kfac_reduce_rows_{entry}
+    entry = 'conv_input'
+
     def __init__(self, module: torch.nn.Module, reduce: bool = False):
         super().__init__(module, reduce=reduce)
         self.nd = len(module.kernel_size)
@@ -404,8 +412,7 @@ class ConvNdModuleHelper(ModuleHelper):
             what = (f'a kernel of {taps} taps, beyond the {REDUCE_MAX_TAPS} of the K-FAC-reduce window sums '
                     "(kfac_approx='reduce')")
         if what is not None:
-            raise ValueError(f'precondition_conv_nd: "{name}" ({m.__class__.__name__}) has {what}; add it to '
-                             'skip_layers')
+            raise ValueError(f'{self.keyword}: "{name}" ({m.__class__.__name__}) has {what}; add it to skip_layers')
 
     @property
     def a_factor_shape(self):
@@ -482,9 +489,9 @@ class ConvNdModuleHelper(ModuleHelper):
         return g, g.size(0), g.size(1), math.prod(out)
 
     def _write_reduced_a(self, x, geo, S, out_ptr, ld):
-        _cabi.check(_cabi.load().kfac_reduce_rows_conv_input(x.data_ptr(), _dtype_code(x), C.byref(geo),
-                                                             int(self.has_bias()), 1.0 / (float(S) * S), out_ptr, ld,
-                                                             _cabi.stream_ptr()), 'kfac_reduce_rows_conv_input')
+        fn = f'kfac_reduce_rows_{self.entry}'
+        _cabi.check(getattr(_cabi.load(), fn)(x.data_ptr(), _dtype_code(x), C.byref(geo), int(self.has_bias()),
+                                              1.0 / (float(S) * S), out_ptr, ld, _cabi.stream_ptr()), fn)
 
     def _write_reduced_g(self, g, B, Cc, S, scale, loss_scale, out_ptr, ld):
         _cabi.check(_cabi.load().kfac_reduce_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, 1, S,
@@ -503,12 +510,12 @@ class ConvNdModuleHelper(ModuleHelper):
         scale = 1.0 / (float(B) * float(S) ** 3)
         lib = _cabi.load()
         ones = int(self.has_bias())
-        need = lib.kfac_factor_conv_input_workspace_bytes(C.byref(geo), ones, CONV_ND_WORKSPACE_BYTES)
+        fn = f'kfac_factor_{self.entry}'
+        need = getattr(lib, fn + '_workspace_bytes')(C.byref(geo), ones, CONV_ND_WORKSPACE_BYTES)
         ws = scratch.get(need, x.device)
         # ws_bytes = need, not the scratch buffer's size: the chunking, and so the bits, depend on it
-        _cabi.check(lib.kfac_factor_conv_input(x.data_ptr(), _dtype_code(x), C.byref(geo), ones, scale, acc.data_ptr(),
-                                               ws.data_ptr() if need else None, need, _cabi.stream_ptr()),
-                    'kfac_factor_conv_input')
+        _cabi.check(getattr(lib, fn)(x.data_ptr(), _dtype_code(x), C.byref(geo), ones, scale, acc.data_ptr(),
+                                     ws.data_ptr() if need else None, need, _cabi.stream_ptr()), fn)
 
     def accumulate_g(self, g, acc, grad_scale, scratch=None):
         g, B, Cc, S = self._gradout(g)
@@ -542,8 +549,9 @@ class ConvNdModuleHelper(ModuleHelper):
             self._write_reduced_a(x, geo, S, out.data_ptr(), ld)
             return
         # rows scaled by 1/S, the ones column included (modules.py:170-178)
-        _cabi.check(_cabi.load().kfac_rows_conv_input(x.data_ptr(), _dtype_code(x), C.byref(geo), ones, 1.0 / S,
-                                                      out.data_ptr(), ld, _cabi.stream_ptr()), 'kfac_rows_conv_input')
+        fn = f'kfac_rows_{self.entry}'
+        _cabi.check(getattr(_cabi.load(), fn)(x.data_ptr(), _dtype_code(x), C.byref(geo), ones, 1.0 / S,
+                                              out.data_ptr(), ld, _cabi.stream_ptr()), fn)
 
     def write_rows_g(self, g, out, grad_scale, loss_scale):
         g, B, Cc, S = self._gradout(g)
@@ -554,6 +562,72 @@ class ConvNdModuleHelper(ModuleHelper):
                                                           1.0 / (float(S) * grad_scale), loss_scale, out.data_ptr(),
                                                           _cabi.ld4(Cc), _cabi.stream_ptr()),
                     'kfac_rows_conv2d_gradout')
+
+
+class ConvTransposeModuleHelper(ConvNdModuleHelper):
+    """torch.nn.ConvTranspose1d / 2d / 3d with groups = 1 (an extension beyond the reference, opt-in through
+    `precondition_conv_transpose`).
+
+    y[b, co, o] = bias[co] + sum_{ci, k, i: o = i s - p + k d} x[b, ci, i] W[ci, co, k], so each output position o has
+    the patch a(o)[ci, k] = x[b, ci, (o + p - k d) / s] when s divides (o + p - k d) on every axis and the quotient is
+    an input position, 0 otherwise, and y[:, o] = Wmat a(o) + bias with Wmat[co, ci K + k] = W[ci, co, k].  The rows are
+    the B * S output positions (S the product of the output extents), A and G rows scaled by 1/S as for a Conv2d layer,
+    A's feature order (C_in, kd, kh, kw) [+ ones] and G C_out x C_out; under K-FAC-reduce R = S.  The G side, the
+    extent check of the output gradient and the reduce constants are those of ConvNdModuleHelper.
+
+    The weight gradient (C_in, C_out, k...) is not Wmat's layout: `wgrad_taps` = K tells the native precondition,
+    kl-clip and write-back to address it in place.  The output padding of a call is torch's (`output_size` passed
+    positionally or as a keyword, through bind_call); the padding mode is always 'zeros'."""
+
+    keyword = 'precondition_conv_transpose'
+    entry = 'conv_transpose_input'
+    call_kwargs = True
+
+    def __init__(self, module: torch.nn.Module, reduce: bool = False):
+        super().__init__(module, reduce=reduce)
+        self._call_op = list(module.output_padding)    # output padding of the call bind_call saw last
+
+    @property
+    def wgrad_taps(self) -> int:
+        return math.prod(self.module.kernel_size)
+
+    def get_grad(self) -> torch.Tensor:
+        m = self.module
+        w = m.weight.grad.reshape(m.in_channels, m.out_channels, -1).permute(1, 0, 2).reshape(m.out_channels, -1)
+        return torch.cat([w, m.bias.grad.view(-1, 1)], 1) if self.has_bias() else w
+
+    def bind_call(self, args: tuple, kwargs: dict) -> None:
+        """Take the output padding of a forward call (module(x), module(x, output_size) or module(x,
+        output_size=...)), derived as the module's forward derives it."""
+        m = self.module
+        output_size = args[1] if len(args) > 1 else kwargs.get('output_size')
+        self._call_op = list(m._output_padding(args[0], output_size, m.stride, m.padding, m.kernel_size, self.nd,
+                                               m.dilation))
+
+    def _geometry(self, shape: torch.Size) -> tuple[_cabi.ConvTransposeGeometry, tuple[int, ...]]:
+        """Native geometry and output extents of a batched input of `shape` with the bound call's output padding."""
+        m = self.module
+        lead, zero = [1] * (3 - self.nd), [0] * (3 - self.nd)
+        ins = lead + list(shape[2:])
+        ker, st, dil = (lead + list(v) for v in (m.kernel_size, m.stride, m.dilation))
+        pad, op = zero + list(m.padding), zero + list(self._call_op)
+        out = [(ins[a] - 1) * st[a] - 2 * pad[a] + dil[a] * (ker[a] - 1) + op[a] + 1 for a in range(3)]
+        arr = lambda v: (C.c_int * 3)(*v)  # noqa: E731
+        geo = _cabi.ConvTransposeGeometry(shape[0], shape[1], arr(ins), arr(ker), arr(st), arr(dil), arr(pad), arr(op))
+        return geo, tuple(out[3 - self.nd:])
+
+    def output_extent(self, x_shape: torch.Size) -> tuple[int, ...]:
+        """Output extents of a (possibly unbatched) input of `x_shape` under the bound call's output padding."""
+        shape = list(x_shape) if len(x_shape) == self.nd + 2 else [1] + list(x_shape)
+        return self._geometry(torch.Size(shape))[1]
+
+    def prepare_input(self, x: torch.Tensor) -> torch.Tensor:
+        """The batched, contiguous input the statistics read."""
+        _cabi.require_device(x)
+        if min(self.output_extent(x.shape)) <= 0:
+            raise ValueError(f'{self.module.__class__.__name__}: input of shape {tuple(x.shape)} gives an empty output')
+        x = self._batched(x.detach())
+        return x if x.is_contiguous() else x.contiguous()
 
 
 class EmbeddingModuleHelper(ModuleHelper):
@@ -884,6 +958,7 @@ class AttentionProjectionHelper(LinearModuleHelper):
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
 CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
 CONV_ND_TYPES: tuple[type, ...] = (torch.nn.Conv1d, torch.nn.Conv3d)
+CONV_TRANSPOSE_TYPES: tuple[type, ...] = (torch.nn.ConvTranspose1d, torch.nn.ConvTranspose2d, torch.nn.ConvTranspose3d)
 EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
 # SyncBatchNorm (global statistics), BatchNorm3d, GroupNorm and InstanceNorm* are not among them
 NORM_TYPES: tuple[type, ...] = (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d, torch.nn.LayerNorm, torch.nn.RMSNorm)
@@ -891,15 +966,18 @@ NORM_TYPES: tuple[type, ...] = (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d, torc
 
 def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
                       diagonal_g: bool = False, norms: bool = False, reduce: bool = False,
-                      conv_nd: bool = False) -> ModuleHelper | None:
+                      conv_nd: bool = False, conv_transpose: bool = False) -> ModuleHelper | None:
     """reduce: K-FAC-reduce statistics for Linear (dense and diagonal-G), Conv2d and (with conv_nd) Conv1d / Conv3d
-    layers; embeddings and normalization layers keep their own statistics."""
+    and (with conv_transpose) ConvTranspose1d / 2d / 3d layers; embeddings and normalization layers keep their own
+    statistics."""
     if isinstance(module, LINEAR_TYPES):
         return (DiagonalGLinearModuleHelper if diagonal_g else LinearModuleHelper)(module, reduce=reduce)
     if isinstance(module, CONV2D_TYPES):
         return Conv2dModuleHelper(module, reduce=reduce)
     if conv_nd and isinstance(module, CONV_ND_TYPES):
         return ConvNdModuleHelper(module, reduce=reduce)
+    if conv_transpose and isinstance(module, CONV_TRANSPOSE_TYPES):
+        return ConvTransposeModuleHelper(module, reduce=reduce)
     if embeddings and isinstance(module, EMBEDDING_TYPES):
         return EmbeddingModuleHelper(module)
     if norms and isinstance(module, NORM_TYPES) and getattr(module, 'weight', None) is not None:
@@ -1100,7 +1178,8 @@ def any_match(query: str, patterns: list[str]) -> bool:
 def register_modules(model: torch.nn.Module, skip_layers: list[str], precondition_embeddings: bool = False,
                      diagonal_g_layers: list[str] | None = None, precondition_norms: bool = False,
                      kfac_approx: str = 'expand', precondition_attention: bool = False,
-                     precondition_conv_nd: bool = False, **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
+                     precondition_conv_nd: bool = False, precondition_conv_transpose: bool = False,
+                     **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
     modules (not in the reference).  diagonal_g_layers: regexes on name and class name; a registered
@@ -1112,7 +1191,9 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     `{name}.q_proj`, `.k_proj`, `.v_proj` and `.out_proj`, keyed by their AttentionProjectionHelper
     (not in the reference); the `out_proj` leaf of an attention is then never registered as a Linear.
     precondition_conv_nd: also register torch.nn.Conv1d and Conv3d modules (not in the reference); grouped ones and
-    ones whose factors exceed the eigensolver are an error.  `layer.index` counts the other layers and the normalization layers separately."""
+    ones whose factors exceed the eigensolver are an error.  precondition_conv_transpose: also register
+    torch.nn.ConvTranspose1d, 2d and 3d modules (not in the reference), with the same errors.  `layer.index` counts the
+    other layers and the normalization layers separately."""
     diagonal_g_layers = diagonal_g_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     counts = [0, 0]
@@ -1135,7 +1216,7 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
         diag_g = any_match(name, diagonal_g_layers) or any_match(module.__class__.__name__, diagonal_g_layers)
         helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g,
                                    norms=precondition_norms, reduce=kfac_approx == 'reduce',
-                                   conv_nd=precondition_conv_nd)
+                                   conv_nd=precondition_conv_nd, conv_transpose=precondition_conv_transpose)
         if helper is None:
             continue
         if diag_g and not helper.diagonal_g:

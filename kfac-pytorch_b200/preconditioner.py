@@ -215,6 +215,20 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     `kfac_b200.layers.ConvNdModuleHelper`.  Refused with a ValueError naming the layer: `groups != 1`, an A dimension
     C_in * kd * kh * kw (+ bias) or `out_channels` above `KFAC_EIGH_MAX_N` (8192), and a `diagonal_g_layers` match.
     Conv2d layers are unaffected by the keyword.
+
+    `precondition_conv_transpose=True` also registers leaf `torch.nn.ConvTranspose1d`, `ConvTranspose2d` and
+    `ConvTranspose3d` modules whose parameters all require grad: the upsampling layers of DCGAN-style generators, U-Net
+    and FCN decoders, 1-D audio upsamplers and 3-D segmentation decoders, which the reference leaves to the first-order
+    optimizer.  Output position o of such a layer reads input (o + p - k d) / s through tap k where s divides
+    (o + p - k d), zero elsewhere; its rows are the B * S output positions with the Conv2d constants (A and G rows
+    scaled by 1/S, 'reduce': R = S), A's features (C_in, kd, kh, kw) [+ ones] and G C_out x C_out.  The gradient
+    matrix is the weight gradient (C_in, C_out, k...) permuted to (C_out, C_in * K); the precondition, the kl-clip
+    inner product and the write-back read and write the weight gradient in place in its own layout.  `output_size`,
+    positional or keyword, sets the output padding as the module's forward does.  It works with unbatched inputs,
+    `kfac_approx`, EKFAC, `grad_scaler`, `accumulation_steps`, `factor_dtype` and every distributed strategy; see
+    `kfac_b200.layers.ConvTransposeModuleHelper`.  Refused with a ValueError naming the layer and `skip_layers`:
+    `groups != 1`, an A dimension C_in * K (+ bias) or `out_channels` above `KFAC_EIGH_MAX_N` (8192), more than 2048
+    taps under 'reduce', and a `diagonal_g_layers` match.
     """
 
     def __init__(
@@ -248,6 +262,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         precondition_attention: bool = False,
         precondition_tied_embeddings: bool = False,
         precondition_conv_nd: bool = False,
+        precondition_conv_transpose: bool = False,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -333,6 +348,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             model, self.skip_layers, precondition_embeddings=precondition_embeddings,
             diagonal_g_layers=diagonal_g_layers, precondition_norms=precondition_norms, kfac_approx=kfac_approx,
             precondition_attention=precondition_attention, precondition_conv_nd=precondition_conv_nd,
+            precondition_conv_transpose=precondition_conv_transpose,
             method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
@@ -373,6 +389,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'precondition_attention': precondition_attention,
             'precondition_tied_embeddings': precondition_tied_embeddings,
             'precondition_conv_nd': precondition_conv_nd,
+            'precondition_conv_transpose': precondition_conv_transpose,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
