@@ -254,6 +254,18 @@ size_t kfac_factor_norm_workspace_bytes(int kind, int64_t rows, int C, int64_t S
 int kfac_factor_norm(const void* x, int x_dtype, const void* g, int g_dtype, int kind, int64_t rows,
                      int C, int64_t S, int k, double eps, float scale, float* acc, void* ws,
                      size_t ws_bytes, void* stream);
+/* kfac_factor_group_norm: the same contract as kfac_factor_norm for GroupNorm and InstanceNorm*
+ * (groups = C): x, g are (B, C, S) contiguous; xhat uses the mean and biased variance, plus eps, of
+ * each example's group, the Cg * S entries of channels [gi * Cg, (gi + 1) * Cg) with Cg = C / groups.
+ * acc (C x k) += scale * sum_{b,s} g^2 a a^T.  x and g take any of KFAC_F32/F16/BF16 independently
+ * and are read once each; the sums are fp64, reduced in a fixed order, so the same input gives the
+ * same bits; no floating-point atomics, no host sync.  Refused: groups not dividing C, k not 1 or 3,
+ * B * C * S >= 2^31.  ws: kfac_factor_group_norm_workspace_bytes(B, C, S, groups) bytes (B * C * 5
+ * doubles of plane sums and B * groups (mean, 1/std) pairs).  Three launches. */
+size_t kfac_factor_group_norm_workspace_bytes(int64_t B, int C, int64_t S, int groups);
+int kfac_factor_group_norm(const void* x, int x_dtype, const void* g, int g_dtype, int64_t B, int C,
+                           int64_t S, int groups, int k, double eps, float scale, float* acc,
+                           void* ws, size_t ws_bytes, void* stream);
 /* P_c = (F_c + damping I)^-1 (wgrad[c], bgrad[c]) for every channel of every item, in fp64, written
  * as P (C x np, ld = np, np = 2 with a bias, else 1): the weight in column 0 and the bias in the last
  * column, the layout kfac_grad_scale / kfac_grad_update read for g = C, a = np.  F is the C x k

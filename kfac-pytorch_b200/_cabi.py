@@ -69,6 +69,8 @@ class TiedItem(C.Structure):
 
 
 KFAC_NORM_BATCH, KFAC_NORM_LAYER, KFAC_NORM_RMS = 0, 1, 2
+# GroupNorm / InstanceNorm*: the statistics of kfac_factor_group_norm (not a kind kfac_factor_norm takes)
+KFAC_NORM_GROUP = 3
 
 
 class NormItem(C.Structure):
@@ -131,6 +133,9 @@ SIGNATURES = {
     'kfac_factor_norm_workspace_bytes': (c_size_t, [c_int, c_int64, c_int, c_int64]),
     'kfac_factor_norm': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int64, c_int, c_int64, c_int, C.c_double,
                                  c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'kfac_factor_group_norm_workspace_bytes': (c_size_t, [c_int64, c_int, c_int64, c_int]),
+    'kfac_factor_group_norm': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_int64, c_int, c_int,
+                                       C.c_double, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     'kfac_norm_precondition_workspace_bytes': (c_size_t, [c_int]),
     'kfac_norm_precondition': (c_int, [C.POINTER(NormItem), c_int, c_float, c_void_p, c_size_t, c_void_p]),
     'kfac_eigh_workspace_bytes': (c_size_t, [C.POINTER(c_int), c_int]),

@@ -1,10 +1,12 @@
-// Normalization layers (BatchNorm, LayerNorm, RMSNorm; an extension beyond the reference, opt-in): the exact
-// per-channel Fisher block of the affine part y = s * xhat + b, and its damped 2 x 2 (or 1 x 1) solve.
+// Normalization layers (BatchNorm, LayerNorm, RMSNorm, GroupNorm, InstanceNorm; an extension beyond the reference,
+// opt-in): the exact per-channel Fisher block of the affine part y = s * xhat + b, and its damped 2 x 2 (or 1 x 1)
+// solve.
 //
 // A channel c is a one-input layer with bias acting on xhat, so its rows are a_r = (xhat_rc, 1) and g_r, and
 //   F_c = (1/N) sum_r g_rc^2 a_r a_r^T = (1/N) (sum g^2 xhat^2, sum g^2 xhat, sum g^2)      (k = 3 packed entries)
 // or (1/N) sum g^2 xhat^2 alone for a scale-only layer (k = 1).  xhat is recomputed from the layer input: BatchNorm
-// with the biased batch statistics of each channel, LayerNorm / RMSNorm with the statistics of each row.
+// with the biased batch statistics of each channel, LayerNorm / RMSNorm with the statistics of each row, GroupNorm /
+// InstanceNorm with the statistics of each example and group.
 //
 // Every sum is accumulated in fp64, every reduction runs in a fixed order and the chunking depends on the shape only:
 // the same input gives the same bits.  No floating-point atomics, no host sync.
@@ -221,6 +223,188 @@ __global__ void row_finalize_kernel(const double* __restrict__ partial, int chun
   }
 }
 
+// ================================================================ GroupNorm / InstanceNorm: x, g are (B, C, S)
+// xhat is normalized per example and group: group gi of example b is the Cg * S contiguous elements of channels
+// [gi * Cg, (gi + 1) * Cg).  Three launches:
+// (1) one pass over x and g: the five NC_SUMS of each (b, c) plane, of y = x - K_bg with the shift K_bg the group's
+//     first element (so a group with |mean| >> std keeps its variance), stored at plane[(b * C + c) * 5 + q];
+// (2) one warp per (b, gi): the Cg planes' sum y and sum y^2 in channel order -> (m_bg, r_bg), the mean of y and
+//     1 / sqrt(var + eps);
+// (3) one thread per channel: for b = 0 .. B-1 in order, the BatchNorm formulas with (m_bg, r_bg), then
+//     acc += scale * F_c.
+// (2) is its own launch so that (3) reads one (m, r) pair per example instead of all Cg planes of the group, which
+// for GroupNorm(1, C) would be B * C serial reads in every thread.
+// Planes of up to GN_WARP_MAX_S elements take a warp each, eight per block.  Larger planes take a block each, unless
+// there are so many that warps alone fill the device (16 x 16 and 32 x 32 maps of a U-Net at batch 64): a block per
+// 256-element plane spends more time in its reduction than in its loads.
+constexpr int GN_WARP_MAX_S = 255, GN_WARP_MAX_S_MANY = 4096;
+constexpr int64_t GN_MANY_PLANES = 4096;
+
+static bool gn_warp_per_plane(int64_t planes, int64_t S) {
+  return S <= GN_WARP_MAX_S || (S <= GN_WARP_MAX_S_MANY && planes >= GN_MANY_PLANES);
+}
+
+template <typename TX, typename TG>
+__device__ __forceinline__ void gn_add(const TX* __restrict__ x, const TG* __restrict__ g, int64_t off, double K,
+                                       double (&v)[NC_SUMS]) {
+  const double y = (double)to_float<TX>(x[off]) - K;
+  const double gv = (double)to_float<TG>(g[off]);
+  const double g2 = gv * gv, g2y = g2 * y;
+  v[0] += y;
+  v[1] = fma(y, y, v[1]);
+  v[2] += g2;
+  v[3] += g2y;
+  v[4] = fma(g2y, y, v[4]);
+}
+
+__device__ __forceinline__ void gn_store(double* __restrict__ plane, int64_t p, const double (&v)[NC_SUMS]) {
+#pragma unroll
+  for (int q = 0; q < NC_SUMS; ++q) plane[p * NC_SUMS + q] = v[q];
+}
+
+// the other planes: block p = b * C + c walks its plane
+template <typename TX, typename TG>
+__global__ void __launch_bounds__(256) gn_plane_block_kernel(const TX* __restrict__ x, const TG* __restrict__ g,
+                                                             int C, int Cg, int64_t S, double* __restrict__ plane) {
+  const int64_t p = blockIdx.x;
+  const int c = (int)(p % C);
+  const double K = (double)to_float<TX>(x[(p - c % Cg) * S]);
+  double v[NC_SUMS] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  const int64_t base = p * S;
+#pragma unroll 4
+  for (int64_t i = threadIdx.x; i < S; i += 256) gn_add(x, g, base + i, K, v);
+  block_sum<NC_SUMS>(v);
+  if (threadIdx.x == 0) gn_store(plane, p, v);
+}
+
+// S >= 2 with gn_warp_per_plane (7 x 7, 8 x 8, short sequences, or many mid-sized planes): one warp per plane, eight
+// planes per block
+template <typename TX, typename TG>
+__global__ void __launch_bounds__(256) gn_plane_warp_kernel(const TX* __restrict__ x, const TG* __restrict__ g,
+                                                            int64_t planes, int C, int Cg, int S,
+                                                            double* __restrict__ plane) {
+  const int64_t p = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (p >= planes) return;
+  const int c = (int)(p % C);
+  const double K = (double)to_float<TX>(x[(p - c % Cg) * S]);
+  double v[NC_SUMS] = {0.0, 0.0, 0.0, 0.0, 0.0};
+#pragma unroll 4
+  for (int i = lane; i < S; i += 32) gn_add(x, g, p * S + i, K, v);
+#pragma unroll
+  for (int q = 0; q < NC_SUMS; ++q)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+  if (lane == 0) gn_store(plane, p, v);
+}
+
+// S = 1 (GroupNorm on (B, C)): one thread per (b, c), coalesced over the channels
+template <typename TX, typename TG>
+__global__ void __launch_bounds__(256) gn_plane_flat_kernel(const TX* __restrict__ x, const TG* __restrict__ g,
+                                                            int64_t planes, int C, int Cg,
+                                                            double* __restrict__ plane) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= planes) return;
+  const int c = (int)(p % C);
+  const double K = (double)to_float<TX>(x[p - c % Cg]);
+  double v[NC_SUMS] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  gn_add(x, g, p, K, v);
+  gn_store(plane, p, v);
+}
+
+// one warp per (b, gi): (mean of y, 1 / sqrt(var + eps)) over the group's Cg * S elements
+__global__ void __launch_bounds__(256) gn_group_stats_kernel(const double* __restrict__ plane, int64_t B, int groups,
+                                                             int Cg, double n, double eps,
+                                                             double2* __restrict__ stats) {
+  const int64_t bg = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (bg >= B * groups) return;
+  const double* pl = plane + bg * Cg * NC_SUMS;   // the group's planes are consecutive: (b * G + gi) * Cg + j
+  double s0 = 0.0, s1 = 0.0;
+  for (int j = lane; j < Cg; j += 32) {
+    s0 += pl[(int64_t)j * NC_SUMS];
+    s1 += pl[(int64_t)j * NC_SUMS + 1];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+  }
+  if (lane == 0) {
+    const double m = s0 / n;
+    const double var = fmax(s1 / n - m * m, 0.0);
+    stats[bg] = make_double2(m, 1.0 / sqrt(var + eps));
+  }
+}
+
+// acc[c * k + .] += scale * F_c, the examples added in order
+__global__ void gn_finalize_kernel(const double* __restrict__ plane, const double2* __restrict__ stats, int64_t B,
+                                   int C, int Cg, int k, float scale, float* acc) {
+  const int groups = C / Cg;
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < C; c += gridDim.x * blockDim.x) {
+    const int gi = c / Cg;
+    double fss = 0.0, fsb = 0.0, fbb = 0.0;
+    for (int64_t b = 0; b < B; ++b) {
+      const double2 st = stats[b * groups + gi];
+      const double* v = plane + (b * C + c) * NC_SUMS;
+      const double m = st.x, r = st.y;
+      fss += (v[4] - 2.0 * m * v[3] + m * m * v[2]) * r * r;
+      fsb += (v[3] - m * v[2]) * r;
+      fbb += v[2];
+    }
+    const double s = (double)scale;
+    if (k == 1) {
+      acc[c] = __fadd_rn(acc[c], (float)(s * fss));
+    } else {
+      acc[3 * c] = __fadd_rn(acc[3 * c], (float)(s * fss));
+      acc[3 * c + 1] = __fadd_rn(acc[3 * c + 1], (float)(s * fsb));
+      acc[3 * c + 2] = __fadd_rn(acc[3 * c + 2], (float)(s * fbb));
+    }
+  }
+}
+
+struct GroupNormArgs {
+  const void* x; const void* g;
+  int64_t B; int C; int64_t S; int groups; int k; double eps; float scale; float* acc; void* ws;
+};
+
+static size_t group_norm_ws_bytes(int64_t B, int C, int groups) {
+  return align_up((size_t)B * (size_t)C * NC_SUMS * sizeof(double), 256) +
+         align_up((size_t)B * (size_t)groups * sizeof(double2), 256);
+}
+
+template <typename TX, typename TG>
+static int launch_group_norm(const GroupNormArgs& a, cudaStream_t s) {
+  const TX* x = (const TX*)a.x;
+  const TG* g = (const TG*)a.g;
+  const int Cg = a.C / a.groups;
+  const int64_t planes = a.B * a.C;
+  double* plane = (double*)a.ws;
+  double2* stats = (double2*)((char*)a.ws + align_up((size_t)planes * NC_SUMS * sizeof(double), 256));
+  if (a.S == 1) {
+    gn_plane_flat_kernel<TX, TG><<<(unsigned)ceil_div(planes, 256), 256, 0, s>>>(x, g, planes, a.C, Cg, plane);
+  } else if (gn_warp_per_plane(planes, a.S)) {
+    gn_plane_warp_kernel<TX, TG><<<(unsigned)ceil_div(planes, 8), 256, 0, s>>>(x, g, planes, a.C, Cg, (int)a.S,
+                                                                                plane);
+  } else {
+    gn_plane_block_kernel<TX, TG><<<(unsigned)planes, 256, 0, s>>>(x, g, a.C, Cg, a.S, plane);
+  }
+  KFAC_LAUNCH_CHECK();
+  gn_group_stats_kernel<<<(unsigned)ceil_div(a.B * a.groups, 8), 256, 0, s>>>(plane, a.B, a.groups, Cg,
+                                                                               (double)Cg * (double)a.S, a.eps, stats);
+  KFAC_LAUNCH_CHECK();
+  gn_finalize_kernel<<<norm_grid_for(a.C), 256, 0, s>>>(plane, stats, a.B, a.C, Cg, a.k, a.scale, a.acc);
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
+template <typename TX>
+static int launch_group_norm_g(const GroupNormArgs& a, int g_dtype, cudaStream_t s) {
+  if (g_dtype == KFAC_F32) return launch_group_norm<TX, float>(a, s);
+  if (g_dtype == KFAC_F16) return launch_group_norm<TX, __half>(a, s);
+  return launch_group_norm<TX, __nv_bfloat16>(a, s);
+}
+
 // ---------------------------------------------------------------- launch
 struct NormArgs {
   const void* x; const void* g;
@@ -334,6 +518,33 @@ extern "C" int kfac_factor_norm(const void* x, int x_dtype, const void* g, int g
   if (x_dtype == KFAC_F32) return launch_norm_g<float>(a, g_dtype, s);
   if (x_dtype == KFAC_F16) return launch_norm_g<__half>(a, g_dtype, s);
   return launch_norm_g<__nv_bfloat16>(a, g_dtype, s);
+}
+
+extern "C" size_t kfac_factor_group_norm_workspace_bytes(int64_t B, int C, int64_t S, int groups) {
+  if (B <= 0 || C <= 0 || S <= 0 || groups <= 0 || C % groups != 0) return 0;
+  return group_norm_ws_bytes(B, C, groups);
+}
+
+extern "C" int kfac_factor_group_norm(const void* x, int x_dtype, const void* g, int g_dtype, int64_t B, int C,
+                                      int64_t S, int groups, int k, double eps, float scale, float* acc, void* ws,
+                                      size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(acc && C > 0 && B >= 0 && S > 0 && ((x && g) || B == 0), "factor_group_norm args");
+  KFAC_CHECK_ARG(groups > 0 && C % groups == 0, "groups must divide the channels");
+  KFAC_CHECK_ARG(k == 1 || k == 3, "k must be 1 or 3");
+  KFAC_CHECK_ARG(eps >= 0.0, "eps");
+  for (int d : {x_dtype, g_dtype}) KFAC_CHECK_ARG(d == KFAC_F32 || d == KFAC_F16 || d == KFAC_BF16, "dtype");
+  KFAC_CHECK_ARG(B * (int64_t)C * S < (1ll << 31), "2^31 or more elements");
+  if (B == 0) return KFAC_OK;
+  const size_t need = kfac_factor_group_norm_workspace_bytes(B, C, S, groups);
+  if (!ws || ws_bytes < need) {
+    set_error("factor_group_norm: workspace too small (%zu < %zu)", ws_bytes, need);
+    return KFAC_ERR_WORKSPACE;
+  }
+  const GroupNormArgs a{x, g, B, C, S, groups, k, eps, scale, acc, ws};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (x_dtype == KFAC_F32) return launch_group_norm_g<float>(a, g_dtype, s);
+  if (x_dtype == KFAC_F16) return launch_group_norm_g<__half>(a, g_dtype, s);
+  return launch_group_norm_g<__nv_bfloat16>(a, g_dtype, s);
 }
 
 extern "C" size_t kfac_norm_precondition_workspace_bytes(int count) {

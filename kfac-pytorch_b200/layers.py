@@ -706,8 +706,9 @@ class DiagonalGLinearModuleHelper(LinearModuleHelper):
 
 
 class NormModuleHelper(ModuleHelper):
-    """torch.nn.BatchNorm1d / BatchNorm2d / LayerNorm / RMSNorm with an affine part (an extension beyond the
-    reference, opt-in through `precondition_norms`).
+    """torch.nn.BatchNorm1d / BatchNorm2d / LayerNorm / RMSNorm (opt-in through `precondition_norms`) and GroupNorm /
+    InstanceNorm1d / 2d / 3d (opt-in through `precondition_group_norms`) with an affine part (an extension beyond the
+    reference).
 
     The affine part y = s * xhat + b is a depthwise layer with bias on the normalized input, so each channel c is a
     one-input layer with rows a_r = (xhat_rc, 1) (or (xhat_rc) for a scale-only layer) and g_r = dL/dy_rc.  Instead
@@ -723,19 +724,27 @@ class NormModuleHelper(ModuleHelper):
       * BatchNorm1d on (B, C), LayerNorm, RMSNorm: every leading position is a row, unscaled, as for nn.Linear;
         xhat from the statistics of each row over `normalized_shape` (mean and biased variance plus eps, or
         x / sqrt(mean(x^2) + eps); when the module's eps is None, torch's: finfo(float32).eps for fp16, bf16 and
-        fp32 inputs, finfo(float64).eps for fp64 inputs).
+        fp32 inputs, finfo(float64).eps for fp64 inputs);
+      * GroupNorm, InstanceNorm* (kind KFAC_NORM_GROUP): the rows of BatchNorm (B * S positions scaled by 1/S; S = 1
+        and unscaled for a GroupNorm on (B, C)); xhat from the mean and biased variance plus eps of each example's
+        group of C / `groups` channels (`groups` = num_groups, or C for an InstanceNorm).  An unbatched
+        InstanceNorm input is one example.
     xhat is recomputed from the layer input, so a gain near zero does not affect it."""
 
     norm = True
 
     def __init__(self, module: torch.nn.Module):
         super().__init__(module)
+        self.groups = 0             # the number of groups of a KFAC_NORM_GROUP layer
         if isinstance(module, (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d)):
             self.kind = _cabi.KFAC_NORM_BATCH
         elif isinstance(module, torch.nn.LayerNorm):
             self.kind = _cabi.KFAC_NORM_LAYER
-        else:
+        elif isinstance(module, torch.nn.RMSNorm):
             self.kind = _cabi.KFAC_NORM_RMS
+        else:
+            self.kind = _cabi.KFAC_NORM_GROUP
+            self.groups = module.num_groups if isinstance(module, torch.nn.GroupNorm) else module.num_features
 
     @property
     def channels(self) -> int:
@@ -783,6 +792,24 @@ class NormModuleHelper(ModuleHelper):
         C = self.channels
         if x.numel() == 0:
             return
+        lib = _cabi.load()
+        if self.kind == _cabi.KFAC_NORM_GROUP:
+            # an InstanceNorm input without the batch dimension is one example, detected as the module's forward does
+            unbatched = (not isinstance(self.module, torch.nn.GroupNorm)
+                         and x.dim() == self.module._get_no_batch_dim())
+            xb = x.unsqueeze(0) if unbatched else x
+            if xb.dim() < 2 or xb.size(1) != C or (not isinstance(self.module, torch.nn.GroupNorm)
+                                                   and xb.dim() != self.module._get_no_batch_dim() + 1):
+                raise ValueError(f'{self.module.__class__.__name__} input of shape {tuple(x.shape)} for {C} channels')
+            B, S = xb.size(0), x.numel() // (xb.size(0) * C)
+            # the rows of BatchNorm: N = B * S, a_r and g_r scaled by 1/S (as a Conv2d layer's): 1 / (N * S^4)
+            scale = 1.0 / (float(B) * float(S) ** 5 * grad_scale * grad_scale)
+            need = lib.kfac_factor_group_norm_workspace_bytes(B, C, S, self.groups)
+            ws = scratch.get(need, x.device)
+            _cabi.check(lib.kfac_factor_group_norm(x.data_ptr(), _dtype_code(x), g.data_ptr(), _dtype_code(g), B, C,
+                                                   S, self.groups, self.k, eps, scale, acc.data_ptr(), ws.data_ptr(),
+                                                   need, _cabi.stream_ptr()), 'kfac_factor_group_norm')
+            return
         if self.kind == _cabi.KFAC_NORM_BATCH:
             if x.dim() not in (2, 3, 4) or x.size(1) != C:
                 raise ValueError(f'BatchNorm input of shape {tuple(x.shape)} for {C} channels')
@@ -792,7 +819,6 @@ class NormModuleHelper(ModuleHelper):
         else:
             rows, S = x.numel() // C, 1
             scale = 1.0 / (float(rows) * grad_scale * grad_scale)
-        lib = _cabi.load()
         need = lib.kfac_factor_norm_workspace_bytes(self.kind, rows, C, S)
         ws = scratch.get(need, x.device)
         _cabi.check(lib.kfac_factor_norm(x.data_ptr(), _dtype_code(x), g.data_ptr(), _dtype_code(g), self.kind, rows,
@@ -960,13 +986,17 @@ CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
 CONV_ND_TYPES: tuple[type, ...] = (torch.nn.Conv1d, torch.nn.Conv3d)
 CONV_TRANSPOSE_TYPES: tuple[type, ...] = (torch.nn.ConvTranspose1d, torch.nn.ConvTranspose2d, torch.nn.ConvTranspose3d)
 EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
-# SyncBatchNorm (global statistics), BatchNorm3d, GroupNorm and InstanceNorm* are not among them
+# SyncBatchNorm (global statistics) and BatchNorm3d are in neither tuple; GroupNorm and InstanceNorm* are registered
+# through their own keyword (precondition_group_norms)
 NORM_TYPES: tuple[type, ...] = (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d, torch.nn.LayerNorm, torch.nn.RMSNorm)
+GROUP_NORM_TYPES: tuple[type, ...] = (torch.nn.GroupNorm, torch.nn.InstanceNorm1d, torch.nn.InstanceNorm2d,
+                                      torch.nn.InstanceNorm3d)
 
 
 def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
                       diagonal_g: bool = False, norms: bool = False, reduce: bool = False,
-                      conv_nd: bool = False, conv_transpose: bool = False) -> ModuleHelper | None:
+                      conv_nd: bool = False, conv_transpose: bool = False,
+                      group_norms: bool = False) -> ModuleHelper | None:
     """reduce: K-FAC-reduce statistics for Linear (dense and diagonal-G), Conv2d and (with conv_nd) Conv1d / Conv3d
     and (with conv_transpose) ConvTranspose1d / 2d / 3d layers; embeddings and normalization layers keep their own
     statistics."""
@@ -982,6 +1012,8 @@ def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
         return EmbeddingModuleHelper(module)
     if norms and isinstance(module, NORM_TYPES) and getattr(module, 'weight', None) is not None:
         return NormModuleHelper(module)      # affine=False / elementwise_affine=False: nothing to precondition
+    if group_norms and isinstance(module, GROUP_NORM_TYPES) and getattr(module, 'weight', None) is not None:
+        return NormModuleHelper(module)      # affine=False: nothing to precondition
     return None
 
 
@@ -1179,6 +1211,7 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
                      diagonal_g_layers: list[str] | None = None, precondition_norms: bool = False,
                      kfac_approx: str = 'expand', precondition_attention: bool = False,
                      precondition_conv_nd: bool = False, precondition_conv_transpose: bool = False,
+                     precondition_group_norms: bool = False,
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
@@ -1192,8 +1225,9 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     (not in the reference); the `out_proj` leaf of an attention is then never registered as a Linear.
     precondition_conv_nd: also register torch.nn.Conv1d and Conv3d modules (not in the reference); grouped ones and
     ones whose factors exceed the eigensolver are an error.  precondition_conv_transpose: also register
-    torch.nn.ConvTranspose1d, 2d and 3d modules (not in the reference), with the same errors.  `layer.index` counts the
-    other layers and the normalization layers separately."""
+    torch.nn.ConvTranspose1d, 2d and 3d modules (not in the reference), with the same errors.
+    precondition_group_norms: also register GroupNorm and InstanceNorm1d/2d/3d modules with affine parameters (not in
+    the reference; `layer.norm`).  `layer.index` counts the other layers and the normalization layers separately."""
     diagonal_g_layers = diagonal_g_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     counts = [0, 0]
@@ -1216,7 +1250,8 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
         diag_g = any_match(name, diagonal_g_layers) or any_match(module.__class__.__name__, diagonal_g_layers)
         helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g,
                                    norms=precondition_norms, reduce=kfac_approx == 'reduce',
-                                   conv_nd=precondition_conv_nd, conv_transpose=precondition_conv_transpose)
+                                   conv_nd=precondition_conv_nd, conv_transpose=precondition_conv_transpose,
+                                   group_norms=precondition_group_norms)
         if helper is None:
             continue
         if diag_g and not helper.diagonal_g:

@@ -159,7 +159,20 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     SyncBatchNorm the BatchNorm statistics are those of each rank's batch, so the all-reduced block is the mean of
     the ranks' blocks.  At factor steps each norm call's input is held until its output's gradient arrives; inside a
     non-reentrant `torch.utils.checkpoint` region that keeps activations the checkpointing would drop.  Not
-    registered: modules without affine parameters, SyncBatchNorm, BatchNorm3d, GroupNorm and InstanceNorm*.
+    registered: modules without affine parameters, SyncBatchNorm, BatchNorm3d, and GroupNorm and InstanceNorm*, which
+    `precondition_group_norms` covers.
+
+    `precondition_group_norms=True` also registers leaf `torch.nn.GroupNorm`, `InstanceNorm1d`, `InstanceNorm2d` and
+    `InstanceNorm3d` modules whose affine parameters exist and all require grad: the normalization of diffusion U-Nets
+    (`GroupNorm(32, C)`), ConvNeXt-style `GroupNorm(1, C)`, and image-to-image and 3-D medical generators
+    (`InstanceNorm2d/3d(affine=True)`).  They take the blocks, P, schedule and local handling of `precondition_norms`
+    with xhat normalized per example and group: for input (B, C, *) with S = prod(*) positions and G groups of
+    Cg = C / G channels (G = C for an InstanceNorm), mu and the biased variance are those of the Cg * S entries of
+    each example's group, and the rows are BatchNorm's (N = B * S positions, a_r and g_r scaled by 1/S; S = 1 for a
+    GroupNorm on (B, C)).  An unbatched InstanceNorm input is one example.  The statistics are exact per example, so
+    with several ranks the all-reduced block is the mean of the ranks' blocks.  The keyword is independent of
+    `precondition_norms`; both may be on.  Not registered: modules without affine parameters or with a frozen one.
+    A `diagonal_g_layers` match is a ValueError, and `skip_layers` takes precedence.
 
     `kfac_approx` chooses the statistics of weight-sharing layers (Eschenhagen et al., 2023): a `torch.nn.Linear`
     on (B, ..., d) applies one weight at R = numel / (B * d) positions of each example, a `torch.nn.Conv2d` at
@@ -263,6 +276,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         precondition_tied_embeddings: bool = False,
         precondition_conv_nd: bool = False,
         precondition_conv_transpose: bool = False,
+        precondition_group_norms: bool = False,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -349,6 +363,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             diagonal_g_layers=diagonal_g_layers, precondition_norms=precondition_norms, kfac_approx=kfac_approx,
             precondition_attention=precondition_attention, precondition_conv_nd=precondition_conv_nd,
             precondition_conv_transpose=precondition_conv_transpose,
+            precondition_group_norms=precondition_group_norms,
             method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
@@ -390,6 +405,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'precondition_tied_embeddings': precondition_tied_embeddings,
             'precondition_conv_nd': precondition_conv_nd,
             'precondition_conv_transpose': precondition_conv_transpose,
+            'precondition_group_norms': precondition_group_norms,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
