@@ -328,7 +328,10 @@ int kfac_dgda(const float* dg, const float* da, int g, int a, float damping,
 
 /* K7: replaces KFACInverseLayer.compute_{a,g}_inv (kfac/layers/inverse.py:
  * 186-213): inv = (F + damping I)^-1, formed as Q diag(1/(d+damping)) Q^T from
- * the eigendecomposition of F (F is symmetric PSD). ws: n*ldq floats. */
+ * the eigendecomposition of F (F is symmetric PSD). ws: n*ldq floats.
+ * Deterministic: the same inputs give the same bits in every call.  For n > 1024 the product's
+ * reduction runs as chains of at most 512 on the tensor cores, one after another into inv (the
+ * first stores, each later one adds), never with floating-point atomics. */
 int kfac_inverse_from_eigh(const float* Q, int ldq, const float* d, int n,
                            float damping, float* inv, int ld_inv, void* ws,
                            size_t ws_bytes, void* stream);

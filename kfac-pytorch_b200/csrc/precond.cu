@@ -147,8 +147,6 @@ static inline int grid_for(int64_t total) {
 struct Epi { int kind = EPI_NONE; const float* E = nullptr; int64_t lde = 0;
              const float* dg = nullptr; const float* da = nullptr; float damping = 0.f; };
 
-// D (M x N, ldd) = epi(A B^T), A (M x K, lda), B (N x K, ldb): tensor-core engine for
-// aligned operands with at least one full tile worth of work, SIMT engine otherwise.
 // row-major (rows x ld) copy of D into the peers' buffers (layers that did not go through
 // the tensor-core epilogue)
 __global__ void peer_scatter_kernel(const float* D, int64_t total, float* p0, float* p1, float* p2, float* p3,
@@ -161,20 +159,11 @@ __global__ void peer_scatter_kernel(const float* D, int64_t total, float* p0, fl
   }
 }
 
-// D[m][n] = sum_sp slab[sp][m][n] (fixed order) -- second half of the deterministic split-K
-__global__ void reduce_slabs_kernel(const float* slab, int64_t slab_stride, int splits, float* D, int64_t total) {
-  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    float t = slab[idx];
-    for (int sp = 1; sp < splits; ++sp) t += slab[(int64_t)sp * slab_stride + idx];
-    D[idx] = t;
-  }
-}
-
-// slab / slab_floats: optional workspace for a DETERMINISTIC split-K (partial tiles stored per split, then summed
-// in a fixed order); without it long reductions use atomic accumulation (order not reproducible).
+// D (M x N, ldd) = epi(A B^T), A (M x K, lda), B (N x K, ldb): tensor-core engine for
+// aligned operands with at least one full tile worth of work, SIMT engine otherwise.
+// Deterministic: no floating-point atomics on any path.
 int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M, int N,
-            int K, const Epi& e, cudaStream_t s, float* const* peers = nullptr, int npeer = 0, float* slab = nullptr,
-            size_t slab_floats = 0) {
+            int K, const Epi& e, cudaStream_t s, float* const* peers = nullptr, int npeer = 0) {
   TcGemmArgs t{};
   t.npeer = 0;
   t.A = A; t.lda = lda; t.B = B; t.ldb = ldb; t.D = D; t.ldd = ldd; t.M = M; t.N = N; t.K = K;
@@ -187,23 +176,20 @@ int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, 
       return launch_tc_gemm(t, s);
     }
     if (e.kind == EPI_NONE && K > 1024) {
-      // long reductions are split across CTAs: the tensor-core accumulator truncates, so short chains
-      // keep the 3xTF32 result at fp32 accuracy, and small tile counts fill the SMs.
-      const int splits = ceil_div(K, 512);
-      const int64_t stride = (int64_t)M * ldd;
-      if (slab && slab_floats >= (size_t)splits * stride) {
-        // deterministic: every split stores its partial tile, a second pass adds them in a fixed order
-        t.slab = slab; t.slab_stride = stride; t.splits = splits;
-        const int rc = launch_tc_gemm(t, s);
+      // long reductions run as chains of <= 512, split the way the engine splits k-blocks for ceil(K / 512)
+      // splits: the tensor-core accumulator truncates, so short chains keep the 3xTF32 result at fp32 accuracy.
+      // The chains run in order on the stream, the first storing D and each later one adding its product to D
+      // (plain read-modify-write epilogue), so the sum has one fixed order; the TMA maps zero-fill past a chain.
+      constexpr int KB = 32;                    // the engine's k-block
+      const int kb_total = ceil_div(K, KB);
+      const int chain = ceil_div(kb_total, tc_normalize_splits(ceil_div(K, 512), kb_total)) * KB;
+      for (int k0 = 0; k0 < K; k0 += chain) {
+        TcGemmArgs c = t;
+        c.A = A + k0; c.B = B + k0; c.K = std::min(chain, K - k0); c.accumulate = k0 > 0;
+        const int rc = launch_tc_gemm(c, s);
         if (rc) return rc;
-        reduce_slabs_kernel<<<grid_for(stride), 256, 0, s>>>(slab, stride, splits, D, stride);
-        KFAC_LAUNCH_CHECK();
-        return KFAC_OK;
       }
-      // no workspace: partial tiles are added with (round-to-nearest) L2 atomics
-      KFAC_CUDA(cudaMemset2DAsync(D, (size_t)ldd * 4, 0, (size_t)N * 4, (size_t)M, s));
-      t.atomic = 1;
-      t.splits = splits;
+      return KFAC_OK;
     }
     return launch_tc_gemm(t, s);
   }
@@ -245,7 +231,7 @@ extern "C" int kfac_inverse_from_eigh(const float* Q, int ldq, const float* d, i
   float* T = (float*)ws;
   scale_cols_kernel<<<grid_for((int64_t)n * ldq), 256, 0, s>>>(Q, ldq, d, n, damping, T);
   KFAC_LAUNCH_CHECK();
-  // inv[i][j] = sum_k T[i][k] Q[j][k]
+  // inv[i][j] = sum_k T[i][k] Q[j][k]; the same bits in every call (for n > 1024 the chains of gemm_tn)
   return gemm_tn(T, ldq, Q, ldq, inv, ld_inv, n, n, n, Epi{}, s);
 }
 

@@ -510,7 +510,7 @@ def test_not_ready_maps_to_runtime_error(lib, dev):
         _cabi.check(lib.kfac_dgda(None, None, 0, 0, 0.1, None, 0, S()))
 
 
-@pytest.mark.parametrize('n', [1, 2, 5, 64, 257])
+@pytest.mark.parametrize('n', [1, 2, 5, 64, 257, 1025, 4608])   # 1025, 4608: several passes of the grid-stride loop
 def test_triu_pack_unpack(lib, dev, n):
     torch.manual_seed(n)
     F = torch.randn(n, n)
