@@ -540,6 +540,36 @@ int kfac_reduce_rows_conv_transpose_input(const void* x, int dtype,
                                           const kfac_conv_transpose_geometry* geom, int append_ones,
                                           float scale, float* out, int ld_out, void* stream);
 
+/* Rows of a recurrent layer's sub-layer (nn.RNN / LSTM / GRU): position (t, b) of a sequence of T
+ * steps, time-major (row t * B + b) or packed (row offsets[t] + b, offsets a DEVICE int[T + 1]
+ * with offsets[0] = 0 and non-increasing batch sizes offsets[t + 1] - offsets[t] <= B, as in a
+ * PackedSequence).  The source row of a position holds `features` elements of dtype `dtype`:
+ *   shift  0: x[row(t, b) * ldx + col0 ...] itself;
+ *   shift +1: the previous hidden state of a forward direction: row (t - 1, b) of x, h0[b * ldh]
+ *             at t = 0;
+ *   shift -1: that of a reverse direction: row (t + 1, b) while sequence b continues there, else
+ *             h0[b * ldh].
+ * With `mul` set, the columns f >= mul_col0 are multiplied by mul[row(t, b) * ldm + f - mul_col0]
+ * (same dtype): the GRU's hidden-gate gradient [dr, dz, r * dn] from the input-gate gradient and r. */
+typedef struct kfac_sequence_rows {
+  const void* x;   int64_t ldx;  int col0;
+  const void* h0;  int64_t ldh;  int shift;
+  const void* mul; int64_t ldm;  int mul_col0;
+  int T; int B; const int* offsets;   /* offsets NULL: T x B time-major positions */
+} kfac_sequence_rows;
+/* One row per position, in row(t, b) order, like kfac_rows_linear (out: rows x ld_out fp32, the
+ * values times scale / *loss_scale, the ones column scale, zeros up to ld_out).  Rows: T * B, or
+ * offsets[T]. */
+int kfac_rows_sequence(const kfac_sequence_rows* src, int dtype, int features, int append_ones,
+                       float scale, const float* loss_scale, float* out, int ld_out, void* stream);
+/* K-FAC-reduce over sequences: row b (b < B) is the sum of sequence b's R_b rows times
+ * scale * R_b^-power / *loss_scale (power 1: the mean, A side; 0.5: G side), the ones column R_b
+ * times that factor.  R_b is T, or the number of steps whose batch size exceeds b.  The sums keep
+ * the order of kfac_reduce_rows_linear. */
+int kfac_reduce_rows_sequence(const kfac_sequence_rows* src, int dtype, int features,
+                              int append_ones, float scale, float power,
+                              const float* loss_scale, float* out, int ld_out, void* stream);
+
 /* S_batch of every item, for all items together; no floating-point atomics, the same bits on
  * every run.  Launches: one grouped wgmma launch of the projections (x^2 epilogue), the K = N
  * product as one grouped launch, and the fixed-order sum of its split partials.  Extra launches:

@@ -83,6 +83,14 @@ class GradItem(C.Structure):
                 ('grad_dtype', c_int), ('g', c_int), ('a', c_int), ('ldp', c_int), ('wgrad_taps', c_int)]
 
 
+class SequenceRows(C.Structure):
+    """kfac_sequence_rows: the source rows of a recurrent sub-layer's positions (time-major or packed)."""
+    _fields_ = [('x', c_void_p), ('ldx', c_int64), ('col0', c_int),
+                ('h0', c_void_p), ('ldh', c_int64), ('shift', c_int),
+                ('mul', c_void_p), ('ldm', c_int64), ('mul_col0', c_int),
+                ('T', c_int), ('B', c_int), ('offsets', c_void_p)]
+
+
 class EkfacStatItem(C.Structure):
     _fields_ = [('X', c_void_p), ('G', c_void_p), ('qaT', c_void_p), ('qgT', c_void_p), ('S_batch', c_void_p),
                 ('N', c_int64), ('a', c_int), ('g', c_int),
@@ -173,6 +181,10 @@ SIGNATURES = {
                                                       c_float, c_void_p, c_int, c_void_p]),
     'kfac_reduce_rows_conv2d_gradout': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                                 c_void_p, c_int, c_void_p]),
+    'kfac_rows_sequence': (c_int, [C.POINTER(SequenceRows), c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
+                                   c_void_p]),
+    'kfac_reduce_rows_sequence': (c_int, [C.POINTER(SequenceRows), c_int, c_int, c_int, c_float, c_float, c_void_p,
+                                          c_void_p, c_int, c_void_p]),
     'kfac_ekfac_statistics_workspace_bytes': (c_size_t, [C.POINTER(EkfacStatItem), c_int]),
     'kfac_ekfac_statistics': (c_int, [C.POINTER(EkfacStatItem), c_int, c_void_p, c_size_t, c_void_p]),
     'kfac_ekfac_update_workspace_bytes': (c_size_t, [c_int]),

@@ -67,7 +67,7 @@ from kfac_b200 import _cabi
 from kfac_b200.assignment import WorkAssignment
 from kfac_b200.distributed import ArenaCommunicator, get_rank
 from kfac_b200.enums import ComputeMethod
-from kfac_b200.layers import AttentionProjectionHelper, KFACLayer, cast_for_factor
+from kfac_b200.layers import AttentionProjectionHelper, KFACLayer, RecurrentSubLayerHelper, cast_for_factor
 
 logger = logging.getLogger(__name__)
 
@@ -406,11 +406,17 @@ class BaseKFACPreconditioner:
         # attention projections (precondition_attention): attention module -> {'q', 'k', 'v', 'o'} -> the helper that
         # keys the projection's layer; their statistics arrive through taps inside the attention's forward
         self._attention_taps: dict[torch.nn.Module, dict[str, AttentionProjectionHelper]] = {}
+        # recurrent sub-layers (precondition_recurrent): RNN / LSTM / GRU module -> {'ih_l0', 'hh_l0_reverse', ...} ->
+        # the helper that keys the sub-layer's layer; their statistics arrive through taps inside the module's forward
+        self._recurrent_taps: dict[torch.nn.Module, dict[str, RecurrentSubLayerHelper]] = {}
         for module in self._norm_layers:
             module.register_forward_hook(self._hook_norm_output)
         for module, (_, layer) in self._layers.items():
             if isinstance(module, AttentionProjectionHelper):
                 self._attention_taps.setdefault(module.attn, {})[module.which[0]] = module
+                continue
+            if isinstance(module, RecurrentSubLayerHelper):
+                self._recurrent_taps.setdefault(module.rnn, {})[module.suffix] = module
                 continue
             if layer.module.call_kwargs:
                 module.register_forward_pre_hook(self._save_input_with_kwargs, with_kwargs=True)
@@ -751,6 +757,22 @@ class BaseKFACPreconditioner:
 
     def _attention_grad_output(self, key: AttentionProjectionHelper, g: torch.Tensor) -> None:
         """G tap of an attention projection: g is the gradient of its output, (L, B, E), possibly a column block."""
+        self._accumulate_grad_output(*self._layers[key], g)
+
+    def _active_recurrent_taps(self, module: torch.nn.Module) -> dict[str, RecurrentSubLayerHelper] | None:
+        """The registered sub-layers of a recurrent module at a factor step (its forward taps them), else None."""
+        if self.steps % self.factor_update_steps != 0:
+            return None
+        return self._recurrent_taps.get(module)
+
+    def _recurrent_input(self, key: RecurrentSubLayerHelper, x: torch.Tensor, tap) -> None:
+        """A tap of a recurrent sub-layer: x is the layer input (ih) or output (hh), `tap` where its rows lie."""
+        key.tap_a = tap
+        self._accumulate_input(*self._layers[key], x)
+
+    def _recurrent_grad_output(self, key: RecurrentSubLayerHelper, g: torch.Tensor, tap) -> None:
+        """G tap of a recurrent sub-layer: g is the gradient of the input projection z_x, `tap` where its rows lie."""
+        key.tap_g = tap
         self._accumulate_grad_output(*self._layers[key], g)
 
     @torch.no_grad()

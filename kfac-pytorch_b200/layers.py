@@ -18,6 +18,7 @@ import torch
 
 from kfac_b200 import _cabi
 from kfac_b200.attention import KFACMultiheadAttention
+from kfac_b200.recurrent import SWAPPED as RECURRENT_SWAPPED
 
 
 class ModuleHelper:
@@ -845,67 +846,10 @@ def _strided_rows(t: torch.Tensor, ordered: bool) -> tuple[torch.Tensor, int]:
     return t.contiguous().view(-1, feat), feat
 
 
-class AttentionProjectionHelper(LinearModuleHelper):
-    """One projection of a `torch.nn.MultiheadAttention` (an extension beyond the reference, opt-in through
-    `precondition_attention`), preconditioned as the `torch.nn.Linear` it is mathematically:
-
-        'q'    Linear(E, E) on query        rows [0, E) of in_proj_weight / in_proj_bias, or q_proj_weight
-        'k'    Linear(kdim, E) on key       rows [E, 2E), or k_proj_weight
-        'v'    Linear(vdim, E) on value     rows [2E, 3E), or v_proj_weight
-        'out'  Linear(E, E) on the concatenated head outputs: out_proj.weight / out_proj.bias
-
-    The gradients are row-slice views, contiguous like a Linear layer's, so the write-back runs in place.  The
-    statistics come from taps inside `kfac_b200.attention.KFACMultiheadAttention`, which see (L, B, features) tensors
-    in the sequence-first layout of torch's attention path: views of the batch-first input, column blocks of a packed
-    projection's gradient.  They are read in place through the strided native entry points.  Under K-FAC-reduce the
-    example dimension is the attention's batch dimension B (dimension 1 here); an unbatched call is one example."""
-
-    def __init__(self, attn: torch.nn.MultiheadAttention, which: str, reduce: bool = False):
-        super().__init__(attn, reduce=reduce)
-        self.attn = attn
-        self.which = which
-        E = attn.embed_dim
-        if which == 'out':
-            self.weight, self.bias, self.rows = attn.out_proj.weight, attn.out_proj.bias, None
-        else:
-            i = 'qkv'.index(which)
-            self.rows = (i * E, (i + 1) * E)
-            self.weight = attn.in_proj_weight if attn._qkv_same_embed_dim else getattr(attn, f'{which}_proj_weight')
-            self.bias = attn.in_proj_bias
-
-    def __repr__(self) -> str:
-        return f'{self.__class__.__name__}({self.which}, in_features={self.in_features}, out_features={self.attn.embed_dim})'
-
-    def parameters(self):
-        """The projection's own parameters (the whole packed in_proj_weight / in_proj_bias for q, k and v)."""
-        return iter([p for p in (self.weight, self.bias) if p is not None])
-
-    @property
-    def in_features(self) -> int:
-        return {'q': self.attn.embed_dim, 'k': self.attn.kdim, 'v': self.attn.vdim, 'out': self.attn.embed_dim}[self.which]
-
-    def has_bias(self) -> bool:
-        return self.bias is not None
-
-    @property
-    def a_factor_shape(self):
-        d = self.in_features + int(self.has_bias())
-        return (d, d)
-
-    @property
-    def g_factor_shape(self):
-        return (self.attn.embed_dim, self.attn.embed_dim)
-
-    def _slice(self, t: torch.Tensor | None, weight: bool) -> torch.Tensor | None:
-        if t is None or self.rows is None or (weight and not self.attn._qkv_same_embed_dim):
-            return t
-        return t[self.rows[0]:self.rows[1]]
-
-    def get_weight_grad(self):
-        return self._slice(self.weight.grad, True)
-
-    def get_bias_grad(self):
-        return self._slice(self.bias.grad, False)
+class SequenceFirstLinearHelper(LinearModuleHelper):
+    """A Linear layer keyed by an object that is not its own module, whose taps see (L, B, features) tensors in a
+    sequence-first layout, read in place through the strided native entry points.  Under K-FAC-reduce the example
+    dimension is B (dimension 1); an unbatched call is one example."""
 
     def get_grad(self):
         g = self.get_weight_grad()
@@ -981,6 +925,212 @@ class AttentionProjectionHelper(LinearModuleHelper):
                                                           _cabi.stream_ptr()), 'kfac_rows_linear_strided')
 
 
+
+class AttentionProjectionHelper(SequenceFirstLinearHelper):
+    """One projection of a `torch.nn.MultiheadAttention` (an extension beyond the reference, opt-in through
+    `precondition_attention`), preconditioned as the `torch.nn.Linear` it is mathematically:
+
+        'q'    Linear(E, E) on query        rows [0, E) of in_proj_weight / in_proj_bias, or q_proj_weight
+        'k'    Linear(kdim, E) on key       rows [E, 2E), or k_proj_weight
+        'v'    Linear(vdim, E) on value     rows [2E, 3E), or v_proj_weight
+        'out'  Linear(E, E) on the concatenated head outputs: out_proj.weight / out_proj.bias
+
+    The gradients are row-slice views, contiguous like a Linear layer's, so the write-back runs in place.  The
+    statistics come from taps inside `kfac_b200.attention.KFACMultiheadAttention`, which see (L, B, features) tensors
+    in the sequence-first layout of torch's attention path: views of the batch-first input, column blocks of a packed
+    projection's gradient.  They are read in place through the strided native entry points.  Under K-FAC-reduce the
+    example dimension is the attention's batch dimension B (dimension 1 here); an unbatched call is one example."""
+
+    def __init__(self, attn: torch.nn.MultiheadAttention, which: str, reduce: bool = False):
+        super().__init__(attn, reduce=reduce)
+        self.attn = attn
+        self.which = which
+        E = attn.embed_dim
+        if which == 'out':
+            self.weight, self.bias, self.rows = attn.out_proj.weight, attn.out_proj.bias, None
+        else:
+            i = 'qkv'.index(which)
+            self.rows = (i * E, (i + 1) * E)
+            self.weight = attn.in_proj_weight if attn._qkv_same_embed_dim else getattr(attn, f'{which}_proj_weight')
+            self.bias = attn.in_proj_bias
+
+    def __repr__(self) -> str:
+        return f'{self.__class__.__name__}({self.which}, in_features={self.in_features}, out_features={self.attn.embed_dim})'
+
+    def parameters(self):
+        """The projection's own parameters (the whole packed in_proj_weight / in_proj_bias for q, k and v)."""
+        return iter([p for p in (self.weight, self.bias) if p is not None])
+
+    @property
+    def in_features(self) -> int:
+        return {'q': self.attn.embed_dim, 'k': self.attn.kdim, 'v': self.attn.vdim, 'out': self.attn.embed_dim}[self.which]
+
+    def has_bias(self) -> bool:
+        return self.bias is not None
+
+    @property
+    def a_factor_shape(self):
+        d = self.in_features + int(self.has_bias())
+        return (d, d)
+
+    @property
+    def g_factor_shape(self):
+        return (self.attn.embed_dim, self.attn.embed_dim)
+
+    def _slice(self, t: torch.Tensor | None, weight: bool) -> torch.Tensor | None:
+        if t is None or self.rows is None or (weight and not self.attn._qkv_same_embed_dim):
+            return t
+        return t[self.rows[0]:self.rows[1]]
+
+    def get_weight_grad(self):
+        return self._slice(self.weight.grad, True)
+
+    def get_bias_grad(self):
+        return self._slice(self.bias.grad, False)
+
+
+class RecurrentSubLayerHelper(SequenceFirstLinearHelper):
+    """One sub-layer of a `torch.nn.RNN`, `LSTM` or `GRU` (an extension beyond the reference, opt-in through
+    `precondition_recurrent`), preconditioned as the `torch.nn.Linear` it is mathematically, time steps being the
+    positions of a weight-shared layer:
+
+        'ih_l{k}{sfx}'   weight_ih_l{k}{sfx}, bias_ih_l{k}{sfx}   A: the layer input x_t    G: d(W_ih x_t + b_ih)
+        'hh_l{k}{sfx}'   weight_hh_l{k}{sfx}, bias_hh_l{k}{sfx}   A: h_{t-1} (h0 first)     G: d(W_hh h_{t-1} + b_hh)
+
+    For RNN and LSTM the two G rows of a position are equal; for GRU the hidden one is [dr, dz, r * dn].  The two biases
+    have the same gradient (RNN, LSTM) and each is preconditioned by its own layer with its own ones column, as the
+    two-Linear twin of the module does.
+
+    The statistics come from taps inside `kfac_b200.recurrent`, which see time-major (T, B, features) tensors or the
+    (N, features) data of a PackedSequence; each statistics call is preceded by the `SequenceTap` of its rows
+    (`tap_a` / `tap_g`).  Unpacked input rows and the RNN / LSTM hidden G rows take the sequence-first Linear path.
+    The hidden-state rows, the GRU hidden G rows and the per-sequence K-FAC-reduce rows of packed input go through
+    `kfac_rows_sequence` / `kfac_reduce_rows_sequence` into scratch rows and the existing statistics call.  Under
+    K-FAC-reduce the example dimension is the module's batch dimension, with R_b = T or the length of sequence b."""
+
+    def __init__(self, rnn: torch.nn.Module, layer: int, direction: int, side: str, reduce: bool = False):
+        super().__init__(rnn, reduce=reduce)
+        self.rnn = rnn
+        self.side = side
+        self.suffix = f'{side}_l{layer}' + ('_reverse' if direction else '')
+        self.tap_a = self.tap_g = None
+
+    def __repr__(self) -> str:
+        return f'{self.__class__.__name__}({self.suffix}, {tuple(self.weight.shape)}, bias={self.has_bias()})'
+
+    @property
+    def weight(self) -> torch.Tensor:
+        return getattr(self.rnn, 'weight_' + self.suffix)
+
+    @property
+    def bias(self) -> torch.Tensor | None:
+        return getattr(self.rnn, 'bias_' + self.suffix) if self.rnn.bias else None
+
+    def parameters(self):
+        return iter([p for p in (self.weight, self.bias) if p is not None])
+
+    def has_bias(self) -> bool:
+        return bool(self.rnn.bias)
+
+    @property
+    def a_factor_shape(self):
+        d = self.weight.size(1) + int(self.has_bias())
+        return (d, d)
+
+    @property
+    def g_factor_shape(self):
+        d = self.weight.size(0)
+        return (d, d)
+
+    def get_weight_grad(self):
+        return self.weight.grad
+
+    def get_bias_grad(self):
+        return self.bias.grad
+
+    # ---- the rows of one tap
+    def _reduced(self, tap) -> bool:
+        return self.reduce and tap.T > 1
+
+    def _native(self, tap) -> bool:
+        """Whether the rows go through the sequence writers (else the sequence-first Linear path reads them)."""
+        return tap.h0 is not None or tap.mul is not None or (tap.offsets is not None and self._reduced(tap))
+
+    @staticmethod
+    def _first(t: torch.Tensor, tap) -> torch.Tensor:
+        """A packed (N, features) tap as the one-position (1, N, features) sequence-first tensor of its rows."""
+        return t.unsqueeze(0) if tap.offsets is not None else t
+
+    def _sequence_call(self, t, tap, side, scale, loss_scale, out_ptr, ld, reduced):
+        t = t if t.is_contiguous() else t.contiguous()
+        feat = (self.a_factor_shape[0] - int(self.has_bias())) if side == 'a' else self.g_factor_shape[0]
+
+        def like(u):         # h0 and r in the dtype of the rows (factor_dtype casts those)
+            return None if u is None else u.to(t.dtype).contiguous()
+        h0, mul = like(tap.h0), like(tap.mul)
+        src = _cabi.SequenceRows(t.data_ptr(), t.size(-1), tap.col0,
+                                 h0.data_ptr() if h0 is not None else None, h0.size(-1) if h0 is not None else 0,
+                                 tap.shift, mul.data_ptr() if mul is not None else None,
+                                 mul.size(-1) if mul is not None else 0, tap.mul_col0, tap.T, tap.B,
+                                 tap.offsets.data_ptr() if tap.offsets is not None else None)
+        ones = int(self.has_bias()) if side == 'a' else 0
+        lib = _cabi.load()
+        if reduced:
+            _cabi.check(lib.kfac_reduce_rows_sequence(C.byref(src), _dtype_code(t), feat, ones, scale,
+                                                      1.0 if side == 'a' else 0.5, loss_scale, out_ptr, ld,
+                                                      _cabi.stream_ptr()), 'kfac_reduce_rows_sequence')
+        else:
+            _cabi.check(lib.kfac_rows_sequence(C.byref(src), _dtype_code(t), feat, ones, scale, loss_scale, out_ptr,
+                                               ld, _cabi.stream_ptr()), 'kfac_rows_sequence')
+
+    def _accumulate_tap(self, t, tap, side, acc, grad_scale, scratch):
+        reduced = self._reduced(tap)
+        n = tap.B if reduced else t.numel() // t.size(-1)
+        if n == 0:
+            return
+        d = (self.a_factor_shape if side == 'a' else self.g_factor_shape)[0]
+        _reduced_factor(lambda p, ld: self._sequence_call(t, tap, side, 1.0, None, p, ld, reduced), n, d,
+                        1.0 / (n * grad_scale * grad_scale), acc, scratch, t.device)
+
+    def accumulate_a(self, x, acc, scratch):
+        _cabi.require_device(x)
+        x, tap = x.detach(), self.tap_a
+        if self._native(tap):
+            return self._accumulate_tap(x, tap, 'a', acc, 1.0, scratch)
+        super().accumulate_a(self._first(x, tap), acc, scratch)
+
+    def accumulate_g(self, g, acc, grad_scale, scratch=None):
+        _cabi.require_device(g)
+        g, tap = g.detach(), self.tap_g
+        if self._native(tap):
+            return self._accumulate_tap(g, tap, 'g', acc, grad_scale, scratch)
+        super().accumulate_g(self._first(g, tap), acc, grad_scale, scratch)
+
+    def num_rows_a(self, x):
+        tap = self.tap_a
+        return tap.B if self._reduced(tap) else x.numel() // x.size(-1)
+
+    def num_rows_g(self, g):
+        tap = self.tap_g
+        return tap.B if self._reduced(tap) else g.numel() // g.size(-1)
+
+    def write_rows_a(self, x, out):
+        tap = self.tap_a
+        if self._native(tap):
+            _cabi.require_device(x)
+            return self._sequence_call(x.detach(), tap, 'a', 1.0, None, out.data_ptr(),
+                                       _cabi.ld4(self.a_factor_shape[0]), self._reduced(tap))
+        self._write_rows(self._first(x, tap), out, 'a', 1.0, None)
+
+    def write_rows_g(self, g, out, grad_scale, loss_scale):
+        tap = self.tap_g
+        if self._native(tap):
+            _cabi.require_device(g)
+            return self._sequence_call(g.detach(), tap, 'g', 1.0 / grad_scale, loss_scale, out.data_ptr(),
+                                       _cabi.ld4(self.g_factor_shape[0]), self._reduced(tap))
+        self._write_rows(self._first(g, tap), out, 'g', 1.0 / grad_scale, loss_scale)
+
+
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
 CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
 CONV_ND_TYPES: tuple[type, ...] = (torch.nn.Conv1d, torch.nn.Conv3d)
@@ -991,6 +1141,8 @@ EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
 NORM_TYPES: tuple[type, ...] = (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d, torch.nn.LayerNorm, torch.nn.RMSNorm)
 GROUP_NORM_TYPES: tuple[type, ...] = (torch.nn.GroupNorm, torch.nn.InstanceNorm1d, torch.nn.InstanceNorm2d,
                                       torch.nn.InstanceNorm3d)
+# registered through their own keyword (precondition_recurrent), as two Linear layers per layer and direction
+RECURRENT_TYPES: tuple[type, ...] = (torch.nn.RNN, torch.nn.LSTM, torch.nn.GRU)
 
 
 def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
@@ -1211,7 +1363,7 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
                      diagonal_g_layers: list[str] | None = None, precondition_norms: bool = False,
                      kfac_approx: str = 'expand', precondition_attention: bool = False,
                      precondition_conv_nd: bool = False, precondition_conv_transpose: bool = False,
-                     precondition_group_norms: bool = False,
+                     precondition_group_norms: bool = False, precondition_recurrent: bool = False,
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
@@ -1227,7 +1379,10 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     ones whose factors exceed the eigensolver are an error.  precondition_conv_transpose: also register
     torch.nn.ConvTranspose1d, 2d and 3d modules (not in the reference), with the same errors.
     precondition_group_norms: also register GroupNorm and InstanceNorm1d/2d/3d modules with affine parameters (not in
-    the reference; `layer.norm`).  `layer.index` counts the other layers and the normalization layers separately."""
+    the reference; `layer.norm`).  precondition_recurrent: register every torch.nn.RNN, LSTM and GRU as two Linear
+    layers per layer k and direction, `{name}.ih_l{k}{sfx}` and `{name}.hh_l{k}{sfx}`, keyed by their
+    RecurrentSubLayerHelper (not in the reference).  `layer.index` counts the other layers and the normalization layers
+    separately."""
     diagonal_g_layers = diagonal_g_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     counts = [0, 0]
@@ -1240,6 +1395,13 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
                 layer.index = counts[0]
                 counts[0] += 1
                 layers[helper] = (f'{name}.{helper.which}_proj', layer)
+            continue
+        if precondition_recurrent and isinstance(module, RECURRENT_TYPES):
+            for helper in _recurrent_sublayers(name, module, skip_layers, diagonal_g_layers, kfac_approx):
+                layer = KFACLayer(helper, **layer_kwargs)
+                layer.index = counts[0]
+                counts[0] += 1
+                layers[helper] = (f'{name}.{helper.suffix}', layer)
             continue
         if len(list(module.children())) != 0 or id(module) in out_projs:
             continue
@@ -1268,7 +1430,8 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     # projections of one attention share in_proj_weight / in_proj_bias by design)
     owners: dict[int, list[tuple[Any, str]]] = {}
     for key, (name, _) in layers.items():
-        owner = key.attn if isinstance(key, AttentionProjectionHelper) else key
+        owner = (key.attn if isinstance(key, AttentionProjectionHelper) else key.rnn
+                 if isinstance(key, RecurrentSubLayerHelper) else key)
         for p in key.parameters():
             owners.setdefault(id(p), []).append((owner, name))
     for key, (name, _) in layers.items():
@@ -1278,6 +1441,12 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
                 if other is not None:
                     raise ValueError(f'attention projection "{name}" shares a weight with "{other}": two layers '
                                      'would precondition one gradient; add one of them to skip_layers')
+        if isinstance(key, RecurrentSubLayerHelper):
+            for p in key.parameters():
+                other = next((n for o, n in owners[id(p)] if o is not key.rnn), None)
+                if other is not None:
+                    raise ValueError(f'recurrent sub-layer "{name}" shares a weight with "{other}": two layers would '
+                                     'precondition one gradient; add one of them to skip_layers')
     return layers
 
 
@@ -1307,4 +1476,38 @@ def _attention_projections(name: str, module: torch.nn.MultiheadAttention, skip_
             raise ValueError(f'diagonal_g_layers matches the attention projection "{pname}": attention projections '
                              'cannot keep a diagonal G (add it to skip_layers or narrow the pattern)')
         helpers.append(AttentionProjectionHelper(module, which, reduce=kfac_approx == 'reduce'))
+    return helpers
+
+
+def _recurrent_sublayers(name: str, module: torch.nn.Module, skip_layers: list[str], diagonal_g_layers: list[str],
+                         kfac_approx: str) -> list[RecurrentSubLayerHelper]:
+    """The registered sub-layers of one RNN / LSTM / GRU: none when skip_layers matches its name or class or one of its
+    parameters is frozen, else those whose name `{name}.{ih,hh}_l{k}{sfx}` skip_layers does not match."""
+    cls = module.__class__.__name__
+    if any_match(name, skip_layers) or any_match(cls, skip_layers):
+        return []
+    if not all(p.requires_grad for p in module.parameters()):
+        return []
+    if type(module) not in RECURRENT_SWAPPED and type(module) not in RECURRENT_SWAPPED.values():
+        base = module.mode.split('_')[0]
+        raise ValueError(f'precondition_recurrent: "{name}" is a {cls}, a subclass of torch.nn.{base} whose forward '
+                         'cannot be tapped; add it to skip_layers')
+    if getattr(module, 'proj_size', 0) > 0:
+        raise ValueError(f'precondition_recurrent does not support proj_size > 0 (LSTM "{name}"); add it to skip_layers')
+    helpers = []
+    for k in range(module.num_layers):
+        for d in range(2 if module.bidirectional else 1):
+            for side in ('ih', 'hh'):
+                helper = RecurrentSubLayerHelper(module, k, d, side, reduce=kfac_approx == 'reduce')
+                sname = f'{name}.{helper.suffix}'
+                if any_match(sname, skip_layers):
+                    continue
+                if any(any_match(q, diagonal_g_layers) for q in (name, cls, sname)):
+                    raise ValueError(f'diagonal_g_layers matches the recurrent sub-layer "{sname}": recurrent layers '
+                                     'cannot keep a diagonal G (add it to skip_layers or narrow the pattern)')
+                n = max(helper.a_factor_shape[0], helper.g_factor_shape[0])
+                if n > _cabi.KFAC_EIGH_MAX_N:
+                    raise ValueError(f'recurrent sub-layer "{sname}" has a factor of {n} > KFAC_EIGH_MAX_N = '
+                                     f'{_cabi.KFAC_EIGH_MAX_N}; add it to skip_layers')
+                helpers.append(helper)
     return helpers

@@ -17,7 +17,7 @@ from typing import Any, Callable
 import torch
 import torch.distributed as dist
 
-from kfac_b200 import attention
+from kfac_b200 import attention, recurrent
 from kfac_b200.assignment import KAISAAssignment
 from kfac_b200.base_preconditioner import BaseKFACPreconditioner
 from kfac_b200.distributed import ArenaCommunicator, get_rank, get_world_size
@@ -242,6 +242,25 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     `kfac_b200.layers.ConvTransposeModuleHelper`.  Refused with a ValueError naming the layer and `skip_layers`:
     `groups != 1`, an A dimension C_in * K (+ bias) or `out_channels` above `KFAC_EIGH_MAX_N` (8192), more than 2048
     taps under 'reduce', and a `diagonal_g_layers` match.
+
+    `precondition_recurrent=True` registers every `torch.nn.RNN` (tanh and relu), `torch.nn.LSTM` and `torch.nn.GRU`
+    whose parameters all require grad, and which `skip_layers` does not match by name or class, as two K-FAC layers per
+    layer k and direction (sfx '' or '_reverse'): `{name}.ih_l{k}{sfx}` (`weight_ih` / `bias_ih`; A: the layer input,
+    G: the gradient of the input projection) and `{name}.hh_l{k}{sfx}` (`weight_hh` / `bias_hh`; A: the previous hidden
+    state h_{t-1} of that direction, h0 at the first position, zeros when `hx` is not passed; G: the gradient of the
+    hidden projection, equal to the input one for RNN and LSTM and [dr, dz, r * dn] for GRU).  Time steps are the
+    positions of a weight-shared Linear layer (the "independent time steps" model of Martens, Ba & Johnson, 2018):
+    N = T * B positions, or the sum of the lengths of a PackedSequence, with A and G scaled by 1/N; under
+    `kfac_approx='reduce'` each sequence is one example (R_b = T or its length).  For RNN and LSTM, `bias_ih` and
+    `bias_hh` have the same gradient; each is preconditioned by its own layer with its own ones column, as in the
+    two-`nn.Linear` twin of the module.  Placement, collectives, `state_dict()` and `memory_usage()` are those of that
+    twin.  A `skip_layers` pattern matching one sub-layer name leaves that sub-layer's gradients untouched.  To see the
+    projections, the constructor sets the class of each registered module to `kfac_b200.recurrent.KFACRNN`, `KFACLSTM`
+    or `KFACGRU`, subclasses that add no state and override only `forward`: at the factor steps in training it runs a
+    restatement of torch's forward with a time loop (its inter-layer dropout mask is drawn differently from cuDNN's),
+    and the stock forward (cuDNN) otherwise.  Refused with a ValueError naming the layer and `skip_layers`:
+    `proj_size > 0`, a factor above `KFAC_EIGH_MAX_N` (8192; an LSTM with H > 2048, a GRU with H > 2730), a
+    `diagonal_g_layers` match, a weight shared with another registered module, and subclasses.
     """
 
     def __init__(
@@ -277,6 +296,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         precondition_conv_nd: bool = False,
         precondition_conv_transpose: bool = False,
         precondition_group_norms: bool = False,
+        precondition_recurrent: bool = False,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -364,6 +384,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             precondition_attention=precondition_attention, precondition_conv_nd=precondition_conv_nd,
             precondition_conv_transpose=precondition_conv_transpose,
             precondition_group_norms=precondition_group_norms,
+            precondition_recurrent=precondition_recurrent,
             method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
@@ -406,6 +427,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'precondition_conv_nd': precondition_conv_nd,
             'precondition_conv_transpose': precondition_conv_transpose,
             'precondition_group_norms': precondition_group_norms,
+            'precondition_recurrent': precondition_recurrent,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
@@ -415,3 +437,5 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             defaults=defaults, tdc=self.tdc, loglevel=loglevel)
         for module in self._attention_taps:
             attention.bind(module, self)
+        for module in self._recurrent_taps:
+            recurrent.bind(module, self)
