@@ -390,8 +390,13 @@ typedef struct kfac_precond_item {
   int ldp;
   /* fused compute + broadcast (replaces KFACBaseLayer.broadcast_grad, layers/base.py:224-252):
    * HOST array of n_peers (<= 7) device pointers -- the same P entry inside the peer ranks'
-   * P arenas, mapped with kfac_peer_open().  The epilogue of the last GEMM stores every tile
-   * to P and to all peers (P2P over NVLink).  n_peers = 0: local only. */
+   * P arenas, mapped with kfac_peer_open().  The last GEMM stores P to all peers too (P2P over
+   * NVLink): from its tile epilogue, or, where its reduction is split (K > 1024), from the pass
+   * that adds the partials.  P does not depend on n_peers: the same bits for 0 to 7 peers, and
+   * columns [0, n) of every peer entry equal P (padding columns hold P's zeros or are left
+   * as they were).  Every peer pointer must be the same offset into an arena with the same
+   * alignment as the local one (the tiles are stored as float2 where P's row is 8-byte
+   * aligned).  n_peers = 0: local only. */
   float* const* peer_P;
   int n_peers;
   int kind; /* kfac_item_kind; 0 (dense) for the positional initialisers written before it */

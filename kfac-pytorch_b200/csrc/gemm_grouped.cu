@@ -122,9 +122,14 @@ struct GroupedPolicy {
   }
 };
 
-// D[idx] = sum_sp slab[sp * stride + idx] over a list of split problems, one launch, fixed order
+// D[idx] = sum_sp slab[sp * stride + idx] over a list of split problems, one launch, fixed order.  The peers of a
+// split problem (peers[i] for probs[i]) get the final sums here, its tiles being partials: every column of D,
+// including the zero padding.  A launch without peers (PEERS = false) does not read the peer table.
 struct RProb { const float* slab; float* D; int64_t stride; int splits; int N; int ldd; long long elem0; };
-__global__ void __launch_bounds__(256) grouped_reduce_kernel(const RProb* probs, int count, long long total) {
+struct RPeers { float* peerD[7]; int npeer; };
+template <bool PEERS>
+__global__ void __launch_bounds__(256) grouped_reduce_kernel(const RProb* probs, const RPeers* peers, int count,
+                                                             long long total) {
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     int lo = 0, hi = count - 1;
     while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (probs[mid].elem0 <= e) lo = mid; else hi = mid - 1; }
@@ -136,6 +141,10 @@ __global__ void __launch_bounds__(256) grouped_reduce_kernel(const RProb* probs,
       for (int sp = 1; sp < p.splits; ++sp) t += p.slab[(int64_t)sp * p.stride + idx];
     }
     p.D[idx] = t;
+    if (PEERS) {
+      const RPeers& r = peers[lo];
+      for (int q = 0; q < r.npeer; ++q) r.peerD[q][idx] = t;
+    }
   }
 }
 
@@ -150,7 +159,8 @@ bool grouped_gemm_tc_ok(const GroupedGemm& g) {
 }
 
 size_t grouped_gemm_ws_bytes(int count) {
-  return align_up(sizeof(GProb) * (size_t)std::max(1, count), 256) + align_up(sizeof(RProb) * (size_t)std::max(1, count), 256);
+  const size_t n = (size_t)std::max(1, count);
+  return align_up(sizeof(GProb) * n, 256) + align_up(sizeof(RProb) * n, 256) + align_up(sizeof(RPeers) * n, 256);
 }
 
 int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws_bytes, cudaStream_t s) {
@@ -169,6 +179,8 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
   // rejected call leaves all outputs untouched
   std::vector<GProb> tab;
   std::vector<RProb> red;
+  std::vector<RPeers> red_peers;
+  bool any_peers = false;
   std::vector<int> simt;
   long long red_total = 0;
   int work = 0;
@@ -176,7 +188,8 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
     const GroupedGemm& g = probs[i];
     if (g.M <= 0 || g.N <= 0 || g.K <= 0) continue;
     const int splits = std::max(1, g.splits);
-    if (splits > 1 && ((!g.slab && g.mode != 2) || g.epi != EPI_NONE || g.npeer > 0 || g.mode == 1)) {
+    if (g.npeer < 0 || g.npeer > 7) { set_error("grouped gemm: at most 7 peers"); return KFAC_ERR_BAD_ARG; }
+    if (splits > 1 && ((!g.slab && g.mode != 2) || g.epi != EPI_NONE || g.mode == 1)) {
       set_error("grouped gemm: split-K needs a slab (or atomic mode) and the plain epilogue");
       return KFAC_ERR_BAD_ARG;
     }
@@ -192,8 +205,6 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
     if ((rc = make_tmap_3d(&p.tmB, g.B, (uint64_t)g.K, (uint64_t)g.N, 1, (uint64_t)g.ldb * 4, (uint64_t)g.ldb * 4 * g.N, GBM))) return rc;
     p.M = g.M; p.N = g.N; p.K = g.K; p.ldd = g.ldd; p.alpha = g.alpha;
     p.epi = g.epi; p.E = g.E; p.lde = g.lde; p.dg = g.dg; p.da = g.da; p.damping = g.damping;
-    p.npeer = g.npeer;
-    for (int q = 0; q < g.npeer && q < 7; ++q) p.peerD[q] = g.peerD[q];
     p.tiles_n = ceil_div(g.N, GBN);
     const int tiles = ceil_div(g.M, GBM) * p.tiles_n;
     p.kb_total = ceil_div(g.K, GBK);
@@ -203,11 +214,18 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
     if (p.splits > 1 && g.mode == 2) {
       p.D = g.D; p.slab_stride = 0;
     } else if (p.splits > 1) {
+      // the tiles are partials: the peers get the final sums from the reduce pass, not from the epilogue
       p.D = g.slab; p.slab_stride = g.slab_stride;
       red.push_back(RProb{g.slab, g.D, g.slab_stride, p.splits, g.N, (int)g.ldd, red_total});
+      RPeers r{{}, g.npeer};
+      for (int q = 0; q < g.npeer; ++q) r.peerD[q] = g.peerD[q];
+      red_peers.push_back(r);
+      any_peers = any_peers || g.npeer > 0;
       red_total += (long long)g.M * g.ldd;
     } else {
       p.D = g.D; p.slab_stride = 0;
+      p.npeer = g.npeer;
+      for (int q = 0; q < g.npeer; ++q) p.peerD[q] = g.peerD[q];
     }
     p.work0 = work;
     work += tiles * p.splits;
@@ -231,6 +249,7 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
   if (tab.empty()) return KFAC_OK;
   GProb* d_tab = (GProb*)ws;
   RProb* d_red = (RProb*)((char*)ws + align_up(sizeof(GProb) * (size_t)std::max(1, count), 256));
+  RPeers* d_red_peers = (RPeers*)((char*)d_red + align_up(sizeof(RProb) * (size_t)std::max(1, count), 256));
   KFAC_CUDA(cudaMemcpyAsync(d_tab, tab.data(), sizeof(GProb) * tab.size(), cudaMemcpyHostToDevice, s));
   GroupedParams gp{d_tab, (int)tab.size()};
   const int grid = std::min(work, tc_num_sms());
@@ -239,7 +258,12 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
   if (!red.empty()) {
     KFAC_CUDA(cudaMemcpyAsync(d_red, red.data(), sizeof(RProb) * red.size(), cudaMemcpyHostToDevice, s));
     const int blocks = (int)std::min<long long>((red_total + 255) / 256, (long long)tc_num_sms() * 8);
-    grouped_reduce_kernel<<<blocks, 256, 0, s>>>(d_red, (int)red.size(), red_total);
+    if (any_peers) {
+      KFAC_CUDA(cudaMemcpyAsync(d_red_peers, red_peers.data(), sizeof(RPeers) * red_peers.size(), cudaMemcpyHostToDevice, s));
+      grouped_reduce_kernel<true><<<blocks, 256, 0, s>>>(d_red, d_red_peers, (int)red.size(), red_total);
+    } else {
+      grouped_reduce_kernel<false><<<blocks, 256, 0, s>>>(d_red, nullptr, (int)red.size(), red_total);
+    }
     KFAC_LAUNCH_CHECK();
   }
   return KFAC_OK;

@@ -11,8 +11,9 @@ struct GroupedGemm {
   int M, N, K;
   float alpha;
   int epi; const float* E; int64_t lde; const float* dg; const float* da; float damping;   // GemmEpilogue
-  float* peerD[7]; int npeer;      // fused broadcast: tiles are also stored into these peer copies of D
-  int splits;                      // > 1: split-K -- deterministic through `slab` (plain epilogue, no peers), or mode 2
+  float* peerD[7]; int npeer;      // fused broadcast (mode 0, npeer <= 7): D is also stored into these peer copies, by
+                                   // the tile epilogue, or by the reduce pass of a slab split (the same bits as D)
+  int splits;                      // > 1: split-K -- deterministic through `slab` (plain epilogue), or mode 2
   float* slab; int64_t slab_stride;
   int mode;                        // 0: D = ..., 1: D += ... (read-modify-write, splits == 1), 2: atomicAdd into D (caller zeroes D)
   const int* krange;               // optional (mode 2 only): DEVICE pointer to {first, end} k-block (32 columns of K) the product

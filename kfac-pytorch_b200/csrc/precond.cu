@@ -147,34 +147,17 @@ static inline int grid_for(int64_t total) {
 struct Epi { int kind = EPI_NONE; const float* E = nullptr; int64_t lde = 0;
              const float* dg = nullptr; const float* da = nullptr; float damping = 0.f; };
 
-// row-major (rows x ld) copy of D into the peers' buffers (layers that did not go through
-// the tensor-core epilogue)
-__global__ void peer_scatter_kernel(const float* D, int64_t total, float* p0, float* p1, float* p2, float* p3,
-                                    float* p4, float* p5, float* p6, int npeer) {
-  float* peers[7] = {p0, p1, p2, p3, p4, p5, p6};
-  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (int64_t)gridDim.x * blockDim.x) {
-    const float v = D[idx];
-    for (int q = 0; q < npeer; ++q) peers[q][idx] = v;
-  }
-}
-
 // D (M x N, ldd) = epi(A B^T), A (M x K, lda), B (N x K, ldb): tensor-core engine for
 // aligned operands with at least one full tile worth of work, SIMT engine otherwise.
 // Deterministic: no floating-point atomics on any path.
 int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M, int N,
-            int K, const Epi& e, cudaStream_t s, float* const* peers = nullptr, int npeer = 0) {
+            int K, const Epi& e, cudaStream_t s) {
   TcGemmArgs t{};
   t.npeer = 0;
   t.A = A; t.lda = lda; t.B = B; t.ldb = ldb; t.D = D; t.ldd = ldd; t.M = M; t.N = N; t.K = K;
   t.kbatch = 1; t.alpha = 1.f; t.splits = 1;
   t.epi = e.kind; t.E = e.E; t.lde = e.lde; t.dg = e.dg; t.da = e.da; t.damping = e.damping;
   if (M >= 64 && N >= 64 && K >= 32 && tc_gemm_supported(t)) {
-    if (npeer > 0) {   // fused broadcast: plain-store epilogue, no split-K
-      t.npeer = npeer;
-      for (int q = 0; q < npeer; ++q) t.peerD[q] = peers[q];
-      return launch_tc_gemm(t, s);
-    }
     if (e.kind == EPI_NONE && K > 1024) {
       // long reductions run as chains of <= 512, split the way the engine splits k-blocks for ceil(K / 512)
       // splits: the tensor-core accumulator truncates, so short chains keep the 3xTF32 result at fp32 accuracy.
@@ -198,14 +181,7 @@ int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, 
   g.C = D; g.ldc = ldd; g.M = M; g.N = N; g.K = K; g.batch = 1; g.splitk = 1;
   g.alpha = 1.f; g.beta = 0.f;
   g.epi = e.kind; g.E = e.E; g.lde = e.lde; g.dg = e.dg; g.da = e.da; g.damping = e.damping;
-  const int rc = launch_gemm(g, s);
-  if (rc || npeer == 0) return rc;
-  float* pp[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  for (int q = 0; q < npeer; ++q) pp[q] = peers[q];
-  const int64_t total = (int64_t)M * ldd;
-  peer_scatter_kernel<<<grid_for(total), 256, 0, s>>>(D, total, pp[0], pp[1], pp[2], pp[3], pp[4], pp[5], pp[6], npeer);
-  KFAC_LAUNCH_CHECK();
-  return KFAC_OK;
+  return launch_gemm(g, s);
 }
 
 int gemm_tn_plain(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M, int N,
@@ -306,22 +282,21 @@ static void precond_layout(const kfac_precond_item* items, int count, PrecondLay
   L.off_slab = off;
   // long reductions (K > 1024) are split into chains of <= 512: the tensor-core accumulator truncates, short
   // chains keep the 3xTF32 result at fp32 accuracy; the partial tiles go to slabs and are added in a fixed order
-  // (deterministic: every replica that preconditions a layer locally must get the same bits)
+  // (deterministic: every replica that preconditions a layer locally must get the same bits).  The layout does not
+  // depend on n_peers: a fused broadcast runs the same split, its peers get the reduced sums.
   for (int i = 0; i < count; ++i) {
     const size_t a = items[i].a, g = items[i].g;
     if (is_diag(items[i])) {
       // only the plain product with Q^T (K = n) can split; the products with an epilogue run unsplit, like stage (2)
       const DiagItem D = diag_view(items[i]);
-      if (D.n > 1024 && items[i].n_peers == 0) {
+      if (D.n > 1024) {
         L.splits_g[i] = ceil_div(D.n, 512);
         L.slab_g[i] = take((size_t)L.splits_g[i] * D.rows * ld4(D.n) * sizeof(float));
       }
       continue;
     }
     if (a > 1024) { L.splits_a[i] = ceil_div(a, 512); L.slab_a[i] = take((size_t)L.splits_a[i] * a * ld4((int)g) * sizeof(float)); }
-    if (g > 1024 && items[i].n_peers == 0) {
-      L.splits_g[i] = ceil_div(g, 512); L.slab_g[i] = take((size_t)L.splits_g[i] * g * ld4((int)a) * sizeof(float));
-    }
+    if (g > 1024) { L.splits_g[i] = ceil_div(g, 512); L.slab_g[i] = take((size_t)L.splits_g[i] * g * ld4((int)a) * sizeof(float)); }
   }
   L.total = off;
 }
@@ -505,12 +480,12 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
     } else {
       plain(i, method == KFAC_EIGEN ? it.qg : it.g_inv, it.ldqg, F(L.t1[i]), ld4(g), it.P, it.ldp, g, a, g);
     }
-    if (it.n_peers > 0) {               // fused compute + broadcast: no split (the tiles are final when stored)
-      st[i].npeer = it.n_peers;
-      for (int q = 0; q < it.n_peers; ++q) st[i].peerD[q] = it.peer_P[q];
-    } else if (L.splits_g[i] > 1 && it.ldp == p_ld && st[i].epi == EPI_NONE) {
+    if (L.splits_g[i] > 1 && it.ldp == p_ld && st[i].epi == EPI_NONE) {
       st[i].splits = L.splits_g[i]; st[i].slab = F(L.slab_g[i]); st[i].slab_stride = p_rows * p_ld;
     }
+    // fused compute + broadcast: the same P goes to the peers, from the tile epilogue or from the split's reduce pass
+    st[i].npeer = it.n_peers;
+    for (int q = 0; q < it.n_peers; ++q) st[i].peerD[q] = it.peer_P[q];
   }
   return run();
 }
