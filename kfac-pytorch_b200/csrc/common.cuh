@@ -229,4 +229,22 @@ inline int tc_normalize_splits(int splits, int kb_total) {
 int launch_tc_gemm(const TcGemmArgs& a, cudaStream_t stream);
 int tc_num_sms();
 
+// Pinned host memory for the small tables a call sends to the device.  A copy from pageable memory may make the host
+// wait until the stream reaches it (the driver stages it), which holds back the enqueue of work for other streams; a
+// copy from pinned memory is only queued.  The tables of a call must stay until the device has read them: begin()
+// waits for the event that the previous call's end() recorded, then reuses the memory (merged into one block).
+struct HostStage {
+  char* buf[8] = {};
+  size_t size[8] = {};
+  int nbuf = 0;
+  size_t used = 0;               // bytes taken from buf[nbuf - 1]
+  cudaEvent_t done = nullptr;
+  bool pending = false;
+  int begin();
+  int send(void* dst, const void* src, size_t bytes, cudaStream_t s);   // cudaMemcpyAsync host -> device through it
+  int end(cudaStream_t s);       // the device has read every table sent since begin() once s reaches this point
+};
+// host -> device copy of a table on s: through `stage` when given, straight from src otherwise
+int send_table(HostStage* stage, void* dst, const void* src, size_t bytes, cudaStream_t s);
+
 }  // namespace kfac

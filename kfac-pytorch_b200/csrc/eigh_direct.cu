@@ -1,8 +1,8 @@
 // Direct symmetric eigensolver for the large K-FAC factors (replaces torch.linalg.eigh of
 // kfac/layers/eigen.py:310,331 for n > 128):  F = H T H^T (sytrd.cu), T = Z L Z^T (stedc.cu),
 // Q = H Z by compact-WY block reflectors of 128 Householder vectors (this file; wgmma GEMMs).
-// Host side: workspace layout, the CTA-group schedule of the tridiagonalisation kernel, and the
-// enqueue of all stages on ONE stream without host synchronisation.
+// Host side: workspace layout, the CTA-group schedule of the tridiagonalisation kernel, its waves, and the
+// enqueue of all stages (one stream per wave) without host synchronisation.
 #include "eigh_direct.cuh"
 
 #include <math.h>
@@ -152,14 +152,29 @@ struct MatLayout {
   int ksplit;      // split count of the longest reduction of the back-transformation (K = np)
 };
 
+// One wave of the schedule (make_waves): a set of jobs whose CTAs no other wave's job uses.  It runs as its own
+// cooperative launch, followed by the divide and conquer and back-transformation of its matrices, on its own stream.
+struct Wave {
+  std::vector<TrdJob> jobs;   // in the schedule's order; cta0 rebased onto the wave's grid, id = place in the schedule
+  int ncta = 0;               // grid of its launch: the CTAs its jobs use
+  int cap = 0;                // grid cap of its grouped GEMMs: the SMs free when it ends (by the predicted ends)
+};
+
+struct WaveLayout {
+  int slot0, blk0;            // first entry of the wave in the job / DcMat / per-wave IoMat tables and in the BtBlock table
+  size_t off_plan, plan_bytes, off_gws, gws_bytes;
+};
+
 struct Layout {
   std::vector<MatLayout> m;
-  size_t off_trd, off_jobs, off_dc, off_blocks, off_io, off_plan, plan_bytes, off_gws, gws_bytes, off_amax, zero_begin, zero_end,
-      total;
+  std::vector<WaveLayout> w;
+  size_t off_trd, off_jobs, off_dc, off_blocks, off_io, off_amax, zero_begin, zero_end, total;
   int nblocks;
 };
 
-void make_layout(const int* n, int count, Layout& L) {
+// Tables that are sent to the device are laid out in wave order, and each wave has its own plan and GEMM workspace:
+// launches on different streams share no table and no workspace.
+void make_layout(const int* n, int count, const std::vector<Wave>& waves, Layout& L) {
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
   L.m.resize(count);
@@ -169,11 +184,21 @@ void make_layout(const int* n, int count, Layout& L) {
   L.nblocks = 0;
   for (int i = 0; i < count; ++i) L.nblocks += ceil_div(n[i], BT);
   L.off_blocks = take(sizeof(BtBlock) * std::max(1, L.nblocks));
-  L.off_io = take(sizeof(IoMat) * count);
-  L.plan_bytes = stedc_plan_bytes(n, count);
-  L.off_plan = take(L.plan_bytes);
-  L.gws_bytes = grouped_gemm_ws_bytes(std::max(L.nblocks, count));
-  L.off_gws = take(L.gws_bytes);
+  L.off_io = take(sizeof(IoMat) * 2 * count);        // [0, count): the input stage, [count, 2 count): per wave
+  L.w.resize(waves.size());
+  int slot = 0, blk = 0;
+  for (size_t k = 0; k < waves.size(); ++k) {
+    WaveLayout& w = L.w[k];
+    std::vector<int> nw;
+    int nblk = 0;
+    for (const TrdJob& j : waves[k].jobs) { nw.push_back(n[j.mat]); nblk += ceil_div(n[j.mat], BT); }
+    w.slot0 = slot; w.blk0 = blk;
+    slot += (int)nw.size(); blk += nblk;
+    w.plan_bytes = stedc_plan_bytes(nw.data(), (int)nw.size());
+    w.off_plan = take(w.plan_bytes);
+    w.gws_bytes = grouped_gemm_ws_bytes(std::max(nblk, (int)nw.size()));
+    w.off_gws = take(w.gws_bytes);
+  }
   const int grid = sytrd_max_grid();
   // everything that must start as zeros lies in ONE region (one memset per call): the reflector stores (their padding
   // is a GEMM reduction dimension), the panel, barrier and partial-scalar state of the tridiagonalisation, the two
@@ -261,7 +286,7 @@ void make_schedule(const int* n, int count, int G, std::vector<TrdJob>& jobs, st
   // a consistent global order (every CTA walks the list front to back) keeps the group barriers deadlock free
   std::stable_sort(placed.begin(), placed.end(), [](const Placed& a, const Placed& b) { return a.start < b.start; });
   jobs.clear();
-  for (auto& p : placed) jobs.push_back(p.job);
+  for (auto& p : placed) { p.job.id = (int)jobs.size(); jobs.push_back(p.job); }
   if (start) {
     start->clear();
     for (auto& p : placed) start->push_back(p.start);
@@ -326,6 +351,84 @@ void make_pin_plan(const int* n, int count, const std::vector<TrdJob>& jobs, con
   }
 }
 
+// ---- waves: parts of the schedule that can run on their own ---------------------------------------------------------
+// Jobs that share a CTA are joined into components; no group barrier crosses from one component to another.  The
+// later stages of a matrix (divide and conquer, back-transformation) can start as soon as its component is done, but
+// in one launch they wait for the slowest job of the whole batch.  So the components are merged into at most
+// `max_waves` waves, each a launch of its own followed by the later stages of its matrices on its own stream.  The
+// waves are contiguous runs of the components sorted by predicted end, cut where the time the later-stage work waits
+// for the end of its wave (weighted by n^3, the scale of that work) is smallest; of equally good cuts the one with the
+// fewest waves is taken.  A wave keeps its jobs in the schedule's order, which keeps its group barriers deadlock free.
+constexpr int EIGH_WAVES = StreamPool::N;
+int g_max_waves = -1;                                 // test override (kfac_stage_eigh_max_waves); < 1: EIGH_WAVES
+
+void make_waves(const int* n, int G, const std::vector<TrdJob>& jobs, const std::vector<double>& start, int max_waves,
+                std::vector<Wave>& waves) {
+  std::vector<int> root(G);
+  for (int c = 0; c < G; ++c) root[c] = c;
+  auto find = [&](int c) { while (root[c] != c) { root[c] = root[root[c]]; c = root[c]; } return c; };
+  for (const TrdJob& j : jobs)
+    for (int c = j.cta0 + 1; c < j.cta0 + j.ncta; ++c) root[find(c)] = find(j.cta0);
+  std::vector<double> end(G, -1.0), work(G, 0.0);
+  for (size_t j = 0; j < jobs.size(); ++j) {
+    const int r = find(jobs[j].cta0), nj = n[jobs[j].mat];
+    end[r] = std::max(end[r], start[j] + job_time(nj, jobs[j].ncta));
+    work[r] += (double)nj * nj * nj;
+  }
+  std::vector<int> comp;
+  for (int c = 0; c < G; ++c) if (end[c] >= 0.0) comp.push_back(c);
+  std::stable_sort(comp.begin(), comp.end(), [&](int a, int b) { return end[a] < end[b]; });
+  const int m = (int)comp.size(), K = std::max(1, std::min(max_waves, m));
+  std::vector<double> W(m + 1, 0.0), WE(m + 1, 0.0);
+  for (int i = 0; i < m; ++i) { W[i + 1] = W[i] + work[comp[i]]; WE[i + 1] = WE[i] + work[comp[i]] * end[comp[i]]; }
+  auto wait = [&](int a, int b) { return end[comp[b]] * (W[b + 1] - W[a]) - (WE[b + 1] - WE[a]); };   // components a..b
+  // f[k][b]: least wait of components 0..b in k + 1 waves; first[k][b]: first component of the last of them
+  std::vector<std::vector<double>> f(K, std::vector<double>(m, 1e300));
+  std::vector<std::vector<int>> first(K, std::vector<int>(m, 0));
+  for (int b = 0; b < m; ++b) f[0][b] = wait(0, b);
+  for (int k = 1; k < K; ++k)
+    for (int b = k; b < m; ++b)
+      for (int a = k; a <= b; ++a) {
+        const double t = f[k - 1][a - 1] + wait(a, b);
+        if (t < f[k][b]) { f[k][b] = t; first[k][b] = a; }
+      }
+  int k = 0;
+  while (k < K - 1 && f[k][m - 1] > f[K - 1][m - 1] + 1e-9 * W[m] * end[comp[m - 1]]) ++k;
+  std::vector<int> wave_of(G, -1);
+  for (int b = m - 1, kk = k; b >= 0; --kk) {
+    const int a = kk > 0 ? first[kk][b] : 0;
+    for (int i = a; i <= b; ++i) wave_of[comp[i]] = kk;
+    b = a - 1;
+  }
+  waves.assign(k + 1, Wave{});
+  std::vector<int> used(G, -1);                        // wave of every CTA a job uses
+  for (const TrdJob& j : jobs)
+    for (int c = j.cta0; c < j.cta0 + j.ncta; ++c) used[c] = wave_of[find(j.cta0)];
+  int freed = 0;                                       // CTAs no job uses, then those of the waves that end earlier
+  for (int c = 0; c < G; ++c) freed += used[c] < 0;
+  for (int w = 0; w <= k; ++w) {
+    std::vector<int> rank(G, 0);                       // CTA -> its place in the wave's grid
+    int nc = 0;
+    for (int c = 0; c < G; ++c) if (used[c] == w) rank[c] = nc++;
+    Wave& wv = waves[w];
+    wv.ncta = nc;
+    // the SMs free when the wave ends, by the predicted ends: its own and those of the waves before it (the last: all)
+    freed += nc;
+    wv.cap = freed;
+    for (const TrdJob& j : jobs)
+      if (used[j.cta0] == w) wv.jobs.push_back(TrdJob{j.mat, rank[j.cta0], j.ncta, j.id});
+  }
+}
+
+// schedule, waves and workspace layout of one call
+void make_plan(const int* n, int count, std::vector<TrdJob>& jobs, std::vector<double>& start, std::vector<Wave>& waves,
+               Layout& L) {
+  const int G = sytrd_max_grid();
+  make_schedule(n, count, G, jobs, &start);
+  make_waves(n, G, jobs, start, g_max_waves >= 1 ? g_max_waves : EIGH_WAVES, waves);
+  make_layout(n, count, waves, L);
+}
+
 }  // namespace
 
 int StreamPool::init() {
@@ -371,13 +474,151 @@ int gemm_tn_acc(const float* A, int64_t lda, const float* B, int64_t ldb, float*
 
 size_t eigh_direct_workspace_bytes(const int* n, int count) {
   if (count <= 0) return 0;
+  std::vector<TrdJob> jobs;
+  std::vector<double> start;
+  std::vector<Wave> waves;
   Layout L;
-  make_layout(n, count, L);
+  make_plan(n, count, jobs, start, waves, L);
   return align_up(L.total, 1024);
 }
 
-// stage selector for tests / profiling: 1 = stop after the tridiagonalisation (d, e in the items' d / Q row 0),
-// 0 = full solve
+namespace {
+
+// divide and conquer and back-transformation of the matrices of one wave, on stream s
+int run_wave_tail(const Wave& wave, const WaveLayout& wl, const Layout& L, char* base, const std::vector<TrdMat>& trd,
+                  std::vector<DcMat>& dc, std::vector<IoMat>& io, int* status, HostStage* stage, cudaStream_t s) {
+  const int cnt = (int)wave.jobs.size(), cap = wave.cap;
+  std::vector<int> mats(cnt);
+  for (int k = 0; k < cnt; ++k) mats[k] = wave.jobs[k].mat;
+  int rc;
+  {
+    std::vector<DcMat> dw(cnt);
+    for (int k = 0; k < cnt; ++k) dw[k] = dc[mats[k]];
+    DcMat* d_dc = (DcMat*)(base + L.off_dc) + wl.slot0;
+    if ((rc = send_table(stage, d_dc, dw.data(), sizeof(DcMat) * cnt, s))) return rc;
+    if ((rc = launch_stedc(dw.data(), d_dc, cnt, base + wl.off_plan, wl.plan_bytes, status, s, /*q_zeroed=*/true, cap, stage)))
+      return rc;
+    for (int k = 0; k < cnt; ++k) dc[mats[k]].result_buf = dw[k].result_buf;
+  }
+
+  // ---- back-transformation: QT = Z^T B_{L-1}^T ... B_0^T, B_k = I - V_k T_k V_k^T
+  std::vector<BtBlock> blocks;
+  for (const int i : mats) {
+    const MatLayout& m = L.m[i];
+    for (int kb = 0; kb < m.nbt; ++kb) {
+      const int j0 = kb * BT, nb = std::min(BT, m.n - j0);
+      blocks.push_back(BtBlock{(float*)(base + m.S) + (size_t)kb * BT * BT, (float*)(base + m.Tm) + (size_t)kb * BT * BT,
+                               (float*)(base + m.TmT) + (size_t)kb * BT * BT, trd[i].tau + j0, nb});
+    }
+    // (S beyond the valid reflectors and the off-diagonal quadrants of T are zero: part of the zeroed region)
+  }
+  BtBlock* d_blocks = (BtBlock*)(base + L.off_blocks) + wl.blk0;
+  if ((rc = send_table(stage, d_blocks, blocks.data(), sizeof(BtBlock) * blocks.size(), s))) return rc;
+  void* gws = base + wl.off_gws;
+  const size_t gws_bytes = wl.gws_bytes;
+  auto plain = [](const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M, int N, int K) {
+    GroupedGemm g{};
+    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.D = D; g.ldd = ldd; g.M = M; g.N = N; g.K = K;
+    g.alpha = 1.f; g.epi = EPI_NONE; g.splits = 1; g.mode = 0;
+    return g;
+  };
+  // S_k = V_k^T V_k for every block of every matrix: one grouped launch (long reductions through slabs)
+  {
+    std::vector<GroupedGemm> gg;
+    for (const int i : mats) {
+      const MatLayout& m = L.m[i];
+      const TrdMat& t = trd[i];
+      for (int kb = 0; kb < m.nbt; ++kb) {
+        const int j0 = kb * BT, nb = std::min(BT, m.n - j0), K = m.np - j0;
+        const float* Vk = t.VT + (size_t)j0 * t.ldv + j0;
+        GroupedGemm g = plain(Vk, t.ldv, Vk, t.ldv, (float*)(base + m.S) + (size_t)kb * BT * BT, BT, nb, nb, K);
+        if (K > 1024 && grouped_gemm_tc_ok(g)) {
+          g.splits = ceil_div(K, 512);
+          g.slab = (float*)(base + m.slabS) + (size_t)kb * m.ksplit * BT * BT; g.slab_stride = (int64_t)nb * BT;
+        }
+        gg.push_back(g);
+      }
+    }
+    if ((rc = launch_grouped_gemm(gg.data(), (int)gg.size(), gws, gws_bytes, s, cap, stage))) return rc;
+  }
+  {
+    static bool attr = false;
+    const int lsmem = LB * (LB + 1) * (int)sizeof(float);
+    if (!attr) { KFAC_CUDA(cudaFuncSetAttribute(larft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lsmem)); attr = true; }
+    larft_kernel<<<2 * (int)blocks.size(), LB, lsmem, s>>>(d_blocks);
+    KFAC_LAUNCH_CHECK();
+    // T12 = -T1 (S12 T2) for every block with more than LB reflectors: X^T = T2^T S12^T, then T12 = -T1 X
+    std::vector<GroupedGemm> x1, x2;
+    for (const int i : mats) {
+      const MatLayout& m = L.m[i];
+      for (int kb = 0; kb < m.nbt; ++kb) {
+        const int nb = std::min(BT, m.n - kb * BT);
+        if (nb <= LB) continue;
+        float* S = (float*)(base + m.S) + (size_t)kb * BT * BT;
+        float* Tm = (float*)(base + m.Tm) + (size_t)kb * BT * BT;
+        float* TmT = (float*)(base + m.TmT) + (size_t)kb * BT * BT;
+        float* Xt = (float*)(base + m.Xt) + (size_t)kb * LB * LB;
+        x1.push_back(plain(TmT + (size_t)LB * BT + LB, BT, S + LB, BT, Xt, LB, LB, LB, LB));
+        GroupedGemm g = plain(Tm, BT, Xt, LB, Tm + LB, BT, LB, LB, LB);
+        g.alpha = -1.f;
+        x2.push_back(g);
+      }
+    }
+    if (!x1.empty()) {
+      if ((rc = launch_grouped_gemm(x1.data(), (int)x1.size(), gws, gws_bytes, s, cap, stage))) return rc;
+      if ((rc = launch_grouped_gemm(x2.data(), (int)x2.size(), gws, gws_bytes, s, cap, stage))) return rc;
+    }
+  }
+  int max_nbt = 0, n_max = 0;
+  std::vector<IoMat> iw(cnt);
+  for (int k = 0; k < cnt; ++k) {
+    const int i = mats[k];
+    const DcMat& d = dc[i];
+    max_nbt = std::max(max_nbt, L.m[i].nbt);
+    n_max = std::max(n_max, L.m[i].n);
+    io[i].Z = d.Q[d.result_buf]; io[i].ZT = d.Q[d.result_buf ^ 1];
+    iw[k] = io[i];
+  }
+  // (the wave's own table, with the buffer parity the plan of the divide and conquer ended on)
+  IoMat* d_io = (IoMat*)(base + L.off_io) + L.m.size() + wl.slot0;
+  if ((rc = send_table(stage, d_io, iw.data(), sizeof(IoMat) * cnt, s))) return rc;
+  transpose_z_kernel<<<dim3(ceil_div(n_max, 32), ceil_div(n_max, 32), cnt), dim3(32, 8), 0, s>>>(d_io);
+  KFAC_LAUNCH_CHECK();
+  // block reflectors, last block first; step t handles block (nbt - 1 - t) of every matrix that still has one:
+  // three grouped launches per step instead of three GEMMs per block and matrix
+  for (int tstep = 0; tstep < max_nbt; ++tstep) {
+    std::vector<GroupedGemm> g1, g2, g3;
+    for (const int i : mats) {
+      const MatLayout& m = L.m[i];
+      if (m.nbt <= tstep) continue;
+      const TrdMat& t = trd[i];
+      const DcMat& d = dc[i];
+      const int n = m.n, np = m.np, kb = m.nbt - 1 - tstep, j0 = kb * BT, nbp = std::min(BT, np - j0), K = np - j0;
+      float* ZT = d.Q[d.result_buf ^ 1];
+      float* Y = (float*)(base + m.Y);
+      float* Y2 = (float*)(base + m.Y2);
+      // Y = ZT[:, j0:] V_k[j0:, :]
+      GroupedGemm a = plain(ZT + j0, np, t.VT + (size_t)j0 * t.ldv + j0, t.ldv, Y, BT, n, nbp, K);
+      if (K > 1024 && grouped_gemm_tc_ok(a)) { a.splits = ceil_div(K, 512); a.slab = (float*)(base + m.slabY); a.slab_stride = (int64_t)n * BT; }
+      g1.push_back(a);
+      // Y2 = Y T_k^T
+      g2.push_back(plain(Y, BT, (float*)(base + m.Tm) + (size_t)kb * BT * BT, BT, Y2, BT, n, nbp, nbp));
+      // ZT[:, j0:] -= Y2 V_k[j0:, :]^T
+      GroupedGemm c = plain(Y2, BT, t.Vb + (size_t)kb * np * BT + (size_t)j0 * BT, BT, ZT + j0, np, n, K, nbp);
+      c.alpha = -1.f; c.mode = 1;
+      g3.push_back(c);
+    }
+    if ((rc = launch_grouped_gemm(g1.data(), (int)g1.size(), gws, gws_bytes, s, cap, stage))) return rc;
+    if ((rc = launch_grouped_gemm(g2.data(), (int)g2.size(), gws, gws_bytes, s, cap, stage))) return rc;
+    if ((rc = launch_grouped_gemm(g3.data(), (int)g3.size(), gws, gws_bytes, s, cap, stage))) return rc;
+  }
+  outputs_kernel<<<dim3(ceil_div(n_max, 32), ceil_div(n_max, 32), cnt), dim3(32, 8), 0, s>>>(d_io, status);
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
+}  // namespace
+
 int eigh_direct_run(const kfac_eigh_item* items, int count, void* ws, size_t ws_bytes, int* status, cudaStream_t s) {
   if (count <= 0) return KFAC_OK;
   std::vector<int> ns(count);
@@ -395,11 +636,13 @@ int eigh_direct_run(const kfac_eigh_item* items, int count, void* ws, size_t ws_
       return KFAC_ERR_UNSUPPORTED;
     }
   }
+  std::vector<TrdJob> jobs;
+  std::vector<double> start;
+  std::vector<Wave> waves;
   Layout L;
-  make_layout(ns.data(), count, L);
+  make_plan(ns.data(), count, jobs, start, waves, L);
   if (!ws || ws_bytes < L.total) { set_error("eigh(direct): workspace too small (%zu < %zu)", ws_bytes, L.total); return KFAC_ERR_WORKSPACE; }
   char* base = (char*)ws;
-  const int G = sytrd_max_grid();
   std::vector<TrdMat> trd(count);
   std::vector<DcMat> dc(count);
   int np_max = 0;
@@ -438,134 +681,47 @@ int eigh_direct_run(const kfac_eigh_item* items, int count, void* ws, size_t ws_
   KFAC_LAUNCH_CHECK();
   pad_copy_kernel<<<io_grid, 256, 0, s>>>(d_io, status);
   KFAC_LAUNCH_CHECK();
-  std::vector<TrdJob> jobs;
-  std::vector<double> start;
-  make_schedule(ns.data(), count, G, jobs, &start);
   std::vector<int> pin_j0;
   make_pin_plan(ns.data(), count, jobs, start, g_pin_budget >= 0 ? g_pin_budget : TRD_PIN_BUDGET, pin_j0);
   bool any_pin = false;
   for (int i = 0; i < count; ++i) any_pin |= pin_j0[i] < trd[i].nblk;
   for (int i = 0; i < count; ++i) { trd[i].pin_j0 = pin_j0[i]; trd[i].stream_first = any_pin ? 1 : 0; }
   TrdMat* d_trd = (TrdMat*)(base + L.off_trd);
-  TrdJob* d_jobs = (TrdJob*)(base + L.off_jobs);
-  DcMat* d_dc = (DcMat*)(base + L.off_dc);
   KFAC_CUDA(cudaMemcpyAsync(d_trd, trd.data(), sizeof(TrdMat) * count, cudaMemcpyHostToDevice, s));
-  KFAC_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(TrdJob) * jobs.size(), cudaMemcpyHostToDevice, s));
-  KFAC_CUDA(cudaMemcpyAsync(d_dc, dc.data(), sizeof(DcMat) * count, cudaMemcpyHostToDevice, s));
+  // one wave runs on s; several run on the side streams, which join s before the call returns (also on an error)
+  const int nw = (int)waves.size();
+  StreamPool& pool = stream_pool();
+  // with several waves their tables go through pinned host memory: a pageable copy may make the host wait for one
+  // wave's stream while the others still need their work enqueued
+  HostStage* stage = nw > 1 ? &pool.stage : nullptr;
   int rc;
-  if ((rc = launch_sytrd(d_trd, d_jobs, (int)jobs.size(), np_max, G, s))) return rc;
-  if ((rc = launch_stedc(dc.data(), d_dc, count, base + L.off_plan, L.plan_bytes, status, s, /*q_zeroed=*/true))) return rc;
-
-  // ---- back-transformation: QT = Z^T B_{L-1}^T ... B_0^T, B_k = I - V_k T_k V_k^T
-  std::vector<BtBlock> blocks;
-  for (int i = 0; i < count; ++i) {
-    const MatLayout& m = L.m[i];
-    for (int kb = 0; kb < m.nbt; ++kb) {
-      const int j0 = kb * BT, nb = std::min(BT, m.n - j0);
-      blocks.push_back(BtBlock{(float*)(base + m.S) + (size_t)kb * BT * BT, (float*)(base + m.Tm) + (size_t)kb * BT * BT,
-                               (float*)(base + m.TmT) + (size_t)kb * BT * BT, trd[i].tau + j0, nb});
+  if (stage && (rc = stage->begin())) return rc;
+  if (nw > 1 && (rc = pool.fork(s))) return rc;
+  auto wave_stream = [&](int w) { return nw > 1 ? pool.st[w] : s; };
+  auto done = [&](int r) -> int {
+    if (nw > 1) {
+      int j = pool.join(s);
+      if (!j) j = stage->end(s);
+      if (!r) r = j;
     }
-    // (S beyond the valid reflectors and the off-diagonal quadrants of T are zero: part of the zeroed region)
-  }
-  BtBlock* d_blocks = (BtBlock*)(base + L.off_blocks);
-  KFAC_CUDA(cudaMemcpyAsync(d_blocks, blocks.data(), sizeof(BtBlock) * blocks.size(), cudaMemcpyHostToDevice, s));
-  void* gws = base + L.off_gws;
-  auto plain = [](const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M, int N, int K) {
-    GroupedGemm g{};
-    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.D = D; g.ldd = ldd; g.M = M; g.N = N; g.K = K;
-    g.alpha = 1.f; g.epi = EPI_NONE; g.splits = 1; g.mode = 0;
-    return g;
+    return r;
   };
-  // S_k = V_k^T V_k for every block of every matrix: one grouped launch (long reductions through slabs)
-  {
-    std::vector<GroupedGemm> gg;
-    for (int i = 0; i < count; ++i) {
-      const MatLayout& m = L.m[i];
-      const TrdMat& t = trd[i];
-      for (int kb = 0; kb < m.nbt; ++kb) {
-        const int j0 = kb * BT, nb = std::min(BT, m.n - j0), K = m.np - j0;
-        const float* Vk = t.VT + (size_t)j0 * t.ldv + j0;
-        GroupedGemm g = plain(Vk, t.ldv, Vk, t.ldv, (float*)(base + m.S) + (size_t)kb * BT * BT, BT, nb, nb, K);
-        if (K > 1024 && grouped_gemm_tc_ok(g)) {
-          g.splits = ceil_div(K, 512);
-          g.slab = (float*)(base + m.slabS) + (size_t)kb * m.ksplit * BT * BT; g.slab_stride = (int64_t)nb * BT;
-        }
-        gg.push_back(g);
-      }
-    }
-    if ((rc = launch_grouped_gemm(gg.data(), (int)gg.size(), gws, L.gws_bytes, s))) return rc;
-  }
-  {
-    static bool attr = false;
-    const int lsmem = LB * (LB + 1) * (int)sizeof(float);
-    if (!attr) { KFAC_CUDA(cudaFuncSetAttribute(larft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lsmem)); attr = true; }
-    larft_kernel<<<2 * (int)blocks.size(), LB, lsmem, s>>>(d_blocks);
-    KFAC_LAUNCH_CHECK();
-    // T12 = -T1 (S12 T2) for every block with more than LB reflectors: X^T = T2^T S12^T, then T12 = -T1 X
-    std::vector<GroupedGemm> x1, x2;
-    for (int i = 0; i < count; ++i) {
-      const MatLayout& m = L.m[i];
-      for (int kb = 0; kb < m.nbt; ++kb) {
-        const int nb = std::min(BT, m.n - kb * BT);
-        if (nb <= LB) continue;
-        float* S = (float*)(base + m.S) + (size_t)kb * BT * BT;
-        float* Tm = (float*)(base + m.Tm) + (size_t)kb * BT * BT;
-        float* TmT = (float*)(base + m.TmT) + (size_t)kb * BT * BT;
-        float* Xt = (float*)(base + m.Xt) + (size_t)kb * LB * LB;
-        x1.push_back(plain(TmT + (size_t)LB * BT + LB, BT, S + LB, BT, Xt, LB, LB, LB, LB));
-        GroupedGemm g = plain(Tm, BT, Xt, LB, Tm + LB, BT, LB, LB, LB);
-        g.alpha = -1.f;
-        x2.push_back(g);
-      }
-    }
-    if (!x1.empty()) {
-      if ((rc = launch_grouped_gemm(x1.data(), (int)x1.size(), gws, L.gws_bytes, s))) return rc;
-      if ((rc = launch_grouped_gemm(x2.data(), (int)x2.size(), gws, L.gws_bytes, s))) return rc;
-    }
-  }
-  int max_nbt = 0, n_max = 0;
-  for (int i = 0; i < count; ++i) {
-    const MatLayout& m = L.m[i];
-    const DcMat& d = dc[i];
-    max_nbt = std::max(max_nbt, m.nbt);
-    n_max = std::max(n_max, m.n);
-    io[i].Z = d.Q[d.result_buf]; io[i].ZT = d.Q[d.result_buf ^ 1];
-  }
-  // (the table is re-sent with the buffer parity the plan of the divide and conquer ended on)
-  KFAC_CUDA(cudaMemcpyAsync(d_io, io.data(), sizeof(IoMat) * count, cudaMemcpyHostToDevice, s));
-  transpose_z_kernel<<<dim3(ceil_div(n_max, 32), ceil_div(n_max, 32), count), dim3(32, 8), 0, s>>>(d_io);
-  KFAC_LAUNCH_CHECK();
-  // block reflectors, last block first; step t handles block (nbt - 1 - t) of every matrix that still has one:
-  // three grouped launches per step instead of three GEMMs per block and matrix
-  for (int tstep = 0; tstep < max_nbt; ++tstep) {
-    std::vector<GroupedGemm> g1, g2, g3;
-    for (int i = 0; i < count; ++i) {
-      const MatLayout& m = L.m[i];
-      if (m.nbt <= tstep) continue;
-      const TrdMat& t = trd[i];
-      const DcMat& d = dc[i];
-      const int n = m.n, np = m.np, kb = m.nbt - 1 - tstep, j0 = kb * BT, nbp = std::min(BT, np - j0), K = np - j0;
-      float* ZT = d.Q[d.result_buf ^ 1];
-      float* Y = (float*)(base + m.Y);
-      float* Y2 = (float*)(base + m.Y2);
-      // Y = ZT[:, j0:] V_k[j0:, :]
-      GroupedGemm a = plain(ZT + j0, np, t.VT + (size_t)j0 * t.ldv + j0, t.ldv, Y, BT, n, nbp, K);
-      if (K > 1024 && grouped_gemm_tc_ok(a)) { a.splits = ceil_div(K, 512); a.slab = (float*)(base + m.slabY); a.slab_stride = (int64_t)n * BT; }
-      g1.push_back(a);
-      // Y2 = Y T_k^T
-      g2.push_back(plain(Y, BT, (float*)(base + m.Tm) + (size_t)kb * BT * BT, BT, Y2, BT, n, nbp, nbp));
-      // ZT[:, j0:] -= Y2 V_k[j0:, :]^T
-      GroupedGemm c = plain(Y2, BT, t.Vb + (size_t)kb * np * BT + (size_t)j0 * BT, BT, ZT + j0, np, n, K, nbp);
-      c.alpha = -1.f; c.mode = 1;
-      g3.push_back(c);
-    }
-    if ((rc = launch_grouped_gemm(g1.data(), (int)g1.size(), gws, L.gws_bytes, s))) return rc;
-    if ((rc = launch_grouped_gemm(g2.data(), (int)g2.size(), gws, L.gws_bytes, s))) return rc;
-    if ((rc = launch_grouped_gemm(g3.data(), (int)g3.size(), gws, L.gws_bytes, s))) return rc;
-  }
-  outputs_kernel<<<dim3(ceil_div(n_max, 32), ceil_div(n_max, 32), count), dim3(32, 8), 0, s>>>(d_io, status);
-  KFAC_LAUNCH_CHECK();
-  return KFAC_OK;
+  // every wave's tridiagonalisation is enqueued before any later stage: the launches start together
+  auto launch_wave = [&](int w) -> int {
+    const Wave& wv = waves[w];
+    const cudaStream_t sw = wave_stream(w);
+    TrdJob* d_jobs = (TrdJob*)(base + L.off_jobs) + L.w[w].slot0;
+    int np_w = 0;
+    for (const TrdJob& j : wv.jobs) np_w = std::max(np_w, L.m[j.mat].np);
+    const int rc = send_table(stage, d_jobs, wv.jobs.data(), sizeof(TrdJob) * wv.jobs.size(), sw);
+    if (rc) return rc;
+    return launch_sytrd(d_trd, d_jobs, (int)wv.jobs.size(), np_w, wv.ncta, sw);
+  };
+  for (int w = 0; w < nw; ++w)
+    if ((rc = launch_wave(w))) return done(rc);
+  for (int w = 0; w < nw; ++w)
+    if ((rc = run_wave_tail(waves[w], L.w[w], L, base, trd, dc, io, status, stage, wave_stream(w)))) return done(rc);
+  return done(KFAC_OK);
 }
 
 }  // namespace kfac
@@ -675,6 +831,27 @@ extern "C" int kfac_stage_pin_plan(const int* n, int count, int grid, long long 
 }
 // test-only: the residency budget (bytes) of the following kfac_eigh_batched calls; < 0 restores the default
 extern "C" void kfac_stage_sytrd_pin_budget(long long bytes) { kfac::g_pin_budget = bytes; }
+
+// host-only: the waves of the schedule of kfac_stage_schedule (same dims and grid).  Per job of that list: its wave, its
+// first CTA on the wave's grid and its place in the wave's job list.  Returns the number of waves.
+extern "C" int kfac_stage_waves(const int* n, int count, int grid, int* wave, int* wave_cta0, int* wave_pos) {
+  using namespace kfac;
+  if (!n || count <= 0 || grid <= 0) return 0;
+  std::vector<TrdJob> jobs;
+  std::vector<double> start;
+  std::vector<Wave> waves;
+  make_schedule(n, count, grid, jobs, &start);
+  make_waves(n, grid, jobs, start, g_max_waves >= 1 ? g_max_waves : EIGH_WAVES, waves);
+  for (size_t w = 0; w < waves.size(); ++w)
+    for (size_t k = 0; k < waves[w].jobs.size(); ++k) {
+      const TrdJob& j = waves[w].jobs[k];
+      wave[j.id] = (int)w; wave_cta0[j.id] = j.cta0; wave_pos[j.id] = (int)k;
+    }
+  return (int)waves.size();
+}
+// test-only: the most waves the following calls (kfac_eigh_batched, its workspace size, kfac_stage_waves) split the
+// schedule into; < 1 restores the default.  1 runs every stage of every matrix on the caller's stream.
+extern "C" void kfac_stage_eigh_max_waves(int w) { kfac::g_max_waves = w; }
 
 namespace kfac {
 int sytrd_profile(int on, unsigned long long* out16);

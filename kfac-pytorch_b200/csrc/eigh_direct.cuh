@@ -37,7 +37,8 @@ struct TrdMat {
   int pin_j0, stream_first;
 };
 
-struct TrdJob { int mat, cta0, ncta; };
+// id: the job's place in the whole schedule (index of its %globaltimer stamps when a launch runs part of the list)
+struct TrdJob { int mat, cta0, ncta, id; };
 
 // all jobs of one launch; a CTA processes the jobs that contain it in list order
 int launch_sytrd(const TrdMat* d_mats, const TrdJob* d_jobs, int njobs, int np_max, int grid, cudaStream_t s);
@@ -64,8 +65,9 @@ size_t stedc_plan_bytes(const int* n, int count);   // includes the grouped-GEMM
 // plan_ws: device scratch of stedc_plan_bytes(); all work is enqueued on `s`
 // status: device int, bit 0 is set when a leaf QL iteration did not converge
 // q_zeroed: the caller has already zeroed Q[0] and Q[1] of every matrix
+// max_ctas, stage: grid cap of the grouped GEMMs and host stage of the tables (launch_grouped_gemm)
 int launch_stedc(DcMat* h_mats, DcMat* d_mats, int count, void* plan_ws, size_t plan_bytes, int* status, cudaStream_t s,
-                 bool q_zeroed = false);
+                 bool q_zeroed = false, int max_ctas = 0, HostStage* stage = nullptr);
 
 // plain fp32 TN GEMM on the wgmma engine: D = alpha * A B^T (+ D when accumulate)
 int gemm_tn_plain(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M, int N,
@@ -76,6 +78,7 @@ struct StreamPool {
   cudaStream_t st[N];
   cudaEvent_t ev_fork, ev_join[N];
   bool ready = false;
+  HostStage stage;              // tables sent by the work on the side streams
   int init();
   int fork(cudaStream_t s);     // side streams wait for everything enqueued on s so far
   int join(cudaStream_t s);     // s waits for everything enqueued on the side streams

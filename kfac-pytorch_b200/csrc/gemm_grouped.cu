@@ -163,7 +163,8 @@ size_t grouped_gemm_ws_bytes(int count) {
   return align_up(sizeof(GProb) * n, 256) + align_up(sizeof(RProb) * n, 256) + align_up(sizeof(RPeers) * n, 256);
 }
 
-int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws_bytes, cudaStream_t s) {
+int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws_bytes, cudaStream_t s, int max_ctas,
+                        HostStage* stage) {
   if (count <= 0) return KFAC_OK;
   if (!ws || ws_bytes < grouped_gemm_ws_bytes(count)) {
     set_error("grouped gemm: workspace too small (%zu < %zu)", ws_bytes, grouped_gemm_ws_bytes(count));
@@ -250,16 +251,18 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
   GProb* d_tab = (GProb*)ws;
   RProb* d_red = (RProb*)((char*)ws + align_up(sizeof(GProb) * (size_t)std::max(1, count), 256));
   RPeers* d_red_peers = (RPeers*)((char*)d_red + align_up(sizeof(RProb) * (size_t)std::max(1, count), 256));
-  KFAC_CUDA(cudaMemcpyAsync(d_tab, tab.data(), sizeof(GProb) * tab.size(), cudaMemcpyHostToDevice, s));
+  int rc;
+  if ((rc = send_table(stage, d_tab, tab.data(), sizeof(GProb) * tab.size(), s))) return rc;
   GroupedParams gp{d_tab, (int)tab.size()};
-  const int grid = std::min(work, tc_num_sms());
+  const int sms = max_ctas > 0 ? std::min(max_ctas, tc_num_sms()) : tc_num_sms();
+  const int grid = std::min(work, sms);
   tc::pipeline_kernel<GroupedPolicy><<<grid, tc::PTHREADS, tc::PSMEM, s>>>(gp, work);
   KFAC_LAUNCH_CHECK();
   if (!red.empty()) {
-    KFAC_CUDA(cudaMemcpyAsync(d_red, red.data(), sizeof(RProb) * red.size(), cudaMemcpyHostToDevice, s));
-    const int blocks = (int)std::min<long long>((red_total + 255) / 256, (long long)tc_num_sms() * 8);
+    if ((rc = send_table(stage, d_red, red.data(), sizeof(RProb) * red.size(), s))) return rc;
+    const int blocks = (int)std::min<long long>((red_total + 255) / 256, (long long)sms * 8);
     if (any_peers) {
-      KFAC_CUDA(cudaMemcpyAsync(d_red_peers, red_peers.data(), sizeof(RPeers) * red_peers.size(), cudaMemcpyHostToDevice, s));
+      if ((rc = send_table(stage, d_red_peers, red_peers.data(), sizeof(RPeers) * red_peers.size(), s))) return rc;
       grouped_reduce_kernel<true><<<blocks, 256, 0, s>>>(d_red, d_red_peers, (int)red.size(), red_total);
     } else {
       grouped_reduce_kernel<false><<<blocks, 256, 0, s>>>(d_red, nullptr, (int)red.size(), red_total);

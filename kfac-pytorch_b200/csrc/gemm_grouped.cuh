@@ -22,7 +22,12 @@ struct GroupedGemm {
 
 size_t grouped_gemm_ws_bytes(int count);
 bool grouped_gemm_tc_ok(const GroupedGemm& g);
-// problems the tensor-core kernel cannot take (tiny / unaligned) run as individual SIMT launches
-int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws_bytes, cudaStream_t s);
+// problems the tensor-core kernel cannot take (tiny / unaligned) run as individual SIMT launches.
+// max_ctas > 0 caps the grid of the tensor-core and reduce launches (default: one CTA per SM).  Work items are dealt
+// statically over the grid, so a launch that shares the GPU with a long-running kernel is capped at the SMs it can
+// get: CTAs that wait for an SM would hold back the whole launch.  The results do not depend on the grid.
+// stage: if given, the problem tables are sent through it (HostStage, common.cuh)
+int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws_bytes, cudaStream_t s, int max_ctas = 0,
+                        HostStage* stage = nullptr);
 
 }  // namespace kfac

@@ -537,7 +537,7 @@ size_t stedc_plan_bytes(const int* n, int count) {
 }
 
 int launch_stedc(DcMat* h_mats, DcMat* d_mats, int count, void* plan_ws, size_t plan_bytes, int* status, cudaStream_t s,
-                 bool q_zeroed) {
+                 bool q_zeroed, int max_ctas, HostStage* stage) {
   std::vector<int> ns(count);
   for (int i = 0; i < count; ++i) ns[i] = h_mats[i].n;
   Plan pl;
@@ -554,12 +554,13 @@ int launch_stedc(DcMat* h_mats, DcMat* d_mats, int count, void* plan_ws, size_t 
   const size_t gws_bytes = grouped_gemm_ws_bytes(2 * (int)widest);
   void* gws = take(gws_bytes);
   if (off > plan_bytes) { set_error("stedc: plan workspace too small (%zu < %zu)", plan_bytes, off); return KFAC_ERR_WORKSPACE; }
-  if (!pl.cuts.empty())
-    KFAC_CUDA(cudaMemcpyAsync(d_cuts, pl.cuts.data(), sizeof(DcCut) * pl.cuts.size(), cudaMemcpyHostToDevice, s));
-  KFAC_CUDA(cudaMemcpyAsync(d_leaves, pl.leaves.data(), sizeof(DcLeaf) * pl.leaves.size(), cudaMemcpyHostToDevice, s));
-  for (size_t l = 0; l < pl.levels.size(); ++l)
-    KFAC_CUDA(cudaMemcpyAsync(d_levels[l], pl.levels[l].data(), sizeof(DcMerge) * pl.levels[l].size(),
-                              cudaMemcpyHostToDevice, s));
+  {
+    int rc;
+    if ((rc = send_table(stage, d_cuts, pl.cuts.data(), sizeof(DcCut) * pl.cuts.size(), s))) return rc;
+    if ((rc = send_table(stage, d_leaves, pl.leaves.data(), sizeof(DcLeaf) * pl.leaves.size(), s))) return rc;
+    for (size_t l = 0; l < pl.levels.size(); ++l)
+      if ((rc = send_table(stage, d_levels[l], pl.levels[l].data(), sizeof(DcMerge) * pl.levels[l].size(), s))) return rc;
+  }
   // Q buffers: off-diagonal blocks must be zero
   for (int i = 0; i < count && !q_zeroed; ++i) {
     const size_t bytes = (size_t)h_mats[i].n * h_mats[i].ld * sizeof(float);
@@ -628,7 +629,7 @@ int launch_stedc(DcMat* h_mats, DcMat* d_mats, int count, void* plan_ws, size_t 
         gg.push_back(g);
       }
     }
-    { const int rc = launch_grouped_gemm(gg.data(), (int)gg.size(), gws, gws_bytes, s); if (rc) return rc; }
+    { const int rc = launch_grouped_gemm(gg.data(), (int)gg.size(), gws, gws_bytes, s, max_ctas, stage); if (rc) return rc; }
     if (mmax > DENSE_MAX) {
       dc_copy_deflated_kernel<<<dim3(ceil_div(mmax, 8), nm), 256, 0, s>>>(d_mats, d_levels[l]);
       KFAC_LAUNCH_CHECK();

@@ -89,7 +89,7 @@ __device__ __forceinline__ void l2_unpin(const float* ptr) {
 }
 
 // optional phase timing (CTA 0, thread 0 of every group accumulates clock64 deltas): set by kfac_stage_sytrd_profile,
-// which also records %globaltimer at the start and end of every job (on the job's first CTA)
+// which also records %globaltimer at the start and end of every job (on the job's first CTA, at TrdJob::id)
 __device__ unsigned long long g_trd_prof[16];
 __device__ int g_trd_prof_on = 0;
 constexpr int MAX_TIMED_JOBS = 512;
@@ -635,11 +635,11 @@ __global__ void __launch_bounds__(TRD_THREADS, 1) sytrd_kernel(const TrdMat* mat
     const TrdJob job = jobs[j];
     const int b = (int)blockIdx.x;
     if (b < job.cta0 || b >= job.cta0 + job.ncta) continue;
-    const bool stamp = g_trd_prof_on != 0 && b == job.cta0 && threadIdx.x == 0 && j < MAX_TIMED_JOBS;
-    if (stamp) g_trd_jobtime[2 * j] = globaltimer();
+    const bool stamp = g_trd_prof_on != 0 && b == job.cta0 && threadIdx.x == 0 && job.id >= 0 && job.id < MAX_TIMED_JOBS;
+    if (stamp) g_trd_jobtime[2 * job.id] = globaltimer();
     tridiagonalise(mats[job.mat], b - job.cta0, job.ncta, trd_smem);
     __syncthreads();
-    if (stamp) g_trd_jobtime[2 * j + 1] = globaltimer();
+    if (stamp) g_trd_jobtime[2 * job.id + 1] = globaltimer();
   }
 }
 
