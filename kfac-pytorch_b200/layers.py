@@ -21,6 +21,21 @@ from kfac_b200.attention import KFACMultiheadAttention
 from kfac_b200.recurrent import SWAPPED as RECURRENT_SWAPPED
 
 
+class FactorRows:
+    """The rows one call of a layer forms a factor's statistics of: n rows (B under K-FAC-reduce) of d features.
+
+    write(out_ptr, ld, grad_scale, loss_scale) writes them in fp32 at out_ptr with row stride ld, divided by grad_scale
+    and by the device float at loss_scale (or None).  direct(acc, grad_scale, scratch), when given, adds their
+    statistics to acc reading the layer's tensor in place (the expand entry points); without it the rows are written
+    and the statistics formed of them (ModuleHelper._accumulate_rows).  A slotted class: every factor hook builds one,
+    so it is kept cheap to construct."""
+    __slots__ = ('n', 'd', 'write', 'direct')
+
+    def __init__(self, n: int, d: int, write: Callable[[int, int, float, int | None], None],
+                 direct: Callable[[torch.Tensor, float, Any], None] | None = None) -> None:
+        self.n, self.d, self.write, self.direct = n, d, write, direct
+
+
 class ModuleHelper:
     """Geometry + native dispatch for one supported module type."""
 
@@ -77,27 +92,69 @@ class ModuleHelper:
         """The tensor accumulate_a, num_rows_a and write_rows_a of one call read, formed once per call."""
         return x
 
-    # native accumulation of the factor statistics of one micro-batch
-    def accumulate_a(self, x: torch.Tensor, acc: torch.Tensor, scratch) -> None:
+    # the declaration of one call's factor rows: each kind decides here, once per side, between K-FAC-reduce and
+    # expand, the row count and the scale of the rows
+    def rows_a(self, x: torch.Tensor) -> FactorRows:
         raise NotImplementedError
 
-    def accumulate_g(self, g: torch.Tensor, acc: torch.Tensor, grad_scale: float, scratch=None) -> None:
+    def rows_g(self, g: torch.Tensor) -> FactorRows:
         raise NotImplementedError
+
+    # native accumulation of the factor statistics of one micro-batch
+    def accumulate_a(self, x: torch.Tensor, acc: torch.Tensor, scratch) -> None:
+        rows = self.rows_a(_detached(x))
+        if rows.direct is not None:
+            rows.direct(acc, 1.0, scratch)
+        else:
+            self._accumulate_rows(rows, acc, 1.0, scratch, False)
+
+    def accumulate_g(self, g: torch.Tensor, acc: torch.Tensor, grad_scale: float, scratch) -> None:
+        rows = self.rows_g(_detached(g))
+        if rows.direct is not None:
+            rows.direct(acc, grad_scale, scratch)
+        else:
+            self._accumulate_rows(rows, acc, grad_scale, scratch, self.diagonal_g)
 
     # EKFAC row writers: the rows x_r / g_r of one micro-batch (exactly the rows the A / G statistics are formed of),
     # written sample-major in fp32 into `out`, a buffer of at least num_rows_{a,g} x ld4(d) floats
     def num_rows_a(self, x: torch.Tensor) -> int:
-        raise NotImplementedError
+        return self.rows_a(x).n
 
     def num_rows_g(self, g: torch.Tensor) -> int:
-        raise NotImplementedError
+        return self.rows_g(g).n
 
     def write_rows_a(self, x: torch.Tensor, out: torch.Tensor) -> None:
-        raise NotImplementedError
+        rows = self.rows_a(_detached(x))
+        rows.write(out.data_ptr(), _cabi.ld4(rows.d), 1.0, None)
 
     def write_rows_g(self, g: torch.Tensor, out: torch.Tensor, grad_scale: float, loss_scale: int | None) -> None:
         """loss_scale: device pointer of a float the rows are divided by (the AMP loss scale), or None."""
-        raise NotImplementedError
+        rows = self.rows_g(_detached(g))
+        rows.write(out.data_ptr(), _cabi.ld4(rows.d), grad_scale, loss_scale)
+
+    @staticmethod
+    def _accumulate_rows(rows: FactorRows, acc: torch.Tensor, grad_scale: float, scratch, diagonal: bool) -> None:
+        """acc += the statistics of one call's rows without a direct statistic: the rows written in fp32 (ld = d) at
+        the start of the scratch buffer and the Linear statistics call on them at 1 / (n * grad_scale^2) (the column
+        sums of squares for a diagonal G)."""
+        n, d = rows.n, rows.d
+        if n == 0:
+            return
+        lib = _cabi.load()
+        row_bytes = (n * d * 4 + 255) // 256 * 256
+        need = (lib.kfac_factor_linear_diag_workspace_bytes(n, d) if diagonal
+                else lib.kfac_factor_linear_workspace_bytes(n, d, 0))
+        ptr = scratch.get(row_bytes + need, acc.device).data_ptr()
+        rows.write(ptr, d, 1.0, None)
+        ws = ptr + row_bytes if need else None
+        scale = 1.0 / (n * grad_scale * grad_scale)
+        f32 = _cabi.DTYPE_CODE[torch.float32]
+        if diagonal:
+            _cabi.check(lib.kfac_factor_linear_diag(ptr, f32, n, d, scale, acc.data_ptr(), ws, need,
+                                                    _cabi.stream_ptr()), 'kfac_factor_linear_diag')
+        else:
+            _cabi.check(lib.kfac_factor_linear(ptr, f32, n, d, 0, scale, acc.data_ptr(), ws, need, _cabi.stream_ptr()),
+                        'kfac_factor_linear')
 
 
 _NATIVE_INPUT_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
@@ -124,26 +181,19 @@ def _dtype_code(t: torch.Tensor) -> int:
         raise ValueError(f'unsupported activation/gradient dtype {t.dtype}') from None
 
 
-def _reduced_factor(write: Callable[[int, int], None], B: int, d: int, scale: float, acc: torch.Tensor, scratch,
-                    device: torch.device, diagonal: bool = False) -> None:
-    """K-FAC-reduce statistics of one call: `write(ptr, ld)` writes the B reduced rows (fp32, B x d, ld = d) at the
-    start of the scratch buffer, and the existing statistics call adds scale * rows^T rows to acc (the column sums of
-    squares for a diagonal G)."""
-    lib = _cabi.load()
-    row_bytes = (B * d * 4 + 255) // 256 * 256
-    need = (lib.kfac_factor_linear_diag_workspace_bytes(B, d) if diagonal
-            else lib.kfac_factor_linear_workspace_bytes(B, d, 0))
-    buf = (scratch.get(row_bytes + need, device) if scratch is not None
-           else torch.empty(row_bytes + need, dtype=torch.uint8, device=device))
-    rows = buf.data_ptr()
-    write(rows, d)
-    ws = rows + row_bytes if need else None
-    if diagonal:
-        _cabi.check(lib.kfac_factor_linear_diag(rows, _cabi.DTYPE_CODE[torch.float32], B, d, scale, acc.data_ptr(), ws,
-                                                need, _cabi.stream_ptr()), 'kfac_factor_linear_diag')
-    else:
-        _cabi.check(lib.kfac_factor_linear(rows, _cabi.DTYPE_CODE[torch.float32], B, d, 0, scale, acc.data_ptr(), ws,
-                                           need, _cabi.stream_ptr()), 'kfac_factor_linear')
+def _detached(t: torch.Tensor) -> torch.Tensor:
+    _cabi.require_device(t)
+    return t.detach()
+
+
+def _dense(t: torch.Tensor) -> torch.Tensor:
+    return t if t.is_contiguous() else t.contiguous()
+
+
+def _workspace(scratch, need: int, device: torch.device) -> int | None:
+    """Device pointer of `need` bytes of the scratch buffer (None for none)."""
+    ws = scratch.get(need, device)
+    return ws.data_ptr() if ws is not None else None
 
 
 class LinearModuleHelper(ModuleHelper):
@@ -171,79 +221,57 @@ class LinearModuleHelper(ModuleHelper):
         R = t.numel() // (B * t.size(-1))
         return (B, R) if R > 1 else None
 
-    def _write_reduced(self, t, side, scale, loss_scale, out_ptr, ld):
-        """The reduced rows of side 'a' (the mean of the R rows, ones column included) or 'g' (their sum / sqrt(R)),
-        times scale / *loss_scale."""
-        B, R = self._positions(t)
-        ones = int(self.has_bias()) if side == 'a' else 0
-        per = 1.0 / R if side == 'a' else 1.0 / math.sqrt(R)
-        _cabi.check(_cabi.load().kfac_reduce_rows_linear(t.data_ptr(), _dtype_code(t), B, R, t.size(-1), ones,
-                                                         scale * per, loss_scale, out_ptr, ld, _cabi.stream_ptr()),
-                    'kfac_reduce_rows_linear')
+    def rows_a(self, x):
+        return self._rows(x, 'a')
 
-    def _accumulate_reduced_g(self, g, acc, grad_scale, scratch, diagonal=False):
-        B = self._positions(g)[0]
-        _reduced_factor(lambda p, ld: self._write_reduced(g, 'g', 1.0, None, p, ld), B, g.size(-1),
-                        1.0 / (B * grad_scale * grad_scale), acc, scratch, g.device, diagonal=diagonal)
+    def rows_g(self, g):
+        return self._rows(g, 'g')
 
-    def accumulate_a(self, x, acc, scratch):
-        _cabi.require_device(x)
-        x = x.detach()
-        x = x if x.is_contiguous() else x.contiguous()
-        if self._positions(x) is not None:
-            _reduced_factor(lambda p, ld: self._write_reduced(x, 'a', 1.0, None, p, ld), x.size(0),
-                            x.size(-1) + int(self.has_bias()), 1.0 / x.size(0), acc, scratch, x.device)
-            return
-        feat = x.size(-1)
-        rows = x.numel() // feat
-        lib = _cabi.load()
-        need = lib.kfac_factor_linear_workspace_bytes(rows, feat, int(self.has_bias()))
-        ws = scratch.get(need, x.device) if need else None
-        _cabi.check(lib.kfac_factor_linear(x.data_ptr(), _dtype_code(x), rows, feat,
-                                           int(self.has_bias()), 1.0 / rows, acc.data_ptr(),
-                                           ws.data_ptr() if ws is not None else None, need,
-                                           _cabi.stream_ptr()), 'kfac_factor_linear')
-
-    def accumulate_g(self, g, acc, grad_scale, scratch=None):
-        _cabi.require_device(g)
-        g = g.detach()
-        g = g if g.is_contiguous() else g.contiguous()
-        if self.reduce and self._positions(g) is not None:     # (an embedding shares this method, never reduced)
-            return self._accumulate_reduced_g(g, acc, grad_scale, scratch)
-        feat = g.size(-1)
-        rows = g.numel() // feat
-        lib = _cabi.load()
-        need = lib.kfac_factor_linear_workspace_bytes(rows, feat, 0) if scratch is not None else 0
-        ws = scratch.get(need, g.device) if need else None
-        _cabi.check(lib.kfac_factor_linear(g.data_ptr(), _dtype_code(g), rows, feat, 0,
-                                           1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
-                                           ws.data_ptr() if ws is not None else None, need,
-                                           _cabi.stream_ptr()), 'kfac_factor_linear')
-
-    def num_rows_a(self, x):
-        pos = self._positions(x)
-        return pos[0] if pos is not None else x.numel() // x.size(-1)
-
-    num_rows_g = num_rows_a
-
-    def _write_rows(self, t, out, side, scale, loss_scale):
-        _cabi.require_device(t)
-        t = t.detach()
-        t = t if t.is_contiguous() else t.contiguous()
+    def _rows(self, t: torch.Tensor, side: str) -> FactorRows:
+        """The rows of one tap of side 'a' (ones column included) or 'g': every position, or under K-FAC-reduce the
+        mean of each example's R A rows and the sum of its R G rows divided by sqrt(R)."""
         feat = t.size(-1)
         ones = int(self.has_bias()) if side == 'a' else 0
-        if self._positions(t) is not None:
-            self._write_reduced(t, side, scale, loss_scale, out.data_ptr(), _cabi.ld4(feat + ones))
-            return
-        _cabi.check(_cabi.load().kfac_rows_linear(t.data_ptr(), _dtype_code(t), t.numel() // feat, feat, ones, scale,
-                                                  loss_scale, out.data_ptr(), _cabi.ld4(feat + ones),
-                                                  _cabi.stream_ptr()), 'kfac_rows_linear')
+        pos = self._positions(t)
+        if pos is not None:
+            B, R = pos
+            per = 1.0 / R if side == 'a' else 1.0 / math.sqrt(R)
 
-    def write_rows_a(self, x, out):
-        self._write_rows(x, out, 'a', 1.0, None)
+            def write_reduced(out, ld, grad_scale, loss_scale):
+                c = _dense(t)
+                _cabi.check(_cabi.load().kfac_reduce_rows_linear(c.data_ptr(), _dtype_code(c), B, R, feat, ones,
+                                                                 1.0 / grad_scale * per, loss_scale, out, ld,
+                                                                 _cabi.stream_ptr()), 'kfac_reduce_rows_linear')
+            return FactorRows(B, feat + ones, write_reduced)
+        rows = t.numel() // feat
 
-    def write_rows_g(self, g, out, grad_scale, loss_scale):
-        self._write_rows(g, out, 'g', 1.0 / grad_scale, loss_scale)
+        def write(out, ld, grad_scale, loss_scale):
+            c = _dense(t)
+            _cabi.check(_cabi.load().kfac_rows_linear(c.data_ptr(), _dtype_code(c), rows, feat, ones,
+                                                      1.0 / grad_scale, loss_scale, out, ld, _cabi.stream_ptr()),
+                        'kfac_rows_linear')
+
+        if side == 'g' and self.diagonal_g:
+            def direct(acc, grad_scale, scratch):
+                if rows == 0:
+                    return
+                lib = _cabi.load()
+                c = _dense(t)
+                need = lib.kfac_factor_linear_diag_workspace_bytes(rows, feat)
+                _cabi.check(lib.kfac_factor_linear_diag(c.data_ptr(), _dtype_code(c), rows, feat,
+                                                        1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
+                                                        _workspace(scratch, need, c.device), need,
+                                                        _cabi.stream_ptr()), 'kfac_factor_linear_diag')
+        else:
+            def direct(acc, grad_scale, scratch):
+                lib = _cabi.load()
+                c = _dense(t)
+                need = lib.kfac_factor_linear_workspace_bytes(rows, feat, ones)
+                _cabi.check(lib.kfac_factor_linear(c.data_ptr(), _dtype_code(c), rows, feat, ones,
+                                                   1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
+                                                   _workspace(scratch, need, c.device), need, _cabi.stream_ptr()),
+                            'kfac_factor_linear')
+        return FactorRows(rows, feat + ones, write, direct)
 
 
 class Conv2dModuleHelper(ModuleHelper):
@@ -274,100 +302,74 @@ class Conv2dModuleHelper(ModuleHelper):
         B, _, H, W, kh, kw, sh, sw, ph, pw = geo
         return ((H + 2 * ph - kh) // sh + 1) * ((W + 2 * pw - kw) // sw + 1)
 
-    # K-FAC-reduce (S = Ho * Wo > 1): one row per example, the mean of its S A rows and the sum of its S G rows divided
-    # by sqrt(S), the rows carrying the 1/S of the expand rows: scale 1/S^2 (A) and S^-3/2 (G) on the plain sums
-    def _write_reduced_a(self, x, geo, out_ptr, ld):
-        S = self._spatial(geo)
-        _cabi.check(_cabi.load().kfac_reduce_rows_conv2d_input(x.data_ptr(), _dtype_code(x), *geo, int(self.has_bias()),
-                                                               1.0 / (float(S) * S), out_ptr, ld, _cabi.stream_ptr()),
-                    'kfac_reduce_rows_conv2d_input')
-
-    def _write_reduced_g(self, g, scale, loss_scale, out_ptr, ld):
-        B, Cc, Ho, Wo = g.shape
-        _cabi.check(_cabi.load().kfac_reduce_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, Ho, Wo,
-                                                                 scale / float(Ho * Wo) ** 1.5, loss_scale, out_ptr,
-                                                                 ld, _cabi.stream_ptr()),
-                    'kfac_reduce_rows_conv2d_gradout')
-
-    def accumulate_a(self, x, acc, scratch):
-        _cabi.require_device(x)
-        x = x.detach()
-        x = x if x.is_contiguous() else x.contiguous()
+    def rows_a(self, x):
         geo = self._geometry(x)
-        B, Cc, H, W, kh, kw, sh, sw, ph, pw = geo
-        Ho, Wo = (H + 2 * ph - kh) // sh + 1, (W + 2 * pw - kw) // sw + 1
-        S = Ho * Wo
-        if self.reduce and S > 1:
-            _reduced_factor(lambda p, ld: self._write_reduced_a(x, geo, p, ld), B, self.a_factor_shape[0], 1.0 / B,
-                            acc, scratch, x.device)
-            return
-        # rows = B*S, features scaled by 1/S  ->  scale = 1/(B*S) * 1/S^2   (modules.py:170-178)
-        scale = 1.0 / (float(B) * float(S) ** 3)
+        return _conv_input_rows(self, x, 'conv2d_input', geo, (), geo[0], self._spatial(geo), geo[1] * geo[4] * geo[5])
+
+    def rows_g(self, g):
+        return _conv_gradout_rows(g, *g.shape, self.reduce)
+
+
+# The rows of a convolution (modules.py:170-192): the B * S output positions, the A and G rows scaled by 1/S, so the
+# statistics are the plain sums scaled by 1/(B*S) * 1/S^2.  Under K-FAC-reduce (S > 1) one row per example, the mean
+# of its S A rows and the sum of its S G rows divided by sqrt(S), the rows carrying the 1/S of the expand rows: scale
+# 1/S^2 (A) and S^-3/2 (G) on the plain window sums.
+def _conv_input_rows(helper: ModuleHelper, x: torch.Tensor, entry: str, geo: tuple, ws_args: tuple, B: int,
+                     S: int, patch: int) -> FactorRows:
+    """A rows of a convolution (`patch` = C_in * taps features before the ones column) through the native entries
+    kfac_factor_{entry}, kfac_rows_{entry} and kfac_reduce_rows_{entry}, which take the geometry arguments `geo` (and
+    `ws_args` after the ones column in the workspace query)."""
+    ones = int(helper.has_bias())
+    d = patch + ones
+    if helper.reduce and S > 1:
+        def write_reduced(out, ld, grad_scale, loss_scale):
+            c, fn = _dense(x), f'kfac_reduce_rows_{entry}'
+            _cabi.check(getattr(_cabi.load(), fn)(c.data_ptr(), _dtype_code(c), *geo, ones, 1.0 / (float(S) * S),
+                                                  out, ld, _cabi.stream_ptr()), fn)
+        return FactorRows(B, d, write_reduced)
+
+    def write(out, ld, grad_scale, loss_scale):
+        c, fn = _dense(x), f'kfac_rows_{entry}'
+        _cabi.check(getattr(_cabi.load(), fn)(c.data_ptr(), _dtype_code(c), *geo, ones, 1.0 / S, out, ld,
+                                              _cabi.stream_ptr()), fn)
+
+    def direct(acc, grad_scale, scratch):
         lib = _cabi.load()
-        ones = int(self.has_bias())
-        need = lib.kfac_factor_conv2d_input_workspace_bytes(*geo, ones)
-        ws = scratch.get(need, x.device)
-        _cabi.check(lib.kfac_factor_conv2d_input(
-            x.data_ptr(), _dtype_code(x), *geo, ones, scale, acc.data_ptr(),
-            ws.data_ptr() if need else None, need, _cabi.stream_ptr()), 'kfac_factor_conv2d_input')
+        c, fn = _dense(x), f'kfac_factor_{entry}'
+        need = getattr(lib, fn + '_workspace_bytes')(*geo, ones, *ws_args)
+        # ws_bytes = need, not the scratch buffer's size: the chunking, and so the bits, depend on it
+        _cabi.check(getattr(lib, fn)(c.data_ptr(), _dtype_code(c), *geo, ones, 1.0 / (float(B) * float(S) ** 3),
+                                     acc.data_ptr(), _workspace(scratch, need, c.device), need, _cabi.stream_ptr()), fn)
+    return FactorRows(B * S, d, write, direct)
 
-    def accumulate_g(self, g, acc, grad_scale, scratch=None):
-        _cabi.require_device(g)
-        g = g.detach()
-        g = g if g.is_contiguous() else g.contiguous()
-        B, Cc, Ho, Wo = g.shape
-        S = Ho * Wo
-        if self.reduce and S > 1:
-            _reduced_factor(lambda p, ld: self._write_reduced_g(g, 1.0, None, p, ld), B, Cc,
-                            1.0 / (B * grad_scale * grad_scale), acc, scratch, g.device)
-            return
-        scale = 1.0 / (float(B) * float(S) ** 3 * grad_scale * grad_scale)
+
+def _conv_gradout_rows(g: torch.Tensor, B: int, Cc: int, Ho: int, Wo: int, reduce: bool) -> FactorRows:
+    """G rows of a convolution whose output gradient g is read as (B, Cc, Ho, Wo)."""
+    S = Ho * Wo
+    if reduce and S > 1:
+        def write_reduced(out, ld, grad_scale, loss_scale):
+            c = _dense(g)
+            _cabi.check(_cabi.load().kfac_reduce_rows_conv2d_gradout(c.data_ptr(), _dtype_code(c), B, Cc, Ho, Wo,
+                                                                     1.0 / grad_scale / float(S) ** 1.5, loss_scale,
+                                                                     out, ld, _cabi.stream_ptr()),
+                        'kfac_reduce_rows_conv2d_gradout')
+        return FactorRows(B, Cc, write_reduced)
+
+    def write(out, ld, grad_scale, loss_scale):
+        c = _dense(g)
+        _cabi.check(_cabi.load().kfac_rows_conv2d_gradout(c.data_ptr(), _dtype_code(c), B, Cc, Ho, Wo,
+                                                          1.0 / (float(S) * grad_scale), loss_scale, out, ld,
+                                                          _cabi.stream_ptr()), 'kfac_rows_conv2d_gradout')
+
+    def direct(acc, grad_scale, scratch):
         lib = _cabi.load()
-        need = lib.kfac_factor_conv2d_gradout_workspace_bytes(B, Cc, Ho, Wo) if scratch is not None else 0
-        ws = scratch.get(need, g.device) if need else None
-        _cabi.check(lib.kfac_factor_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, Ho, Wo,
-                                                   scale, acc.data_ptr(),
-                                                   ws.data_ptr() if ws is not None else None, need,
-                                                   _cabi.stream_ptr()),
-                    'kfac_factor_conv2d_gradout')
-
-    def num_rows_a(self, x):
-        geo = self._geometry(x)
-        S = self._spatial(geo)
-        return geo[0] if self.reduce and S > 1 else geo[0] * S
-
-    def num_rows_g(self, g):
-        S = g.size(2) * g.size(3)
-        return g.size(0) if self.reduce and S > 1 else g.size(0) * S
-
-    def write_rows_a(self, x, out):
-        _cabi.require_device(x)
-        x = x.detach()
-        x = x if x.is_contiguous() else x.contiguous()
-        geo = self._geometry(x)
-        B, Cc, H, W, kh, kw, sh, sw, ph, pw = geo
-        S = ((H + 2 * ph - kh) // sh + 1) * ((W + 2 * pw - kw) // sw + 1)
-        ones = int(self.has_bias())
-        if self.reduce and S > 1:
-            self._write_reduced_a(x, geo, out.data_ptr(), _cabi.ld4(Cc * kh * kw + ones))
-            return
-        # rows scaled by 1/S, the ones column included (modules.py:170-178)
-        _cabi.check(_cabi.load().kfac_rows_conv2d_input(x.data_ptr(), _dtype_code(x), *geo, ones, 1.0 / S, out.data_ptr(),
-                                                        _cabi.ld4(Cc * kh * kw + ones), _cabi.stream_ptr()),
-                    'kfac_rows_conv2d_input')
-
-    def write_rows_g(self, g, out, grad_scale, loss_scale):
-        _cabi.require_device(g)
-        g = g.detach()
-        g = g if g.is_contiguous() else g.contiguous()
-        B, Cc, Ho, Wo = g.shape
-        if self.reduce and Ho * Wo > 1:
-            self._write_reduced_g(g, 1.0 / grad_scale, loss_scale, out.data_ptr(), _cabi.ld4(Cc))
-            return
-        _cabi.check(_cabi.load().kfac_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, Ho, Wo,
-                                                          1.0 / (float(Ho * Wo) * grad_scale), loss_scale,
-                                                          out.data_ptr(), _cabi.ld4(Cc), _cabi.stream_ptr()),
-                    'kfac_rows_conv2d_gradout')
+        c = _dense(g)
+        need = lib.kfac_factor_conv2d_gradout_workspace_bytes(B, Cc, Ho, Wo)
+        _cabi.check(lib.kfac_factor_conv2d_gradout(c.data_ptr(), _dtype_code(c), B, Cc, Ho, Wo,
+                                                   1.0 / (float(B) * float(S) ** 3 * grad_scale * grad_scale),
+                                                   acc.data_ptr(), _workspace(scratch, need, c.device), need,
+                                                   _cabi.stream_ptr()), 'kfac_factor_conv2d_gradout')
+    return FactorRows(B * S, Cc, write, direct)
 
 
 # Largest im2col chunk of a Conv1d / Conv3d factor call: a video layer's im2col is tens of times its input (r2plus1d_18
@@ -478,91 +480,19 @@ class ConvNdModuleHelper(ModuleHelper):
             self._extents = (self._extents + [out])[-8:]
         return geo, math.prod(out)
 
-    def _gradout(self, g: torch.Tensor) -> tuple[torch.Tensor, int, int, int]:
-        """(batched contiguous g, B, C, S); the extent must be one an A call of this window computed."""
-        _cabi.require_device(g)
-        g = self._batched(g.detach())
-        g = g if g.is_contiguous() else g.contiguous()
+    def rows_a(self, x):
+        geo, S = self._prepared_geometry(x)
+        return _conv_input_rows(self, x, self.entry, (C.byref(geo),), (CONV_ND_WORKSPACE_BYTES,), geo.batch, S,
+                                geo.C * math.prod(self.module.kernel_size))
+
+    def rows_g(self, g):
+        """The output gradient read as (B, C, 1, S); its extent must be one an A call of this window computed."""
+        g = self._batched(g)
         out = tuple(g.shape[2:])
         if self._extents and out not in self._extents:
             raise ValueError(f'{self.module.__class__.__name__}: output gradient extent {out} does not match the '
                              f'output extent {self._extents[-1]} computed from the input and the padding')
-        return g, g.size(0), g.size(1), math.prod(out)
-
-    def _write_reduced_a(self, x, geo, S, out_ptr, ld):
-        fn = f'kfac_reduce_rows_{self.entry}'
-        _cabi.check(getattr(_cabi.load(), fn)(x.data_ptr(), _dtype_code(x), C.byref(geo), int(self.has_bias()),
-                                              1.0 / (float(S) * S), out_ptr, ld, _cabi.stream_ptr()), fn)
-
-    def _write_reduced_g(self, g, B, Cc, S, scale, loss_scale, out_ptr, ld):
-        _cabi.check(_cabi.load().kfac_reduce_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, 1, S,
-                                                                 scale / float(S) ** 1.5, loss_scale, out_ptr, ld,
-                                                                 _cabi.stream_ptr()),
-                    'kfac_reduce_rows_conv2d_gradout')
-
-    def accumulate_a(self, x, acc, scratch):
-        geo, S = self._prepared_geometry(x)
-        B = geo.batch
-        if self.reduce and S > 1:
-            _reduced_factor(lambda p, ld: self._write_reduced_a(x, geo, S, p, ld), B, self.a_factor_shape[0], 1.0 / B,
-                            acc, scratch, x.device)
-            return
-        # rows = B*S, features scaled by 1/S  ->  scale = 1/(B*S) * 1/S^2   (modules.py:170-178)
-        scale = 1.0 / (float(B) * float(S) ** 3)
-        lib = _cabi.load()
-        ones = int(self.has_bias())
-        fn = f'kfac_factor_{self.entry}'
-        need = getattr(lib, fn + '_workspace_bytes')(C.byref(geo), ones, CONV_ND_WORKSPACE_BYTES)
-        ws = scratch.get(need, x.device)
-        # ws_bytes = need, not the scratch buffer's size: the chunking, and so the bits, depend on it
-        _cabi.check(getattr(lib, fn)(x.data_ptr(), _dtype_code(x), C.byref(geo), ones, scale, acc.data_ptr(),
-                                     ws.data_ptr() if need else None, need, _cabi.stream_ptr()), fn)
-
-    def accumulate_g(self, g, acc, grad_scale, scratch=None):
-        g, B, Cc, S = self._gradout(g)
-        if self.reduce and S > 1:
-            _reduced_factor(lambda p, ld: self._write_reduced_g(g, B, Cc, S, 1.0, None, p, ld), B, Cc,
-                            1.0 / (B * grad_scale * grad_scale), acc, scratch, g.device)
-            return
-        scale = 1.0 / (float(B) * float(S) ** 3 * grad_scale * grad_scale)
-        lib = _cabi.load()
-        need = lib.kfac_factor_conv2d_gradout_workspace_bytes(B, Cc, 1, S) if scratch is not None else 0
-        ws = scratch.get(need, g.device) if need else None
-        _cabi.check(lib.kfac_factor_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, 1, S, scale, acc.data_ptr(),
-                                                   ws.data_ptr() if ws is not None else None, need,
-                                                   _cabi.stream_ptr()), 'kfac_factor_conv2d_gradout')
-
-    def num_rows_a(self, x):
-        geo, out = self._geometry(x.shape)
-        S = math.prod(out)
-        return geo.batch if self.reduce and S > 1 else geo.batch * S
-
-    def num_rows_g(self, g):
-        B = g.size(0) if g.dim() == self.nd + 2 else 1
-        S = math.prod(g.shape[-self.nd:])
-        return B if self.reduce and S > 1 else B * S
-
-    def write_rows_a(self, x, out):
-        geo, S = self._prepared_geometry(x)
-        ones = int(self.has_bias())
-        ld = _cabi.ld4(self.a_factor_shape[0])
-        if self.reduce and S > 1:
-            self._write_reduced_a(x, geo, S, out.data_ptr(), ld)
-            return
-        # rows scaled by 1/S, the ones column included (modules.py:170-178)
-        fn = f'kfac_rows_{self.entry}'
-        _cabi.check(getattr(_cabi.load(), fn)(x.data_ptr(), _dtype_code(x), C.byref(geo), ones, 1.0 / S,
-                                              out.data_ptr(), ld, _cabi.stream_ptr()), fn)
-
-    def write_rows_g(self, g, out, grad_scale, loss_scale):
-        g, B, Cc, S = self._gradout(g)
-        if self.reduce and S > 1:
-            self._write_reduced_g(g, B, Cc, S, 1.0 / grad_scale, loss_scale, out.data_ptr(), _cabi.ld4(Cc))
-            return
-        _cabi.check(_cabi.load().kfac_rows_conv2d_gradout(g.data_ptr(), _dtype_code(g), B, Cc, 1, S,
-                                                          1.0 / (float(S) * grad_scale), loss_scale, out.data_ptr(),
-                                                          _cabi.ld4(Cc), _cabi.stream_ptr()),
-                    'kfac_rows_conv2d_gradout')
+        return _conv_gradout_rows(g, g.size(0), g.size(1), 1, math.prod(out), self.reduce)
 
 
 class ConvTransposeModuleHelper(ConvNdModuleHelper):
@@ -631,14 +561,14 @@ class ConvTransposeModuleHelper(ConvNdModuleHelper):
         return x if x.is_contiguous() else x.contiguous()
 
 
-class EmbeddingModuleHelper(ModuleHelper):
+class EmbeddingModuleHelper(LinearModuleHelper):
     """torch.nn.Embedding (an extension beyond the reference, opt-in through `precondition_embeddings`).
 
     An embedding is a Linear layer whose input rows are one-hot vectors e_idx, so A = (1/N) sum_r e_r e_r^T is
     DIAGONAL: the token frequencies counts / N, kept as a vector of V floats (`a_factor_shape` is (V,)).  Every
     index position is one row, `padding_idx` positions included (their gradient row is zero, so their P row is
     zero), which keeps N = idx.numel() known on the host.  G is formed from the grad-output rows exactly like a
-    Linear layer's.  The gradient and P use the weight's own layout (V x d)."""
+    Linear layer's (never K-FAC-reduced).  The gradient and P use the weight's own layout (V x d)."""
 
     diagonal_a = True
 
@@ -655,55 +585,36 @@ class EmbeddingModuleHelper(ModuleHelper):
         return False
 
     def accumulate_a(self, x, acc, scratch):
-        _cabi.require_device(x)
+        """acc += the index histogram of one call / N."""
+        x = _detached(x)
         try:
             code = _cabi.INDEX_DTYPE_CODE[x.dtype]
         except KeyError:
             raise ValueError(f'unsupported embedding index dtype {x.dtype}') from None
-        x = x.detach()
-        x = x if x.is_contiguous() else x.contiguous()
+        x = _dense(x)
         V = self.module.num_embeddings
         n = x.numel()
         if n == 0:
             return
         lib = _cabi.load()
         need = lib.kfac_factor_embedding_workspace_bytes(V)
-        ws = scratch.get(need, x.device)
-        _cabi.check(lib.kfac_factor_embedding(x.data_ptr(), code, n, V, 1.0 / n, acc.data_ptr(), ws.data_ptr(), need,
-                                              _cabi.stream_ptr()), 'kfac_factor_embedding')
-
-    accumulate_g = LinearModuleHelper.accumulate_g
+        _cabi.check(lib.kfac_factor_embedding(x.data_ptr(), code, n, V, 1.0 / n, acc.data_ptr(),
+                                              _workspace(scratch, need, x.device), need, _cabi.stream_ptr()),
+                    'kfac_factor_embedding')
 
 
 class DiagonalGLinearModuleHelper(LinearModuleHelper):
     """torch.nn.Linear with G approximated by its diagonal (an extension beyond the reference, opt-in through
     `diagonal_g_layers`), for layers with too many outputs for a dense G: an LM head of V = 50257 outputs would need
     a V x V factor (10 GB) beyond the eigensolver.  diag(G) = (1/N) sum_r g_r^2 is kept as a vector of V floats
-    (`g_factor_shape` is (V,)); it is its own eigendecomposition (Qg = I).  A, the gradient and P are those of a
-    Linear layer."""
+    (`g_factor_shape` is (V,)); it is its own eigendecomposition (Qg = I).  A, the gradient, P and the G rows are
+    those of a Linear layer; `diagonal_g` selects the diagonal statistics of the G rows."""
 
     diagonal_g = True
 
     @property
     def g_factor_shape(self):
         return (self.module.weight.size(0),)
-
-    def accumulate_g(self, g, acc, grad_scale, scratch=None):
-        _cabi.require_device(g)
-        g = g.detach()
-        g = g if g.is_contiguous() else g.contiguous()
-        if self._positions(g) is not None:      # diag(G) of the reduced rows
-            return self._accumulate_reduced_g(g, acc, grad_scale, scratch, diagonal=True)
-        feat = g.size(-1)
-        rows = g.numel() // feat
-        if rows == 0:
-            return
-        lib = _cabi.load()
-        need = lib.kfac_factor_linear_diag_workspace_bytes(rows, feat)
-        ws = scratch.get(need, g.device)
-        _cabi.check(lib.kfac_factor_linear_diag(g.data_ptr(), _dtype_code(g), rows, feat,
-                                                1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
-                                                ws.data_ptr(), need, _cabi.stream_ptr()), 'kfac_factor_linear_diag')
 
 
 class NormModuleHelper(ModuleHelper):
@@ -861,69 +772,41 @@ class SequenceFirstLinearHelper(LinearModuleHelper):
             return None
         return (t.size(1), t.size(0))
 
-    def _write_reduced(self, t, side, scale, loss_scale, out_ptr, ld):
-        B, R = self._positions(t)
-        if t.stride(-1) != 1:
-            t = t.contiguous()
+    def _rows(self, t, side):
+        """The rows of one tap, read in place through the strided entry points."""
+        feat = t.size(-1)
         ones = int(self.has_bias()) if side == 'a' else 0
-        per = 1.0 / R if side == 'a' else 1.0 / math.sqrt(R)
-        _cabi.check(_cabi.load().kfac_reduce_rows_linear_strided(
-            t.data_ptr(), _dtype_code(t), B, R, t.size(-1), t.stride(1), t.stride(0), ones, scale * per, loss_scale,
-            out_ptr, ld, _cabi.stream_ptr()), 'kfac_reduce_rows_linear_strided')
+        pos = self._positions(t)
+        if pos is not None:
+            B, R = pos
+            per = 1.0 / R if side == 'a' else 1.0 / math.sqrt(R)
 
-    def _accumulate(self, t, acc, ones, grad_scale, scratch):
-        r, ld = _strided_rows(t, ordered=False)
-        rows, feat = r.shape
-        if rows == 0:
-            return
-        lib = _cabi.load()
-        need = lib.kfac_factor_linear_strided_workspace_bytes(rows, feat, ld, ones)
-        ws = scratch.get(need, t.device) if (need and scratch is not None) else None
-        _cabi.check(lib.kfac_factor_linear_strided(r.data_ptr(), _dtype_code(r), rows, feat, ld, ones,
-                                                   1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
-                                                   ws.data_ptr() if ws is not None else None,
-                                                   need if ws is not None else 0, _cabi.stream_ptr()),
-                    'kfac_factor_linear_strided')
+            def write_reduced(out, ld, grad_scale, loss_scale):
+                c = t if t.stride(-1) == 1 else t.contiguous()
+                _cabi.check(_cabi.load().kfac_reduce_rows_linear_strided(
+                    c.data_ptr(), _dtype_code(c), B, R, feat, c.stride(1), c.stride(0), ones, 1.0 / grad_scale * per,
+                    loss_scale, out, ld, _cabi.stream_ptr()), 'kfac_reduce_rows_linear_strided')
+            return FactorRows(B, feat + ones, write_reduced)
 
-    def accumulate_a(self, x, acc, scratch):
-        _cabi.require_device(x)
-        x = x.detach()
-        if self._positions(x) is not None:
-            _reduced_factor(lambda p, ld: self._write_reduced(x, 'a', 1.0, None, p, ld), x.size(1),
-                            x.size(-1) + int(self.has_bias()), 1.0 / x.size(1), acc, scratch, x.device)
-            return
-        self._accumulate(x, acc, int(self.has_bias()), 1.0, scratch)
+        def write(out, ld, grad_scale, loss_scale):
+            # the A and G rows of EKFAC are paired row by row: both in the (L, B) order of the taps
+            r, ldr = _strided_rows(t, ordered=True)
+            _cabi.check(_cabi.load().kfac_rows_linear_strided(r.data_ptr(), _dtype_code(r), r.size(0), feat, ldr,
+                                                              ones, 1.0 / grad_scale, loss_scale, out, ld,
+                                                              _cabi.stream_ptr()), 'kfac_rows_linear_strided')
 
-    def accumulate_g(self, g, acc, grad_scale, scratch=None):
-        _cabi.require_device(g)
-        g = g.detach()
-        if self._positions(g) is not None:
-            B = g.size(1)
-            _reduced_factor(lambda p, ld: self._write_reduced(g, 'g', 1.0, None, p, ld), B, g.size(-1),
-                            1.0 / (B * grad_scale * grad_scale), acc, scratch, g.device)
-            return
-        self._accumulate(g, acc, 0, grad_scale, scratch)
-
-    def num_rows_a(self, x):
-        pos = self._positions(x)
-        return pos[0] if pos is not None else x.numel() // x.size(-1)
-
-    num_rows_g = num_rows_a
-
-    def _write_rows(self, t, out, side, scale, loss_scale):
-        _cabi.require_device(t)
-        t = t.detach()
-        ones = int(self.has_bias()) if side == 'a' else 0
-        if self._positions(t) is not None:
-            self._write_reduced(t, side, scale, loss_scale, out.data_ptr(), _cabi.ld4(t.size(-1) + ones))
-            return
-        # the A and G rows of EKFAC are paired row by row: both in the (L, B) order of the taps
-        r, ld = _strided_rows(t, ordered=True)
-        rows, feat = r.shape
-        _cabi.check(_cabi.load().kfac_rows_linear_strided(r.data_ptr(), _dtype_code(r), rows, feat, ld, ones, scale,
-                                                          loss_scale, out.data_ptr(), _cabi.ld4(feat + ones),
-                                                          _cabi.stream_ptr()), 'kfac_rows_linear_strided')
-
+        def direct(acc, grad_scale, scratch):
+            r, ldr = _strided_rows(t, ordered=False)
+            rows = r.size(0)
+            if rows == 0:
+                return
+            lib = _cabi.load()
+            need = lib.kfac_factor_linear_strided_workspace_bytes(rows, feat, ldr, ones)
+            _cabi.check(lib.kfac_factor_linear_strided(r.data_ptr(), _dtype_code(r), rows, feat, ldr, ones,
+                                                       1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
+                                                       _workspace(scratch, need, r.device), need, _cabi.stream_ptr()),
+                        'kfac_factor_linear_strided')
+        return FactorRows(t.numel() // feat, feat + ones, write, direct)
 
 
 class AttentionProjectionHelper(SequenceFirstLinearHelper):
@@ -1083,52 +966,16 @@ class RecurrentSubLayerHelper(SequenceFirstLinearHelper):
             _cabi.check(lib.kfac_rows_sequence(C.byref(src), _dtype_code(t), feat, ones, scale, loss_scale, out_ptr,
                                                ld, _cabi.stream_ptr()), 'kfac_rows_sequence')
 
-    def _accumulate_tap(self, t, tap, side, acc, grad_scale, scratch):
+    def _rows(self, t, side):
+        """The rows of the tap `tap_a` / `tap_g` describes."""
+        tap = self.tap_a if side == 'a' else self.tap_g
+        if not self._native(tap):
+            return super()._rows(self._first(t, tap), side)
         reduced = self._reduced(tap)
         n = tap.B if reduced else t.numel() // t.size(-1)
-        if n == 0:
-            return
         d = (self.a_factor_shape if side == 'a' else self.g_factor_shape)[0]
-        _reduced_factor(lambda p, ld: self._sequence_call(t, tap, side, 1.0, None, p, ld, reduced), n, d,
-                        1.0 / (n * grad_scale * grad_scale), acc, scratch, t.device)
-
-    def accumulate_a(self, x, acc, scratch):
-        _cabi.require_device(x)
-        x, tap = x.detach(), self.tap_a
-        if self._native(tap):
-            return self._accumulate_tap(x, tap, 'a', acc, 1.0, scratch)
-        super().accumulate_a(self._first(x, tap), acc, scratch)
-
-    def accumulate_g(self, g, acc, grad_scale, scratch=None):
-        _cabi.require_device(g)
-        g, tap = g.detach(), self.tap_g
-        if self._native(tap):
-            return self._accumulate_tap(g, tap, 'g', acc, grad_scale, scratch)
-        super().accumulate_g(self._first(g, tap), acc, grad_scale, scratch)
-
-    def num_rows_a(self, x):
-        tap = self.tap_a
-        return tap.B if self._reduced(tap) else x.numel() // x.size(-1)
-
-    def num_rows_g(self, g):
-        tap = self.tap_g
-        return tap.B if self._reduced(tap) else g.numel() // g.size(-1)
-
-    def write_rows_a(self, x, out):
-        tap = self.tap_a
-        if self._native(tap):
-            _cabi.require_device(x)
-            return self._sequence_call(x.detach(), tap, 'a', 1.0, None, out.data_ptr(),
-                                       _cabi.ld4(self.a_factor_shape[0]), self._reduced(tap))
-        self._write_rows(self._first(x, tap), out, 'a', 1.0, None)
-
-    def write_rows_g(self, g, out, grad_scale, loss_scale):
-        tap = self.tap_g
-        if self._native(tap):
-            _cabi.require_device(g)
-            return self._sequence_call(g.detach(), tap, 'g', 1.0 / grad_scale, loss_scale, out.data_ptr(),
-                                       _cabi.ld4(self.g_factor_shape[0]), self._reduced(tap))
-        self._write_rows(self._first(g, tap), out, 'g', 1.0 / grad_scale, loss_scale)
+        return FactorRows(n, d, lambda out, ld, grad_scale, loss_scale: self._sequence_call(
+            t, tap, side, 1.0 / grad_scale, loss_scale, out, ld, reduced))
 
 
 LINEAR_TYPES: tuple[type, ...] = (torch.nn.Linear,)
