@@ -226,6 +226,28 @@ int kfac_factor_ema_diag_guarded(const kfac_ema_item* items, int count, float al
 size_t kfac_factor_linear_diag_workspace_bytes(int64_t rows, int features);
 int kfac_factor_linear_diag(const void* x, int dtype, int64_t rows, int features, float scale,
                             float* acc, void* ws, size_t ws_bytes, void* stream);
+/* Diagonal-A layers (an extension beyond the reference, opt-in): a Linear or convolution layer with
+ * more inputs than the eigensolver takes keeps its A factor as the vector diag(A), bias entry last.
+ * kfac_factor_linear_diag_ones: kfac_factor_linear_diag with the ones column of kfac_factor_linear
+ * appended when append_ones: acc has features + append_ones entries, and acc[features] += scale *
+ * rows (the squares of the ones column).  Same workspace query, chunking and bits on the features
+ * as kfac_factor_linear_diag (which is this call with append_ones = 0). */
+int kfac_factor_linear_diag_ones(const void* x, int dtype, int64_t rows, int features,
+                                 int append_ones, float scale, float* acc, void* ws,
+                                 size_t ws_bytes, void* stream);
+/* kfac_factor_conv_input_diag: acc (d = C * kd * kh * kw + append_ones floats) += scale * the
+ * diagonal of the X^T X kfac_factor_conv_input accumulates for the same geometry, without the
+ * im2col: acc[(c, taps)] += scale * sum over the im2col rows of row^2, and acc[d - 1] += scale *
+ * batch * Do * Ho * Wo for the ones column.  Each (b, c) volume is read once from HBM; the window
+ * sums of its squares over the output lattice are formed from it (a kernel window of at most 2048
+ * taps, else KFAC_ERR_BAD_ARG).  x in fp32, fp16 or bf16.  Deterministic and without a host sync:
+ * every example's sums go to ws as fp32 partials (batch x (d - append_ones) floats,
+ * kfac_factor_conv_input_diag_workspace_bytes), and a second launch adds them in example order in
+ * fp64.  No floating-point atomics. */
+size_t kfac_factor_conv_input_diag_workspace_bytes(const kfac_conv_geometry* geom);
+int kfac_factor_conv_input_diag(const void* x, int dtype, const kfac_conv_geometry* geom,
+                                int append_ones, float scale, float* acc, void* ws,
+                                size_t ws_bytes, void* stream);
 /* dst[i] = src[i] for n floats; ORs 2 (the non-finite bit of the kfac_eigh_batched status word)
  * into the DEVICE int *status when an entry is not finite or exceeds 1e15 in magnitude.  The
  * snapshot of a diagonal factor at an inverse step, checked like a decomposed factor. */
@@ -369,8 +391,22 @@ int kfac_transpose(const float* src, int ld_src, float* dst, int ld_dst, int row
  * wgrad is (a = V, g = d), bgrad NULL, qg = M, qgT = M^T (ld = ldqg), da = f, dh = h (V floats each),
  * dg = mu (d floats), P (V x ldp, ldp >= d).  `method` and `damping` of the call are not used; the
  * two GEMMs join the grouped launches, the division is one more launch over all tied items (the
- * engines' epilogues are left as they are), and the other items' results do not depend on tied items. */
-enum kfac_item_kind { KFAC_ITEM_DENSE = 0, KFAC_ITEM_EMBEDDING = 1, KFAC_ITEM_DIAG_G = 2, KFAC_ITEM_TIED = 3 };
+ * engines' epilogues are left as they are), and the other items' results do not depend on tied items.
+ * Diagonal-A items (kind = KFAC_ITEM_DIAG_A): a Linear or convolution layer whose A factor is kept
+ * as its diagonal.  wgrad (g, a - has_bias) and bgrad as for a dense item (fp32, fp16 or bf16; no
+ * wgrad_taps), da the diagonal A factor (a floats, bias entry last; its own eigenvalues), P (g x ldp,
+ * ldp >= a) in the dense layout:
+ *   EIGEN  : P = Qg [(Qg^T grad) / (dg x da + damping)]       (qg, qgT, dg; dgda is not used)
+ *   INVERSE: P = Ginv grad diag(1 / (da + damping))            (g_inv)
+ * qa, qaT, a_inv, dgda, ldqa and ld_dgda are ignored.  The gradient is gathered transposed (one
+ * more launch per item), and the products are those of an embedding item on grad^T (the division
+ * is the EPI_DIV_OUTER epilogue of the first product), the last one formed transposed so that P is
+ * g x a.  The two (one) GEMMs join the grouped launches; the last one is split into chains of at
+ * most 512 for g > 1024 (eigen), and its peer stores give the bits of the local P.  The other
+ * items' results do not depend on diagonal-A items. */
+enum kfac_item_kind {
+  KFAC_ITEM_DENSE = 0, KFAC_ITEM_EMBEDDING = 1, KFAC_ITEM_DIAG_G = 2, KFAC_ITEM_TIED = 3, KFAC_ITEM_DIAG_A = 4
+};
 typedef struct kfac_precond_item {
   const void* wgrad; /* (g, a - has_bias) */
   const void* bgrad; /* (g) or NULL */

@@ -23,7 +23,7 @@ KFAC_EKFAC_KEEP, KFAC_EKFAC_EMA, KFAC_EKFAC_RESET, KFAC_EKFAC_SEED = 0, 1, 2, 3
 
 KFAC_EIGH_MAX_N = 8192   # largest factor dimension the eigensolver takes
 
-KFAC_ITEM_DENSE, KFAC_ITEM_EMBEDDING, KFAC_ITEM_DIAG_G, KFAC_ITEM_TIED = 0, 1, 2, 3
+KFAC_ITEM_DENSE, KFAC_ITEM_EMBEDDING, KFAC_ITEM_DIAG_G, KFAC_ITEM_TIED, KFAC_ITEM_DIAG_A = 0, 1, 2, 3, 4
 
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 INDEX_DTYPE_CODE = {torch.int32: 3, torch.int64: 4}
@@ -137,6 +137,11 @@ SIGNATURES = {
     'kfac_factor_linear_diag_workspace_bytes': (c_size_t, [c_int64, c_int]),
     'kfac_factor_linear_diag': (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_void_p, c_void_p, c_size_t,
                                         c_void_p]),
+    'kfac_factor_linear_diag_ones': (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_float, c_void_p, c_void_p,
+                                             c_size_t, c_void_p]),
+    'kfac_factor_conv_input_diag_workspace_bytes': (c_size_t, [C.POINTER(ConvGeometry)]),
+    'kfac_factor_conv_input_diag': (c_int, [c_void_p, c_int, C.POINTER(ConvGeometry), c_int, c_float, c_void_p,
+                                            c_void_p, c_size_t, c_void_p]),
     'kfac_diag_snapshot': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     'kfac_factor_norm_workspace_bytes': (c_size_t, [c_int, c_int64, c_int, c_int64]),
     'kfac_factor_norm': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int64, c_int, c_int64, c_int, C.c_double,

@@ -175,8 +175,9 @@ def second_order_layout(layer: KFACLayer) -> Layout:
                     for s in 'ag')
     snapshots, post = (), ()
     if layer.diag_side:
-        # embedding (d = 'a') or diagonal-G layer (d = 'g'): the diagonal factor is its own eigendecomposition and
-        # ships as a snapshot; only the dense factor f is decomposed, and there is never a V x d dgda
+        # embedding or diagonal-A layer (d = 'a') or diagonal-G layer (d = 'g'): the diagonal factor is its own
+        # eigendecomposition and ships as a snapshot; only the dense factor f is decomposed, and there is never a
+        # V x d dgda
         d, f = layer.diag_side, layer.dense_side
         D, F, n, nd = d.upper(), f.upper(), (a if f == 'a' else g), (a if d == 'a' else g)
         snapshots = ((D, layer, d, 'd' + d),)
@@ -191,8 +192,11 @@ def second_order_layout(layer: KFACLayer) -> Layout:
             decompositions = ((f, 1, '_q' + f, None, '_d' + f),)
             post = ((F, 'inverse', ('_q' + f, '_d' + f, f + '_inv')),)
             needs = {'d' + d, f + '_inv'}
-        unready = f'The second-order data of the {"embedding" if d == "a" else "diagonal-G layer"} has not been computed'
-        item = dict(kind=_cabi.KFAC_ITEM_EMBEDDING if d == 'a' else _cabi.KFAC_ITEM_DIAG_G,
+        kind, what = ((_cabi.KFAC_ITEM_EMBEDDING, 'embedding') if layer.embedding
+                      else (_cabi.KFAC_ITEM_DIAG_A, 'diagonal-A layer') if d == 'a'
+                      else (_cabi.KFAC_ITEM_DIAG_G, 'diagonal-G layer'))
+        unready = f'The second-order data of the {what} has not been computed'
+        item = dict(kind=kind,
                     ldqa=ld4(n) if f == 'a' else 0, ldqg=ld4(n) if f == 'g' else 0, ld_dgda=0)
         eigen = layer.method == ComputeMethod.EIGEN
     else:
@@ -422,7 +426,7 @@ class BaseKFACPreconditioner:
                 module.register_forward_pre_hook(self._save_input_with_kwargs, with_kwargs=True)
             else:
                 module.register_forward_pre_hook(self._save_input)
-            if layer.diag_a:
+            if layer.embedding:
                 # the input of an embedding (the indices) never requires grad: a full backward hook would fire through
                 # the output with a warning on every backward pass, so the output tensor is hooked directly
                 module.register_forward_hook(self._hook_output)
@@ -789,7 +793,7 @@ class BaseKFACPreconditioner:
             self._a_reduce_work.wait()
             self._a_reduce_work = None
             self._a_block_reduced = False
-        if not layer.diag_a:        # integer indices are counted as they are
+        if not layer.embedding:     # integer indices are counted as they are
             x = cast_for_factor(x, layer.factor_dtype)
         x = layer.module.prepare_input(x)
         layer.module.accumulate_a(x, layer._a_batch_view, self._scratch)
@@ -975,13 +979,17 @@ class BaseKFACPreconditioner:
         lib = _cabi.load()
         stream = _cabi.stream_ptr()
         flags = None
-        # diagonal factors (an embedding's A, a diagonal-G layer's G) take the EMA of vectors.  A window of token counts
-        # is finite whatever the loss scale and is never guarded; a diagonal G is guarded like every G.  The blocks of a
-        # normalization layer (G side) are element-wise too and take the same path
+        # diagonal factors (an embedding's or a diagonal-A layer's A, a diagonal-G layer's G) take the EMA of vectors.
+        # A window of token counts is finite whatever the loss scale and is never guarded; a diagonal A of activations
+        # and a diagonal G are guarded like every dense A and G.  The blocks of a normalization layer (G side) are
+        # element-wise too and take the same path
         def vec(l, w):
             return l.diag_side == w or l.norm
-        split = {alpha: ([(l, w) for l, w in todo if vec(l, w) and not (self._guard_factors and w == 'g')],
-                         [(l, w) for l, w in todo if vec(l, w) and self._guard_factors and w == 'g'],
+
+        def guard(l, w):
+            return self._guard_factors and (w == 'g' or not l.embedding)
+        split = {alpha: ([(l, w) for l, w in todo if vec(l, w) and not guard(l, w)],
+                         [(l, w) for l, w in todo if vec(l, w) and guard(l, w)],
                          [(l, w) for l, w in todo if not vec(l, w)])
                  for alpha, todo in self._pending_alpha.items()}
         if self._guard_factors:
@@ -1001,7 +1009,7 @@ class BaseKFACPreconditioner:
                 scales = (C.c_void_p * len(guarded))()
                 for i, (layer, which) in enumerate(guarded):
                     items[i] = self._take_window(layer, which)
-                    if layer.device_grad_scaler:
+                    if which == 'g' and layer.device_grad_scaler:
                         scales[i] = layer._g_scale_slot.data_ptr()
                 need = lib.kfac_factor_ema_diag_guarded_workspace_bytes(len(guarded))
                 ws = flags.data_ptr() + flag_off

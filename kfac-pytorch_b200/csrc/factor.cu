@@ -518,11 +518,16 @@ __global__ void __launch_bounds__(256) linear_diag_kernel(const T* __restrict__ 
     if (j0 + k < V) out[j0 + k] = (float)acc[k];
 }
 
-// acc[j] += scale * sum_c partial[c][j], the chunks added in order in fp64
-__global__ void linear_diag_reduce_kernel(const float* __restrict__ partial, int chunks, int V, float scale, float* acc) {
-  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < V; j += gridDim.x * blockDim.x) {
+// acc[j] += scale * sum_c partial[c][j], the chunks added in order in fp64; acc[V] += scale * ones_sum when ones (the
+// bias entry of a diagonal A: the sum of the ones column's squares)
+__global__ void linear_diag_reduce_kernel(const float* __restrict__ partial, int chunks, int V, int ones,
+                                          double ones_sum, float scale, float* acc) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < V + ones; j += gridDim.x * blockDim.x) {
     double t = 0.0;
-    for (int c = 0; c < chunks; ++c) t += (double)partial[(int64_t)c * V + j];
+    if (j < V)
+      for (int c = 0; c < chunks; ++c) t += (double)partial[(int64_t)c * V + j];
+    else
+      t = ones_sum;
     acc[j] = __fadd_rn(acc[j], (float)((double)scale * t));
   }
 }
@@ -1012,6 +1017,15 @@ extern "C" int kfac_factor_ema_diag_guarded(const kfac_ema_item* items, int coun
   return launch_ema_diag(items, count, alpha, loss_scale, (int*)ws, skipped, s);
 }
 
+namespace kfac {
+int launch_diag_reduce(const float* partial, int chunks, int V, int ones, double ones_sum, float scale, float* acc,
+                       cudaStream_t s) {
+  linear_diag_reduce_kernel<<<grid_for(V + ones), 256, 0, s>>>(partial, chunks, V, ones, ones_sum, scale, acc);
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+}  // namespace kfac
+
 extern "C" size_t kfac_factor_linear_diag_workspace_bytes(int64_t rows, int features) {
   if (rows <= 0 || features <= 0) return 0;
   return align_up((size_t)linear_diag_chunks(rows) * (size_t)features * sizeof(float), 256);
@@ -1019,6 +1033,11 @@ extern "C" size_t kfac_factor_linear_diag_workspace_bytes(int64_t rows, int feat
 
 extern "C" int kfac_factor_linear_diag(const void* x, int dtype, int64_t rows, int features, float scale, float* acc,
                                        void* ws, size_t ws_bytes, void* stream) {
+  return kfac_factor_linear_diag_ones(x, dtype, rows, features, 0, scale, acc, ws, ws_bytes, stream);
+}
+
+extern "C" int kfac_factor_linear_diag_ones(const void* x, int dtype, int64_t rows, int features, int append_ones,
+                                            float scale, float* acc, void* ws, size_t ws_bytes, void* stream) {
   KFAC_CHECK_ARG(acc && features > 0 && rows >= 0 && (x || rows == 0), "linear_diag args");
   KFAC_CHECK_ARG(dtype == KFAC_F32 || dtype == KFAC_F16 || dtype == KFAC_BF16, "dtype");
   if (rows == 0) return KFAC_OK;
@@ -1036,9 +1055,7 @@ extern "C" int kfac_factor_linear_diag(const void* x, int dtype, int64_t rows, i
   else if (dtype == KFAC_F16) linear_diag_kernel<__half><<<grid, 256, 0, s>>>((const __half*)x, rows, features, chunk_rows, partial);
   else linear_diag_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, rows, features, chunk_rows, partial);
   KFAC_LAUNCH_CHECK();
-  linear_diag_reduce_kernel<<<grid_for(features), 256, 0, s>>>(partial, (int)chunks, features, scale, acc);
-  KFAC_LAUNCH_CHECK();
-  return KFAC_OK;
+  return launch_diag_reduce(partial, (int)chunks, features, append_ones ? 1 : 0, (double)rows, scale, acc, s);
 }
 
 extern "C" int kfac_diag_snapshot(const float* src, float* dst, int n, int* status, void* stream) {

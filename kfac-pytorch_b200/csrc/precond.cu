@@ -52,6 +52,28 @@ __global__ void __launch_bounds__(256) gather_all_kernel(const GatherDev* items,
   }
 }
 
+// out (a x ldo) = grad^T for the (g, a) grad matrix [wgrad | bgrad], zero in the columns [g, ldo): the K-major operand of a
+// diagonal-A item's products.  32 x 32 tiles through shared memory, so that both the reads of grad and the writes of
+// out are coalesced
+__global__ void __launch_bounds__(256) gather_t_kernel(const void* w, const void* b, int dtype, int g, int a, float* out,
+                                                       int ldo) {
+  __shared__ float tile[32][33];
+  const int j0 = blockIdx.x * 32, i0 = blockIdx.y * 32;   // j: row of grad (column of out), i: column of grad
+  const int aw = b ? a - 1 : a;
+  for (int r = threadIdx.y; r < 32; r += 8) {
+    const int j = j0 + r, i = i0 + threadIdx.x;
+    float v = 0.f;
+    if (j < g && i < aw) v = load_as_float(w, dtype, (long long)j * aw + i);
+    else if (j < g && i < a) v = load_as_float(b, dtype, j);
+    tile[r][threadIdx.x] = v;
+  }
+  __syncthreads();
+  for (int r = threadIdx.y; r < 32; r += 8) {
+    const int i = i0 + r, j = j0 + threadIdx.x;
+    if (i < a && j < ldo) out[(long long)i * ldo + j] = tile[threadIdx.x][r];
+  }
+}
+
 // ---- kl-clip scale and write-back: ONE launch each over all layers, deterministic ---------------
 // device copy of a kfac_grad_item + the offset of its g*a elements in the concatenated element space
 struct GradDev { const float* P; void* w; void* b; int dtype, g, a, ldp; long long elem0; int taps; };
@@ -224,7 +246,8 @@ struct TiedScaleDev { float* T; const float* f; const float* h; const float* mu;
 
 // ---- precondition: stage-wise over ALL layers ------------------------------------------------------
 // workspace: [GatherDev table][grouped-GEMM tables][ones vector][per layer: GR (g x ld4 a), T1 (a x ld4 g),
-// T2 (g x ld4 a)][slabs].  A diagonal item (rows x n, see DiagItem) takes GR and T1 as rows x ld4(n) and no T2.
+// T2 (g x ld4 a)][slabs].  A diagonal item (rows x n, see DiagItem) takes GR and T1 as rows x ld4(n) and no T2; a
+// diagonal-A item's GR is grad^T (a x ld4 g).
 struct PrecondLayout {
   size_t off_gather, off_tied, off_gemm, off_ones, off_tiles, off_slab, total;
   int ones_n;                                          // length of the ones vector (inverse method, diagonal items)
@@ -236,7 +259,9 @@ struct PrecondLayout {
 // (V x d for an embedding, V x a for a diagonal-G layer), one dense factor of size n on its columns (G, resp. A:
 // basis q, its transpose qT, inverse inv, eigenvalues vcol) and one diagonal factor vrow on its rows.  P has the
 // gradient's layout, rows x n.  A tied item is an embedding item whose basis q = M is not orthogonal and whose
-// epilogue reads a second row vector vrow2 = h and its own damping (KFAC_ITEM_TIED in the header).
+// epilogue reads a second row vector vrow2 = h and its own damping (KFAC_ITEM_TIED in the header).  A diagonal-A item
+// is the embedding problem on grad^T (rows = a, n = g), gathered transposed; its last product is formed transposed,
+// so that P keeps the dense layout n x rows (g x a).
 struct DiagItem {
   int rows, n;
   const float *q, *qT, *inv, *vrow, *vcol;
@@ -246,9 +271,10 @@ struct DiagItem {
 };
 
 static bool is_diag(const kfac_precond_item& it) { return it.kind != KFAC_ITEM_DENSE; }
+static bool is_diag_a(const kfac_precond_item& it) { return it.kind == KFAC_ITEM_DIAG_A; }
 
 static DiagItem diag_view(const kfac_precond_item& it) {
-  if (it.kind == KFAC_ITEM_EMBEDDING) return DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg, nullptr, 0.f};
+  if (it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_A) return DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg, nullptr, 0.f};
   if (it.kind == KFAC_ITEM_TIED) return DiagItem{it.a, it.g, it.qg, it.qgT, nullptr, it.da, it.dg, it.ldqg, it.dh, it.tied_damping};
   return DiagItem{it.g, it.a, it.qa, it.qaT, it.a_inv, it.dg, it.da, it.ldqa, nullptr, 0.f};
 }
@@ -290,8 +316,10 @@ static void precond_layout(const kfac_precond_item* items, int count, PrecondLay
       // only the plain product with Q^T (K = n) can split; the products with an epilogue run unsplit, like stage (2)
       const DiagItem D = diag_view(items[i]);
       if (D.n > 1024) {
+        // P is rows x ld4(n), or n x ld4(rows) for a diagonal-A item
+        const size_t p_elems = is_diag_a(items[i]) ? (size_t)D.n * ld4(D.rows) : (size_t)D.rows * ld4(D.n);
         L.splits_g[i] = ceil_div(D.n, 512);
-        L.slab_g[i] = take((size_t)L.splits_g[i] * D.rows * ld4(D.n) * sizeof(float));
+        L.slab_g[i] = take((size_t)L.splits_g[i] * p_elems * sizeof(float));
       }
       continue;
     }
@@ -346,12 +374,13 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
   for (int i = 0; i < count; ++i) {
     const kfac_precond_item& it = items[i];
     KFAC_CHECK_ARG(it.kind == KFAC_ITEM_DENSE || it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_G ||
-                   it.kind == KFAC_ITEM_TIED, "precond item kind");
+                   it.kind == KFAC_ITEM_TIED || it.kind == KFAC_ITEM_DIAG_A, "precond item kind");
     KFAC_CHECK_ARG(it.n_peers >= 0 && it.n_peers <= 7 && (it.n_peers == 0 || it.peer_P), "precond peers");
     if (is_diag(it)) {
       const DiagItem D = diag_view(it);
-      KFAC_CHECK_ARG(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= D.n && D.ldq >= D.n &&
-                     (it.kind == KFAC_ITEM_DIAG_G || !it.bgrad), "precond diagonal item");
+      KFAC_CHECK_ARG(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= (is_diag_a(it) ? D.rows : D.n) &&
+                     D.ldq >= D.n && (it.kind == KFAC_ITEM_DIAG_G || is_diag_a(it) || !it.bgrad),
+                     "precond diagonal item");
       KFAC_CHECK_ARG(it.kind != KFAC_ITEM_TIED || it.tied_damping > 0.f, "precond tied item damping");
       const bool ready = D.vrow && (it.kind == KFAC_ITEM_TIED ? (D.q && D.qT && D.vcol && D.vrow2)
                                     : method == KFAC_EIGEN ? (D.q && D.qT && D.vcol) : D.inv != nullptr);
@@ -360,8 +389,14 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
                       ? "precondition: the second-order data of an embedding layer has not been computed"
                   : it.kind == KFAC_ITEM_TIED
                       ? "precondition: the second-order data of a tied embedding / head pair has not been computed"
+                  : it.kind == KFAC_ITEM_DIAG_A
+                      ? "precondition: the second-order data of a diagonal-A layer has not been computed"
                       : "precondition: the second-order data of a diagonal-G layer has not been computed");
         return KFAC_ERR_NOT_READY;
+      }
+      if (is_diag_a(it)) {              // grad^T, by gather_t_kernel below: no elements in the gather of the others
+        gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, 0, 0, 1, F(L.gr[i]), total, 0};
+        continue;
       }
       // [wgrad | bgrad] as a (rows, n) layer: an embedding's V x d weight gradient, or a diagonal-G layer's own
       gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, D.rows, D.n, ld4(D.n), F(L.gr[i]), total, 0};
@@ -387,6 +422,14 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
   KFAC_CUDA(cudaMemcpyAsync(base + L.off_gather, gat.data(), sizeof(GatherDev) * count, cudaMemcpyHostToDevice, s));
   gather_all_kernel<<<grid_for(total), 256, 0, s>>>((const GatherDev*)(base + L.off_gather), count, total);
   KFAC_LAUNCH_CHECK();
+  for (int i = 0; i < count; ++i) {
+    const kfac_precond_item& it = items[i];
+    if (!is_diag_a(it)) continue;
+    KFAC_CHECK_ARG(ceil_div(it.a, 32) <= 65535, "precond diagonal-A item: a");
+    const dim3 grid((unsigned)ceil_div(ld4(it.g), 32), (unsigned)ceil_div(it.a, 32));
+    gather_t_kernel<<<grid, dim3(32, 8), 0, s>>>(it.wgrad, it.bgrad, it.grad_dtype, it.g, it.a, F(L.gr[i]), ld4(it.g));
+    KFAC_LAUNCH_CHECK();
+  }
   const float* ones = F(L.off_ones);
   if (L.ones_n && method == KFAC_INVERSE) {
     fill_ones_kernel<<<grid_for(L.ones_n), 256, 0, s>>>(F(L.off_ones), L.ones_n);
@@ -468,7 +511,16 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
     const kfac_precond_item& it = items[i];
     const int g = it.g, a = it.a;
     int64_t p_rows = g, p_ld = ld4(a);
-    if (is_diag(it)) {
+    if (is_diag_a(it)) {
+      const DiagItem D = diag_view(it);
+      if (method == KFAC_EIGEN) {       // (4a) P[r, c] = sum_k Qg[r, k] T[c, k]  (g x a, K = g)
+        plain(i, D.q, D.ldq, F(L.t1[i]), ld4(D.n), it.P, it.ldp, D.n, D.rows, D.n);
+      } else {                          // (4a) P[r, c] = (sum_k Ginv[r, k] grad^T[c, k]) / (a[c] + damping)  (g x a, K = g)
+        plain(i, D.inv, D.ldq, F(L.gr[i]), ld4(D.n), it.P, it.ldp, D.n, D.rows, D.n);
+        st[i].epi = EPI_DIV_OUTER; st[i].dg = ones; st[i].da = D.vrow; st[i].damping = damping;
+      }
+      p_rows = D.n; p_ld = ld4(D.rows);
+    } else if (is_diag(it)) {
       const DiagItem D = diag_view(it);
       if (method == KFAC_EIGEN || it.kind == KFAC_ITEM_TIED) {   // (4d) P[v, c] = sum_k T[v, k] Q[c, k]  (rows x n, K = n)
         plain(i, F(L.t1[i]), ld4(D.n), D.q, D.ldq, it.P, it.ldp, D.rows, D.n, D.n);

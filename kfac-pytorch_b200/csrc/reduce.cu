@@ -69,11 +69,15 @@ __global__ void __launch_bounds__(256) reduce_linear_kernel(const T* __restrict_
 // read.
 constexpr int CONV_SMEM = 2048;   // doubles of rowsum per chunk, and the most (l, i, j) taps of a CTA
 
-// fp32 sum of row[m step] over one run [m0, m1), in order
-template <typename T>
+// fp32 sum of row[m step] (of its squares: SQ) over one run [m0, m1), in order
+template <typename T, bool SQ = false>
 __device__ __forceinline__ float run_sum(const T* __restrict__ row, int m0, int m1, int step) {
   float acc = 0.f;
-  for (int m = m0; m < m1; ++m) acc += to_float<T>(row[m * step]);
+  for (int m = m0; m < m1; ++m) {
+    const float v = to_float<T>(row[m * step]);
+    if constexpr (SQ) acc = fmaf(v, v, acc);
+    else acc += v;
+  }
   return acc;
 }
 
@@ -84,7 +88,8 @@ __device__ __forceinline__ void ones_and_padding(const ConvGeo& g, int ones, dou
     o[f] = (f == d && ones) ? (float)((double)g.spatial() * sc) : 0.f;
 }
 
-template <typename T, bool TRANSPOSED>
+// SQ: the window sums of the squared input (kfac_factor_conv_input_diag), with ones = 0 and ld = features
+template <typename T, bool TRANSPOSED, bool SQ = false>
 __global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restrict__ x, const ConvGeo g, int ones,
                                                                 float scale, float* out, int64_t ld) {
   using Tap = TapMap<TRANSPOSED>;
@@ -111,7 +116,7 @@ __global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restr
         int first, step, n;
         Tap::span(g.W, j, g.sw, g.dw, g.pw, g.Wo, first, step, n);
         const T* __restrict__ row = xp + (int64_t)q * g.W + first;
-        for (int m0 = 0; m0 < n; m0 += RUN) acc += (double)run_sum(row, m0, min(n, m0 + RUN), step);
+        for (int m0 = 0; m0 < n; m0 += RUN) acc += (double)run_sum<T, SQ>(row, m0, min(n, m0 + RUN), step);
       }
       rowsum[e] = acc;
     }
@@ -142,7 +147,7 @@ __global__ void __launch_bounds__(256) reduce_conv_input_kernel(const T* __restr
 // reduce_conv_input_kernel would give one thread per tap j a whole signal; here a CTA per (b, c, j) forms the fp32 runs
 // of the tap's sum in parallel and one thread adds them in fp64 in run order -- the order of reduce_conv_input_kernel,
 // so both give the same bits.
-template <typename T, bool TRANSPOSED>
+template <typename T, bool TRANSPOSED, bool SQ = false>
 __global__ void __launch_bounds__(256) reduce_conv_input_1d_kernel(const T* __restrict__ x, const ConvGeo g, int ones,
                                                                    float scale, float* out, int64_t ld) {
   __shared__ double runs[CONV_SMEM];
@@ -159,7 +164,7 @@ __global__ void __launch_bounds__(256) reduce_conv_input_1d_kernel(const T* __re
     const int kn = min(CONV_SMEM, n - k0);
     for (int k = threadIdx.x; k < kn; k += blockDim.x) {
       const int m0 = (k0 + k) * RUN;
-      runs[k] = (double)run_sum(row, m0, min(cnt, m0 + RUN), step);
+      runs[k] = (double)run_sum<T, SQ>(row, m0, min(cnt, m0 + RUN), step);
     }
     __syncthreads();
     if (threadIdx.x == 0)
@@ -208,6 +213,13 @@ __global__ void __launch_bounds__(256) reduce_planes_kernel(const T* __restrict_
 }  // namespace
 }  // namespace kfac
 
+namespace kfac {
+// acc[j] += scale * sum_c partial[c][j] (j < V, the chunks added in order in fp64), acc[V] += scale * ones_sum when
+// ones: the second launch of the diagonal statistics (factor.cu)
+int launch_diag_reduce(const float* partial, int chunks, int V, int ones, double ones_sum, float scale, float* acc,
+                       cudaStream_t s);
+}  // namespace kfac
+
 using namespace kfac;
 
 extern "C" int kfac_reduce_rows_linear_strided(const void* x, int dtype, int64_t B, int64_t R, int features,
@@ -244,7 +256,7 @@ extern "C" int kfac_reduce_rows_linear(const void* x, int dtype, int64_t B, int6
                                          loss_scale, out, ld_out, stream);
 }
 
-template <bool TRANSPOSED = false>
+template <bool TRANSPOSED = false, bool SQ = false>
 static int reduce_conv_input(const void* x, int dtype, const ConvGeo& g, int append_ones, float scale, float* out,
                              int ld_out, cudaStream_t s) {
   KFAC_CHECK_ARG((int64_t)g.kd * g.kh * g.kw <= CONV_SMEM, "kernel window of more than 2048 taps");
@@ -257,23 +269,23 @@ static int reduce_conv_input(const void* x, int dtype, const ConvGeo& g, int app
   if (g.D == 1 && g.H == 1 && g.kd == 1 && g.kh == 1 && g.pd == 0 && g.ph == 0 && g.Do == 1 && g.Ho == 1) {
     const dim3 grid(planes, (unsigned)g.kw);
     if (dtype == KFAC_F32)
-      reduce_conv_input_1d_kernel<float, TRANSPOSED><<<grid, 256, 0, s>>>((const float*)x, g, ones, scale, out,
+      reduce_conv_input_1d_kernel<float, TRANSPOSED, SQ><<<grid, 256, 0, s>>>((const float*)x, g, ones, scale, out,
                                                                           ld_out);
     else if (dtype == KFAC_F16)
-      reduce_conv_input_1d_kernel<__half, TRANSPOSED><<<grid, 256, 0, s>>>((const __half*)x, g, ones, scale, out,
+      reduce_conv_input_1d_kernel<__half, TRANSPOSED, SQ><<<grid, 256, 0, s>>>((const __half*)x, g, ones, scale, out,
                                                                            ld_out);
     else if (dtype == KFAC_BF16)
-      reduce_conv_input_1d_kernel<__nv_bfloat16, TRANSPOSED><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones,
+      reduce_conv_input_1d_kernel<__nv_bfloat16, TRANSPOSED, SQ><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones,
                                                                                   scale, out, ld_out);
     else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   } else {
     if (dtype == KFAC_F32)
-      reduce_conv_input_kernel<float, TRANSPOSED><<<planes, 256, 0, s>>>((const float*)x, g, ones, scale, out, ld_out);
+      reduce_conv_input_kernel<float, TRANSPOSED, SQ><<<planes, 256, 0, s>>>((const float*)x, g, ones, scale, out, ld_out);
     else if (dtype == KFAC_F16)
-      reduce_conv_input_kernel<__half, TRANSPOSED><<<planes, 256, 0, s>>>((const __half*)x, g, ones, scale, out,
+      reduce_conv_input_kernel<__half, TRANSPOSED, SQ><<<planes, 256, 0, s>>>((const __half*)x, g, ones, scale, out,
                                                                           ld_out);
     else if (dtype == KFAC_BF16)
-      reduce_conv_input_kernel<__nv_bfloat16, TRANSPOSED><<<planes, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones,
+      reduce_conv_input_kernel<__nv_bfloat16, TRANSPOSED, SQ><<<planes, 256, 0, s>>>((const __nv_bfloat16*)x, g, ones,
                                                                                  scale, out, ld_out);
     else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   }
@@ -331,4 +343,40 @@ extern "C" int kfac_reduce_rows_conv2d_gradout(const void* g, int dtype, int bat
   else { set_error("unknown dtype %d", dtype); return KFAC_ERR_BAD_ARG; }
   KFAC_LAUNCH_CHECK();
   return KFAC_OK;
+}
+
+// The diagonal of kfac_factor_conv_input's A without the im2col: each (b, c) volume is read once, and the window sums
+// of its squares over the output lattice (reduce_conv_input_kernel with SQ, the re-reads of a row from L1) give the
+// example's partial for the C x taps features; the partials (B x features fp32, example-major) are added per feature
+// in example order, in fp64, by a second launch.
+static size_t conv_diag_ws_bytes(const ConvGeo& g) {
+  return align_up((size_t)g.batch * (size_t)g.features() * sizeof(float), 256);
+}
+
+extern "C" size_t kfac_factor_conv_input_diag_workspace_bytes(const kfac_conv_geometry* geom) {
+  ConvGeo g;
+  if (resolve_conv_geometry(geom, &g) != KFAC_OK) return 0;
+  return conv_diag_ws_bytes(g);
+}
+
+extern "C" int kfac_factor_conv_input_diag(const void* x, int dtype, const kfac_conv_geometry* geom, int append_ones,
+                                           float scale, float* acc, void* ws, size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(x && acc, "null pointer");
+  ConvGeo g;
+  const int rc = resolve_conv_geometry(geom, &g);
+  if (rc) return rc;
+  KFAC_CHECK_ARG(dtype == KFAC_F32 || dtype == KFAC_F16 || dtype == KFAC_BF16, "dtype");
+  KFAC_CHECK_ARG(g.features() < (1ll << 31), "features");
+  const size_t need = conv_diag_ws_bytes(g);
+  if (!ws || ws_bytes < need) {
+    set_error("factor_conv_input_diag: workspace too small (%zu < %zu)", ws_bytes, need);
+    return KFAC_ERR_WORKSPACE;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const int d = (int)g.features();
+  float* partial = (float*)ws;
+  const int r = reduce_conv_input<false, true>(x, dtype, g, 0, 1.f, partial, d, s);
+  if (r) return r;
+  return launch_diag_reduce(partial, g.batch, d, append_ones ? 1 : 0, (double)g.batch * (double)g.spatial(), scale,
+                            acc, s);
 }

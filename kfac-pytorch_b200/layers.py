@@ -39,19 +39,23 @@ class FactorRows:
 class ModuleHelper:
     """Geometry + native dispatch for one supported module type."""
 
-    diagonal_a = False      # True: A is diagonal and kept as a vector (embeddings)
+    diagonal_a = False      # True: A is kept as a vector (embeddings; Linear and convolutions in diagonal_a_layers)
     diagonal_g = False      # True: G is approximated by its diagonal and kept as a vector (diagonal_g_layers)
+    embedding = False       # True: an nn.Embedding (its diagonal A is exact, its input indices, P is (V, d))
     norm = False            # True: exact per-channel Fisher blocks instead of two factors (precondition_norms)
     call_kwargs = False     # True: the A hook passes every call's arguments to bind_call (output_size)
     # 0: the weight gradient is the row-major (g, a - has_bias) gradient matrix; T > 0: it is (C_in, g, T), a transposed
     # convolution's, with grad-matrix element (r, ci * T + t) at [ci, r, t] (kfac_precond_item.wgrad_taps)
     wgrad_taps = 0
 
-    def __init__(self, module: torch.nn.Module, reduce: bool = False):
+    def __init__(self, module: torch.nn.Module, reduce: bool = False, diagonal_a: bool = False):
         self.module = module
         # K-FAC-reduce (kfac_approx='reduce', Linear and Conv2d only): a call with R > 1 shared positions per example
         # forms its statistics from one row per example; R = 1 takes the expand path
         self.reduce = reduce
+        # diagonal_a_layers (Linear, Conv2d, Conv1d / Conv3d): A is approximated by diag(A), the diagonal of the dense
+        # A of the same rows, kept as a vector of a_dim floats
+        self.diagonal_a = diagonal_a or type(self).diagonal_a
 
     def __repr__(self) -> str:
         return f'{self.__class__.__name__}({repr(self.module)})'
@@ -106,7 +110,7 @@ class ModuleHelper:
         if rows.direct is not None:
             rows.direct(acc, 1.0, scratch)
         else:
-            self._accumulate_rows(rows, acc, 1.0, scratch, False)
+            self._accumulate_rows(rows, acc, 1.0, scratch, self.diagonal_a)
 
     def accumulate_g(self, g: torch.Tensor, acc: torch.Tensor, grad_scale: float, scratch) -> None:
         rows = self.rows_g(_detached(g))
@@ -206,7 +210,7 @@ class LinearModuleHelper(ModuleHelper):
     @property
     def a_factor_shape(self):
         d = self.module.weight.size(1) + int(self.has_bias())
-        return (d, d)
+        return (d,) if self.diagonal_a else (d, d)
 
     @property
     def g_factor_shape(self):
@@ -251,7 +255,18 @@ class LinearModuleHelper(ModuleHelper):
                                                       1.0 / grad_scale, loss_scale, out, ld, _cabi.stream_ptr()),
                         'kfac_rows_linear')
 
-        if side == 'g' and self.diagonal_g:
+        if side == 'a' and self.diagonal_a:
+            def direct(acc, grad_scale, scratch):
+                if rows == 0:
+                    return
+                lib = _cabi.load()
+                c = _dense(t)
+                need = lib.kfac_factor_linear_diag_workspace_bytes(rows, feat)
+                _cabi.check(lib.kfac_factor_linear_diag_ones(c.data_ptr(), _dtype_code(c), rows, feat, ones,
+                                                             1.0 / (rows * grad_scale * grad_scale), acc.data_ptr(),
+                                                             _workspace(scratch, need, c.device), need,
+                                                             _cabi.stream_ptr()), 'kfac_factor_linear_diag_ones')
+        elif side == 'g' and self.diagonal_g:
             def direct(acc, grad_scale, scratch):
                 if rows == 0:
                     return
@@ -282,7 +297,7 @@ class Conv2dModuleHelper(ModuleHelper):
     def a_factor_shape(self):
         m = self.module
         d = m.in_channels * m.kernel_size[0] * m.kernel_size[1] + int(self.has_bias())
-        return (d, d)
+        return (d,) if self.diagonal_a else (d, d)
 
     @property
     def g_factor_shape(self):
@@ -304,7 +319,11 @@ class Conv2dModuleHelper(ModuleHelper):
 
     def rows_a(self, x):
         geo = self._geometry(x)
-        return _conv_input_rows(self, x, 'conv2d_input', geo, (), geo[0], self._spatial(geo), geo[1] * geo[4] * geo[5])
+        B, Cc, H, W, kh, kw, sh, sw, ph, pw = geo
+        arr = lambda v: (C.c_int * 3)(*v)  # noqa: E731
+        diag = (_cabi.ConvGeometry(B, Cc, arr((1, H, W)), arr((1, kh, kw)), arr((1, sh, sw)), arr((1, 1, 1)),
+                                   arr((0, ph, pw)), arr((0, ph, pw))) if self.diagonal_a else None)
+        return _conv_input_rows(self, x, 'conv2d_input', geo, (), B, self._spatial(geo), Cc * kh * kw, diag)
 
     def rows_g(self, g):
         return _conv_gradout_rows(g, *g.shape, self.reduce)
@@ -315,10 +334,12 @@ class Conv2dModuleHelper(ModuleHelper):
 # of its S A rows and the sum of its S G rows divided by sqrt(S), the rows carrying the 1/S of the expand rows: scale
 # 1/S^2 (A) and S^-3/2 (G) on the plain window sums.
 def _conv_input_rows(helper: ModuleHelper, x: torch.Tensor, entry: str, geo: tuple, ws_args: tuple, B: int,
-                     S: int, patch: int) -> FactorRows:
+                     S: int, patch: int, diag: _cabi.ConvGeometry | None = None) -> FactorRows:
     """A rows of a convolution (`patch` = C_in * taps features before the ones column) through the native entries
     kfac_factor_{entry}, kfac_rows_{entry} and kfac_reduce_rows_{entry}, which take the geometry arguments `geo` (and
-    `ws_args` after the ones column in the workspace query)."""
+    `ws_args` after the ones column in the workspace query).  A diagonal A (`diag`: the geometry as a
+    kfac_conv_geometry) takes kfac_factor_conv_input_diag in expand mode, and the diagonal statistics of the reduced
+    rows under K-FAC-reduce."""
     ones = int(helper.has_bias())
     d = patch + ones
     if helper.reduce and S > 1:
@@ -332,6 +353,17 @@ def _conv_input_rows(helper: ModuleHelper, x: torch.Tensor, entry: str, geo: tup
         c, fn = _dense(x), f'kfac_rows_{entry}'
         _cabi.check(getattr(_cabi.load(), fn)(c.data_ptr(), _dtype_code(c), *geo, ones, 1.0 / S, out, ld,
                                               _cabi.stream_ptr()), fn)
+
+    if diag is not None:
+        def direct_diag(acc, grad_scale, scratch):
+            lib = _cabi.load()
+            c = _dense(x)
+            need = lib.kfac_factor_conv_input_diag_workspace_bytes(C.byref(diag))
+            _cabi.check(lib.kfac_factor_conv_input_diag(c.data_ptr(), _dtype_code(c), C.byref(diag), ones,
+                                                        1.0 / (float(B) * float(S) ** 3), acc.data_ptr(),
+                                                        _workspace(scratch, need, c.device), need, _cabi.stream_ptr()),
+                        'kfac_factor_conv_input_diag')
+        return FactorRows(B * S, d, write, direct_diag)
 
     def direct(acc, grad_scale, scratch):
         lib = _cabi.load()
@@ -395,8 +427,8 @@ class ConvNdModuleHelper(ModuleHelper):
     # the native input-side entries: kfac_factor_{entry}, kfac_rows_{entry}, kfac_reduce_rows_{entry}
     entry = 'conv_input'
 
-    def __init__(self, module: torch.nn.Module, reduce: bool = False):
-        super().__init__(module, reduce=reduce)
+    def __init__(self, module: torch.nn.Module, reduce: bool = False, diagonal_a: bool = False):
+        super().__init__(module, reduce=reduce, diagonal_a=diagonal_a)
         self.nd = len(module.kernel_size)
         # output extents of the recent A calls: the G call checks its output gradient against them
         self._extents: list[tuple[int, ...]] = []
@@ -408,7 +440,11 @@ class ConvNdModuleHelper(ModuleHelper):
         taps = math.prod(m.kernel_size)
         if m.groups != 1:
             what = f'groups={m.groups} (grouped and depthwise convolutions are not supported)'
-        elif max(self.a_factor_shape[0], m.out_channels) > _cabi.KFAC_EIGH_MAX_N:
+        elif self.diagonal_a and m.out_channels > _cabi.KFAC_EIGH_MAX_N:
+            what = f'a G factor of {m.out_channels}, beyond the eigensolver\'s {_cabi.KFAC_EIGH_MAX_N}'
+        elif self.diagonal_a and taps > REDUCE_MAX_TAPS:
+            what = f'a kernel of {taps} taps, beyond the {REDUCE_MAX_TAPS} of the diagonal A statistics'
+        elif not self.diagonal_a and max(self.a_factor_shape[0], m.out_channels) > _cabi.KFAC_EIGH_MAX_N:
             what = (f'factors of {self.a_factor_shape[0]} (A) and {m.out_channels} (G), beyond the eigensolver\'s '
                     f'{_cabi.KFAC_EIGH_MAX_N}')
         elif self.reduce and taps > REDUCE_MAX_TAPS:
@@ -420,7 +456,7 @@ class ConvNdModuleHelper(ModuleHelper):
     @property
     def a_factor_shape(self):
         d = self.module.in_channels * math.prod(self.module.kernel_size) + int(self.has_bias())
-        return (d, d)
+        return (d,) if self.diagonal_a else (d, d)
 
     @property
     def g_factor_shape(self):
@@ -483,7 +519,7 @@ class ConvNdModuleHelper(ModuleHelper):
     def rows_a(self, x):
         geo, S = self._prepared_geometry(x)
         return _conv_input_rows(self, x, self.entry, (C.byref(geo),), (CONV_ND_WORKSPACE_BYTES,), geo.batch, S,
-                                geo.C * math.prod(self.module.kernel_size))
+                                geo.C * math.prod(self.module.kernel_size), geo if self.diagonal_a else None)
 
     def rows_g(self, g):
         """The output gradient read as (B, C, 1, S); its extent must be one an A call of this window computed."""
@@ -571,6 +607,7 @@ class EmbeddingModuleHelper(LinearModuleHelper):
     Linear layer's (never K-FAC-reduced).  The gradient and P use the weight's own layout (V x d)."""
 
     diagonal_a = True
+    embedding = True
 
     @property
     def a_factor_shape(self):
@@ -995,16 +1032,19 @@ RECURRENT_TYPES: tuple[type, ...] = (torch.nn.RNN, torch.nn.LSTM, torch.nn.GRU)
 def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
                       diagonal_g: bool = False, norms: bool = False, reduce: bool = False,
                       conv_nd: bool = False, conv_transpose: bool = False,
-                      group_norms: bool = False) -> ModuleHelper | None:
+                      group_norms: bool = False, diagonal_a: bool = False) -> ModuleHelper | None:
     """reduce: K-FAC-reduce statistics for Linear (dense and diagonal-G), Conv2d and (with conv_nd) Conv1d / Conv3d
     and (with conv_transpose) ConvTranspose1d / 2d / 3d layers; embeddings and normalization layers keep their own
-    statistics."""
+    statistics.  diagonal_a: a diagonal A for a Linear, Conv2d or (with conv_nd) Conv1d / Conv3d layer; the other
+    kinds ignore it (register_modules refuses them)."""
     if isinstance(module, LINEAR_TYPES):
-        return (DiagonalGLinearModuleHelper if diagonal_g else LinearModuleHelper)(module, reduce=reduce)
+        if diagonal_g:
+            return DiagonalGLinearModuleHelper(module, reduce=reduce)
+        return LinearModuleHelper(module, reduce=reduce, diagonal_a=diagonal_a)
     if isinstance(module, CONV2D_TYPES):
-        return Conv2dModuleHelper(module, reduce=reduce)
+        return Conv2dModuleHelper(module, reduce=reduce, diagonal_a=diagonal_a)
     if conv_nd and isinstance(module, CONV_ND_TYPES):
-        return ConvNdModuleHelper(module, reduce=reduce)
+        return ConvNdModuleHelper(module, reduce=reduce, diagonal_a=diagonal_a)
     if conv_transpose and isinstance(module, CONV_TRANSPOSE_TYPES):
         return ConvTransposeModuleHelper(module, reduce=reduce)
     if embeddings and isinstance(module, EMBEDDING_TYPES):
@@ -1043,8 +1083,10 @@ class KFACLayer:
         self.symmetric_factors = module.has_symmetric_factors()
         self.a_dim = module.a_factor_shape[0]
         self.g_dim = module.g_factor_shape[0]
-        # A is a vector of a_dim floats (embeddings); P then has the weight's layout (a x g) instead of (g x a)
+        # A is a vector of a_dim floats (embeddings, diagonal_a_layers)
         self.diag_a = module.diagonal_a
+        # an nn.Embedding: its input is indices, and P has the weight's layout (a x g) instead of (g x a)
+        self.embedding = module.embedding
         # G is a vector of g_dim floats (diagonal_g_layers); P keeps the dense layout (g x a)
         self.diag_g = module.diagonal_g
         # normalization layer (precondition_norms): no A factor, G holds the C x k blocks, P is C x a_dim
@@ -1132,13 +1174,14 @@ class KFACLayer:
 
     @property
     def dense_side(self) -> str | None:
-        """The dense factor of a diagonal layer ('g' for an embedding, 'a' for a diagonal-G layer)."""
+        """The dense factor of a diagonal layer ('g' for an embedding or a diagonal-A layer, 'a' for a diagonal-G
+        layer)."""
         return {'a': 'g', 'g': 'a'}.get(self.diag_side)
 
     @property
     def p_shape(self) -> tuple[int, int]:
         """Logical shape of P: (g, a), or the weight layout (a, g) = (V, d) of an embedding."""
-        return (self.a_dim, self.g_dim) if self.diag_a else (self.g_dim, self.a_dim)
+        return (self.a_dim, self.g_dim) if self.embedding else (self.g_dim, self.a_dim)
 
     @property
     def grad(self):
@@ -1156,8 +1199,15 @@ class KFACLayer:
             for key, want in (('A', self.a_factor_shape), ('G', self.g_factor_shape)):
                 t = state_dict[key]
                 if t is not None and tuple(t.shape) != want:
-                    kind = 'embedding' if self.diag_a else 'diagonal-G layer'
+                    kind = ('embedding' if self.embedding else 'diagonal-A layer' if self.diag_a
+                            else 'diagonal-G layer')
                     raise ValueError(f'{kind} factor {key} has shape {tuple(t.shape)}, expected {want}')
+        elif not self.norm:
+            # a vector (a diagonal factor's entry) would broadcast into a dense factor
+            for key, want in (('A', self.a_factor_shape), ('G', self.g_factor_shape)):
+                t = state_dict[key]
+                if t is not None and t.dim() != len(want):
+                    raise ValueError(f'factor {key} has shape {tuple(t.shape)}, expected {want}')
         if self.norm:
             if state_dict['A'] is not None:
                 raise ValueError('a normalization layer has no A factor (expected None)')
@@ -1211,6 +1261,7 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
                      kfac_approx: str = 'expand', precondition_attention: bool = False,
                      precondition_conv_nd: bool = False, precondition_conv_transpose: bool = False,
                      precondition_group_norms: bool = False, precondition_recurrent: bool = False,
+                     diagonal_a_layers: list[str] | None = None,
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
@@ -1228,23 +1279,29 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     precondition_group_norms: also register GroupNorm and InstanceNorm1d/2d/3d modules with affine parameters (not in
     the reference; `layer.norm`).  precondition_recurrent: register every torch.nn.RNN, LSTM and GRU as two Linear
     layers per layer k and direction, `{name}.ih_l{k}{sfx}` and `{name}.hh_l{k}{sfx}`, keyed by their
-    RecurrentSubLayerHelper (not in the reference).  `layer.index` counts the other layers and the normalization layers
-    separately."""
+    RecurrentSubLayerHelper (not in the reference).  diagonal_a_layers: regexes on name and class name; a registered
+    torch.nn.Linear, Conv2d or (precondition_conv_nd) Conv1d / Conv3d that matches keeps a diagonal A and may have an A
+    above the eigensolver's limit (not in the reference); any other registered module that matches, a match of
+    diagonal_g_layers too and a G above the limit are errors.  `layer.index` counts the other layers and the
+    normalization layers separately."""
     diagonal_g_layers = diagonal_g_layers or []
+    diagonal_a_layers = diagonal_a_layers or []
     layers: dict[torch.nn.Module, tuple[str, KFACLayer]] = {}
     counts = [0, 0]
     out_projs = ({id(m.out_proj) for m in model.modules() if isinstance(m, torch.nn.MultiheadAttention)}
                  if precondition_attention else set())
     for name, module in model.named_modules():
         if precondition_attention and isinstance(module, torch.nn.MultiheadAttention):
-            for helper in _attention_projections(name, module, skip_layers, diagonal_g_layers, kfac_approx):
+            for helper in _attention_projections(name, module, skip_layers, diagonal_g_layers, kfac_approx,
+                                                 diagonal_a_layers):
                 layer = KFACLayer(helper, **layer_kwargs)
                 layer.index = counts[0]
                 counts[0] += 1
                 layers[helper] = (f'{name}.{helper.which}_proj', layer)
             continue
         if precondition_recurrent and isinstance(module, RECURRENT_TYPES):
-            for helper in _recurrent_sublayers(name, module, skip_layers, diagonal_g_layers, kfac_approx):
+            for helper in _recurrent_sublayers(name, module, skip_layers, diagonal_g_layers, kfac_approx,
+                                               diagonal_a_layers):
                 layer = KFACLayer(helper, **layer_kwargs)
                 layer.index = counts[0]
                 counts[0] += 1
@@ -1257,15 +1314,18 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
         if not all(p.requires_grad for p in module.parameters()):
             continue
         diag_g = any_match(name, diagonal_g_layers) or any_match(module.__class__.__name__, diagonal_g_layers)
+        diag_a = any_match(name, diagonal_a_layers) or any_match(module.__class__.__name__, diagonal_a_layers)
         helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g,
                                    norms=precondition_norms, reduce=kfac_approx == 'reduce',
                                    conv_nd=precondition_conv_nd, conv_transpose=precondition_conv_transpose,
-                                   group_norms=precondition_group_norms)
+                                   group_norms=precondition_group_norms, diagonal_a=diag_a and not diag_g)
         if helper is None:
             continue
         if diag_g and not helper.diagonal_g:
             raise ValueError(f'diagonal_g_layers matches "{name}" ({module.__class__.__name__}): only torch.nn.Linear '
                              'layers can keep a diagonal G (add it to skip_layers or narrow the pattern)')
+        if diag_a:
+            _check_diagonal_a(name, module, helper, diag_g)
         if isinstance(helper, ConvNdModuleHelper):
             helper.check(name)
         assert module not in layers
@@ -1297,8 +1357,25 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     return layers
 
 
+def _check_diagonal_a(name: str, module: torch.nn.Module, helper: ModuleHelper, diag_g: bool) -> None:
+    """Refuse a diagonal_a_layers match that cannot keep a diagonal A."""
+    cls = module.__class__.__name__
+    if diag_g:
+        raise ValueError(f'diagonal_a_layers and diagonal_g_layers both match "{name}" ({cls}): a layer keeps at most '
+                         'one diagonal factor (add it to skip_layers or narrow a pattern)')
+    if helper.embedding or not helper.diagonal_a:
+        raise ValueError(f'diagonal_a_layers matches "{name}" ({cls}): only torch.nn.Linear, Conv2d and (with '
+                         'precondition_conv_nd) Conv1d / Conv3d layers can keep a diagonal A (add it to skip_layers or '
+                         'narrow the pattern)')
+    g = helper.g_factor_shape[0]
+    if g > _cabi.KFAC_EIGH_MAX_N:
+        raise ValueError(f'diagonal_a_layers matches "{name}" ({cls}), whose G factor of {g} exceeds '
+                         f'KFAC_EIGH_MAX_N = {_cabi.KFAC_EIGH_MAX_N}; add it to skip_layers')
+
+
 def _attention_projections(name: str, module: torch.nn.MultiheadAttention, skip_layers: list[str],
-                           diagonal_g_layers: list[str], kfac_approx: str) -> list[AttentionProjectionHelper]:
+                           diagonal_g_layers: list[str], kfac_approx: str,
+                           diagonal_a_layers: list[str]) -> list[AttentionProjectionHelper]:
     """The registered projections of one attention: none when skip_layers matches its name or class or one of its
     parameters is frozen, else those whose name `{name}.{q,k,v,out}_proj` skip_layers does not match."""
     cls = module.__class__.__name__
@@ -1322,12 +1399,15 @@ def _attention_projections(name: str, module: torch.nn.MultiheadAttention, skip_
                                                                                                diagonal_g_layers):
             raise ValueError(f'diagonal_g_layers matches the attention projection "{pname}": attention projections '
                              'cannot keep a diagonal G (add it to skip_layers or narrow the pattern)')
+        if any(any_match(q, diagonal_a_layers) for q in (name, cls, pname)):
+            raise ValueError(f'diagonal_a_layers matches the attention projection "{pname}": attention projections '
+                             'cannot keep a diagonal A (add it to skip_layers or narrow the pattern)')
         helpers.append(AttentionProjectionHelper(module, which, reduce=kfac_approx == 'reduce'))
     return helpers
 
 
 def _recurrent_sublayers(name: str, module: torch.nn.Module, skip_layers: list[str], diagonal_g_layers: list[str],
-                         kfac_approx: str) -> list[RecurrentSubLayerHelper]:
+                         kfac_approx: str, diagonal_a_layers: list[str]) -> list[RecurrentSubLayerHelper]:
     """The registered sub-layers of one RNN / LSTM / GRU: none when skip_layers matches its name or class or one of its
     parameters is frozen, else those whose name `{name}.{ih,hh}_l{k}{sfx}` skip_layers does not match."""
     cls = module.__class__.__name__
@@ -1352,6 +1432,9 @@ def _recurrent_sublayers(name: str, module: torch.nn.Module, skip_layers: list[s
                 if any(any_match(q, diagonal_g_layers) for q in (name, cls, sname)):
                     raise ValueError(f'diagonal_g_layers matches the recurrent sub-layer "{sname}": recurrent layers '
                                      'cannot keep a diagonal G (add it to skip_layers or narrow the pattern)')
+                if any(any_match(q, diagonal_a_layers) for q in (name, cls, sname)):
+                    raise ValueError(f'diagonal_a_layers matches the recurrent sub-layer "{sname}": recurrent layers '
+                                     'cannot keep a diagonal A (add it to skip_layers or narrow the pattern)')
                 n = max(helper.a_factor_shape[0], helper.g_factor_shape[0])
                 if n > _cabi.KFAC_EIGH_MAX_N:
                     raise ValueError(f'recurrent sub-layer "{sname}" has a factor of {n} > KFAC_EIGH_MAX_N = '

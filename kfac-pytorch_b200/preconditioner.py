@@ -35,7 +35,7 @@ def _mock_new_group(x: list[int]) -> None:
 def layer_work(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
                assignment_strategy: AssignmentStrategy) -> dict[str, dict[str, float]]:
     """Per-factor cost the KAISA placement balances: d^3 (COMPUTE) or d^2 (MEMORY) for a dense factor.  A diagonal
-    factor (an embedding's A, a diagonal-G layer's G) is never decomposed and takes V floats, so its cost is V under
+    factor (an embedding's or a diagonal-A layer's A, a diagonal-G layer's G) is never decomposed and takes V floats, so its cost is V under
     both strategies; a V^3 cost would let one vocabulary dominate the greedy placement.  A tied pair is one unit
     under the embedding's name with the single factor 'G' (one rank holds E, H, f and h whatever colocate_factors
     says), costed 2 cost(d) + 2 V; the head has no entry."""
@@ -58,21 +58,23 @@ def layer_work(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
 
 def _check_diagonal_layers(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
                            compute_method: ComputeMethod, tied_embeddings: bool = False) -> None:
-    """Reject the registered diagonal layers (embeddings, diagonal-G layers) this preconditioner cannot handle.  With
+    """Reject the registered diagonal layers (embeddings, diagonal-A and diagonal-G layers) this preconditioner cannot
+    handle.  With
     `tied_embeddings`, an embedding whose weight is the weight of one bias-less diagonal-G Linear forms a tied pair
     with it instead (`KFACLayer.tied_head` / `tied_embedding`)."""
     diag = [(module, name, l) for module, (name, l) in layers.items() if l.diag_side]
     if tied_embeddings:
         _tie_pairs(layers, compute_method)
     for module, name, l in diag:
-        kind, keyword = ('embedding', 'precondition_embeddings') if l.diag_a else ('layer', 'diagonal_g_layers')
+        kind, keyword = (('embedding', 'precondition_embeddings') if l.embedding
+                         else ('layer', 'diagonal_a_layers') if l.diag_a else ('layer', 'diagonal_g_layers'))
         if compute_method == ComputeMethod.EKFAC:
             raise ValueError(f'{keyword} does not support compute_method=EKFAC ({kind} "{name}"); '
                              f'add the {kind}s to skip_layers')
-        if l.diag_a and module.sparse:
+        if l.embedding and module.sparse:
             raise ValueError(f'embedding "{name}" has sparse=True: K-FAC needs a dense weight gradient '
                              '(add it to skip_layers or use sparse=False)')
-        if l.diag_a and module.scale_grad_by_freq:
+        if l.embedding and module.scale_grad_by_freq:
             raise ValueError(f'embedding "{name}" has scale_grad_by_freq=True: its weight gradient is then not the '
                              'one the K-FAC factors model (add it to skip_layers)')
         for other, (other_name, _) in layers.items():
@@ -87,7 +89,7 @@ def _tie_pairs(layers: dict[torch.nn.Module, tuple[str, KFACLayer]], compute_met
     """Form the tied pairs of precondition_tied_embeddings: a registered embedding and the one other registered module
     that owns its weight, which must be a bias-less torch.nn.Linear matched by diagonal_g_layers."""
     for module, (name, l) in layers.items():
-        if not l.diag_a:
+        if not l.embedding:
             continue
         owners = [(other, other_name, ol) for other, (other_name, ol) in layers.items()
                   if other is not module and any(p is module.weight for p in other.parameters())]
@@ -261,6 +263,23 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     and the stock forward (cuDNN) otherwise.  Refused with a ValueError naming the layer and `skip_layers`:
     `proj_size > 0`, a factor above `KFAC_EIGH_MAX_N` (8192; an LSTM with H > 2048, a GRU with H > 2730), a
     `diagonal_g_layers` match, a weight shared with another registered module, and subclasses.
+
+    `diagonal_a_layers` takes regexes matched against module names and class names, like `diagonal_g_layers`.  A
+    registered `torch.nn.Linear` or `torch.nn.Conv2d` (and, with `precondition_conv_nd`, `Conv1d` / `Conv3d`) that
+    matches keeps its A factor as the vector diag(A) of `a_dim` floats, bias entry included: the diagonal of the dense A
+    the layer would form from the same rows (the conv rows' 1/S, the K-FAC-reduce rows), with the same EMA,
+    `accumulation_steps`, schedules and `grad_scaler` handling.  This is for layers with more inputs than the
+    eigensolver takes (`KFAC_EIGH_MAX_N` = 8192): the `down_proj` of a LLaMA-style MLP (11008 or 14336 inputs), or a
+    3 x 3 convolution on 1024 or 1280 channels (A = 9217 or 11521).  G stays dense (and must be at most 8192), and the
+    layer's P is
+        eigen:   P = Qg [(Qg^T grad) / (dg x da + damping)]
+        inverse: P = (G + damping I)^-1 grad diag(1 / (da + damping))
+    with da = diag(A) its own eigenvalues (Qa = I).  It is a different approximation of the curvature, hence opt-in.
+    As for diagonal-G layers, `compute_eigenvalue_outer_product` does not apply and the damping is the one of the step
+    that preconditions; P keeps the dense layout, so kl-clip and the write-back are unchanged.  Refused with a
+    ValueError naming the layer and `skip_layers`: EKFAC, a match on an embedding, a normalization layer, an attention
+    projection, a recurrent sub-layer or a transposed convolution, a layer matched by `diagonal_g_layers` too, a G
+    above 8192, and a weight shared with another registered module.
     """
 
     def __init__(
@@ -297,6 +316,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         precondition_conv_transpose: bool = False,
         precondition_group_norms: bool = False,
         precondition_recurrent: bool = False,
+        diagonal_a_layers: list[str] | None = None,
     ) -> None:
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
@@ -384,7 +404,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             precondition_attention=precondition_attention, precondition_conv_nd=precondition_conv_nd,
             precondition_conv_transpose=precondition_conv_transpose,
             precondition_group_norms=precondition_group_norms,
-            precondition_recurrent=precondition_recurrent,
+            precondition_recurrent=precondition_recurrent, diagonal_a_layers=diagonal_a_layers,
             method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
@@ -428,6 +448,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'precondition_conv_transpose': precondition_conv_transpose,
             'precondition_group_norms': precondition_group_norms,
             'precondition_recurrent': precondition_recurrent,
+            'diagonal_a_layers': diagonal_a_layers,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
