@@ -61,7 +61,8 @@ long long kfac_launch_count(void);
  * tall inputs (rows >= 512, features >= 128) are transposed once into a feature-major matrix
  * and the SYRK runs on the wgmma engine; the workspace also holds the per-split partials of a
  * reduction split over the SMs.  Every factor call is deterministic (partials are added in a
- * fixed order; without a workspace the reduction runs unsplit). */
+ * fixed order; without a workspace the reduction runs unsplit).  rows = 0 adds nothing and
+ * launches nothing. */
 size_t kfac_factor_linear_workspace_bytes(int64_t rows, int features, int append_ones);
 int kfac_factor_linear(const void* x, int dtype, int64_t rows, int features,
                        int append_ones, float scale, float* acc, void* ws,

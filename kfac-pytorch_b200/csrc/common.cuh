@@ -220,8 +220,10 @@ struct TcGemmArgs {
   float* peerD[7]; int npeer;      // fused broadcast: the epilogue also stores the tile into these peer copies of D
 };
 bool tc_gemm_supported(const TcGemmArgs& a);
-// the split count launch_tc_gemm runs for a request of `splits` over kb_total k-blocks (every split non-empty)
+// the split count launch_tc_gemm runs for a request of `splits` over kb_total k-blocks (every split non-empty); one
+// when there is nothing to reduce (the split plan of a factor call on zero rows)
 inline int tc_normalize_splits(int splits, int kb_total) {
+  if (kb_total < 1) return 1;
   splits = splits < 1 ? 1 : (splits > kb_total ? kb_total : splits);
   const int per = (kb_total + splits - 1) / splits;
   return (kb_total + per - 1) / per;

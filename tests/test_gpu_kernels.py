@@ -123,14 +123,21 @@ def test_factor_conv2d_input(lib, dev, geo):
     assert rel_fro(0.5 * (acc + acc.t()), ref) < 2e-5
 
 
-@pytest.mark.parametrize('B,Cc,Ho,Wo', [(2, 6, 8, 8), (3, 10, 3, 3), (4, 64, 14, 14), (2, 130, 5, 7), (1, 1, 1, 1),
-                                        (8, 256, 7, 7), (32, 512, 7, 7)])
+GRADOUT_SHAPES = [(2, 6, 8, 8), (3, 10, 3, 3), (4, 64, 14, 14), (2, 130, 5, 7), (1, 1, 1, 1), (8, 256, 7, 7),
+                  (32, 512, 7, 7)]
+# fp16 / bf16 gradients (autocast): read in place by the SIMT kernel, or packed by im2col for the tensor-core SYRK
+GRADOUT_CASES = ([pytest.param(*s, torch.float32, id='-'.join(map(str, s))) for s in GRADOUT_SHAPES] +
+                 [pytest.param(*s, dt, id='-'.join(map(str, s)) + '-' + name) for dt, name in
+                  ((torch.float16, 'f16'), (torch.bfloat16, 'bf16')) for s in GRADOUT_SHAPES])
+
+
+@pytest.mark.parametrize('B,Cc,Ho,Wo,dtype', GRADOUT_CASES)
 @pytest.mark.parametrize('with_ws', [True, False])
-def test_factor_conv2d_gradout(lib, dev, B, Cc, Ho, Wo, with_ws):
+def test_factor_conv2d_gradout(lib, dev, B, Cc, Ho, Wo, dtype, with_ws):
     from oracle import kfac_oracle as O
     torch.manual_seed(B + Cc)
-    g = torch.randn(B, Cc, Ho, Wo)
-    ref = O.conv2d_g_factor(g)
+    g = torch.randn(B, Cc, Ho, Wo).to(dtype)
+    ref = O.conv2d_g_factor(g.double())            # on the values as stored
     acc = torch.zeros(Cc, Cc, device=dev)
     gd = g.to(dev)
     scale = 1.0 / (B * float(Ho * Wo) ** 3)
@@ -141,8 +148,9 @@ def test_factor_conv2d_gradout(lib, dev, B, Cc, Ho, Wo, with_ws):
     assert not with_ws or need >= packed
     ws = torch.empty(max(need, 1), dtype=torch.uint8, device=dev)
     acc2 = torch.zeros_like(acc)
+    code = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}[dtype]
     for out in (acc, acc2):
-        assert lib.kfac_factor_conv2d_gradout(gd.data_ptr(), 0, B, Cc, Ho, Wo, scale, out.data_ptr(),
+        assert lib.kfac_factor_conv2d_gradout(gd.data_ptr(), code, B, Cc, Ho, Wo, scale, out.data_ptr(),
                                               ws.data_ptr() if need else None, need, S()) == 0
     torch.cuda.synchronize()
     assert rel_fro(0.5 * (acc + acc.t()), ref) < 2e-5

@@ -283,3 +283,14 @@ def test_sytrd_schedule_covers_all_and_cannot_deadlock():
                         done += 1
                         progress = True
             assert done == jobs, f'schedule deadlocks: {done} of {jobs} jobs can run (grid {grid})'
+
+
+def test_linear_factor_workspace_of_zero_rows():
+    """A Linear layer called on an empty batch: its factor call asks for the workspace of zero rows, which needs none
+    (the split plan of an empty reduction is one split; host-only entries of the library, no GPU)."""
+    from kfac_b200 import _cabi
+    lib = _cabi.load()
+    for feat, ones in ((64, 1), (1024, 0), (2048, 1)):
+        assert lib.kfac_factor_linear_workspace_bytes(0, feat, ones) == 0
+        assert lib.kfac_factor_linear_strided_workspace_bytes(0, feat, feat + 3, ones) == 0
+    assert lib.kfac_factor_linear_workspace_bytes(2048, 1024, 1) > 0
