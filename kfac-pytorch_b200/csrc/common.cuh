@@ -39,6 +39,9 @@ void count_launch(int n);
 
 inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+// The number of chains a tensor-core reduction of length K runs in: above 1024, chains of at most 512.  The engine's
+// accumulator truncates, and short chains keep the 3xTF32 result at fp32 accuracy.
+inline int chain_splits(int64_t K) { return K > 1024 ? ceil_div(K, 512) : 1; }
 
 // A kfac_conv_geometry flattened for the kernels, with its output extents.  Only the padding before an axis enters the
 // input index; the padding after it only extends the output.

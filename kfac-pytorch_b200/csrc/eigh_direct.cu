@@ -208,7 +208,7 @@ void make_layout(const int* n, int count, const std::vector<Wave>& waves, Layout
   for (int i = 0; i < count; ++i) {
     MatLayout& m = L.m[i];
     m.n = n[i]; m.np = round_up(n[i], TRD_T); m.nblk = m.np / TRD_T; m.nbt = ceil_div(n[i], BT);
-    m.ksplit = m.np > 1024 ? ceil_div(m.np, 512) : 1;
+    m.ksplit = chain_splits(m.np);
     const size_t sq = (size_t)m.np * m.np * sizeof(float);
     m.VT = take(sq); m.Vb = take(sq + (size_t)m.np * BT * 4); m.Q0 = take(sq); m.Q1 = take(sq);
     m.Vp = take((size_t)m.np * TRD_NB * 4); m.Wp = take((size_t)m.np * TRD_NB * 4);
@@ -532,8 +532,8 @@ int run_wave_tail(const Wave& wave, const WaveLayout& wl, const Layout& L, char*
         const int j0 = kb * BT, nb = std::min(BT, m.n - j0), K = m.np - j0;
         const float* Vk = t.VT + (size_t)j0 * t.ldv + j0;
         GroupedGemm g = plain(Vk, t.ldv, Vk, t.ldv, (float*)(base + m.S) + (size_t)kb * BT * BT, BT, nb, nb, K);
-        if (K > 1024 && grouped_gemm_tc_ok(g)) {
-          g.splits = ceil_div(K, 512);
+        if (chain_splits(K) > 1 && grouped_gemm_tc_ok(g)) {
+          g.splits = chain_splits(K);
           g.slab = (float*)(base + m.slabS) + (size_t)kb * m.ksplit * BT * BT; g.slab_stride = (int64_t)nb * BT;
         }
         gg.push_back(g);
@@ -599,7 +599,7 @@ int run_wave_tail(const Wave& wave, const WaveLayout& wl, const Layout& L, char*
       float* Y2 = (float*)(base + m.Y2);
       // Y = ZT[:, j0:] V_k[j0:, :]
       GroupedGemm a = plain(ZT + j0, np, t.VT + (size_t)j0 * t.ldv + j0, t.ldv, Y, BT, n, nbp, K);
-      if (K > 1024 && grouped_gemm_tc_ok(a)) { a.splits = ceil_div(K, 512); a.slab = (float*)(base + m.slabY); a.slab_stride = (int64_t)n * BT; }
+      if (chain_splits(K) > 1 && grouped_gemm_tc_ok(a)) { a.splits = chain_splits(K); a.slab = (float*)(base + m.slabY); a.slab_stride = (int64_t)n * BT; }
       g1.push_back(a);
       // Y2 = Y T_k^T
       g2.push_back(plain(Y, BT, (float*)(base + m.Tm) + (size_t)kb * BT * BT, BT, Y2, BT, n, nbp, nbp));

@@ -178,10 +178,10 @@ static void stat_layout(const kfac_ekfac_stat_item* items, int count, StatLayout
   for (int i = 0; i < count; ++i) {
     const kfac_ekfac_stat_item& it = items[i];
     const int N = (int)it.N, ldN = (int)ld4(it.N);
-    if (it.a > 1024 && grouped_gemm_tc_ok(gemm(al, it.ldqa, al, it.ldx, nullptr, ldN, it.a, N, it.a, 1.f, EPI_NONE)))
-      L.ch_x[i] = ceil_div(it.a, CHAIN);
-    if (it.g > 1024 && grouped_gemm_tc_ok(gemm(al, it.ldqg, al, it.ldg, nullptr, ldN, it.g, N, it.g, 1.f, EPI_NONE)))
-      L.ch_g[i] = ceil_div(it.g, CHAIN);
+    if (grouped_gemm_tc_ok(gemm(al, it.ldqa, al, it.ldx, nullptr, ldN, it.a, N, it.a, 1.f, EPI_NONE)))
+      L.ch_x[i] = chain_splits(it.a);
+    if (grouped_gemm_tc_ok(gemm(al, it.ldqg, al, it.ldg, nullptr, ldN, it.g, N, it.g, 1.f, EPI_NONE)))
+      L.ch_g[i] = chain_splits(it.g);
     const bool tc = grouped_gemm_tc_ok(gemm(al, ldN, al, ldN, nullptr, it.lds, it.g, it.a, N, 1.f, EPI_NONE));
     const int chain = tc ? CHAIN : SIMT_CHAIN;
     if (N > 2 * chain) {

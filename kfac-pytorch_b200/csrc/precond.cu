@@ -3,6 +3,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <vector>
 
 #include "common.cuh"
@@ -180,14 +181,14 @@ int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, 
   t.kbatch = 1; t.alpha = 1.f; t.splits = 1;
   t.epi = e.kind; t.E = e.E; t.lde = e.lde; t.dg = e.dg; t.da = e.da; t.damping = e.damping;
   if (M >= 64 && N >= 64 && K >= 32 && tc_gemm_supported(t)) {
-    if (e.kind == EPI_NONE && K > 1024) {
+    if (e.kind == EPI_NONE && chain_splits(K) > 1) {
       // long reductions run as chains of <= 512, split the way the engine splits k-blocks for ceil(K / 512)
       // splits: the tensor-core accumulator truncates, so short chains keep the 3xTF32 result at fp32 accuracy.
       // The chains run in order on the stream, the first storing D and each later one adding its product to D
       // (plain read-modify-write epilogue), so the sum has one fixed order; the TMA maps zero-fill past a chain.
       constexpr int KB = 32;                    // the engine's k-block
       const int kb_total = ceil_div(K, KB);
-      const int chain = ceil_div(kb_total, tc_normalize_splits(ceil_div(K, 512), kb_total)) * KB;
+      const int chain = ceil_div(kb_total, tc_normalize_splits(chain_splits(K), kb_total)) * KB;
       for (int k0 = 0; k0 < K; k0 += chain) {
         TcGemmArgs c = t;
         c.A = A + k0; c.B = B + k0; c.K = std::min(chain, K - k0); c.accumulate = k0 > 0;
@@ -244,17 +245,11 @@ extern "C" int kfac_transpose(const float* src, int ld_src, float* dst, int ld_d
 
 struct TiedScaleDev { float* T; const float* f; const float* h; const float* mu; float t; int n, ld; long long elem0; };
 
-// ---- precondition: stage-wise over ALL layers ------------------------------------------------------
-// workspace: [GatherDev table][grouped-GEMM tables][ones vector][per layer: GR (g x ld4 a), T1 (a x ld4 g),
-// T2 (g x ld4 a)][slabs].  A diagonal item (rows x n, see DiagItem) takes GR and T1 as rows x ld4(n) and no T2; a
-// diagonal-A item's GR is grad^T (a x ld4 g).
-struct PrecondLayout {
-  size_t off_gather, off_tied, off_gemm, off_ones, off_tiles, off_slab, total;
-  int ones_n;                                          // length of the ones vector (inverse method, diagonal items)
-  std::vector<size_t> gr, t1, t2, slab_a, slab_g;     // byte offsets per layer (slab_*: 0 = no split)
-  std::vector<int> splits_a, splits_g;
-};
-
+// ---- precondition: stage-wise over ALL items -------------------------------------------------------
+// Every item is a chain of up to four products, and stage k of all items is one grouped launch.  An item's plan
+// (plan_item) says how its gradient is gathered, which scratch matrices it needs and which product it runs in each
+// stage; the workspace and the launches are derived from the plans.
+//
 // An embedding item and a diagonal-G item are the same problem with the sides swapped: a gradient of `rows` x n
 // (V x d for an embedding, V x a for a diagonal-G layer), one dense factor of size n on its columns (G, resp. A:
 // basis q, its transpose qT, inverse inv, eigenvalues vcol) and one diagonal factor vrow on its rows.  P has the
@@ -270,63 +265,183 @@ struct DiagItem {
   float damping;
 };
 
-static bool is_diag(const kfac_precond_item& it) { return it.kind != KFAC_ITEM_DENSE; }
 static bool is_diag_a(const kfac_precond_item& it) { return it.kind == KFAC_ITEM_DIAG_A; }
 
-static DiagItem diag_view(const kfac_precond_item& it) {
-  if (it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_A) return DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg, nullptr, 0.f};
-  if (it.kind == KFAC_ITEM_TIED) return DiagItem{it.a, it.g, it.qg, it.qgT, nullptr, it.da, it.dg, it.ldqg, it.dh, it.tied_damping};
-  return DiagItem{it.g, it.a, it.qa, it.qaT, it.a_inv, it.dg, it.da, it.ldqa, nullptr, 0.f};
+// the workspace regions of one item (null while the workspace is being sized)
+struct Scratch { float *gr, *t1, *t2; const float* ones; };
+
+struct ItemPlan {
+  int rc = KFAC_OK; const char* err = nullptr;   // the first check the item fails, reported after the workspace check
+  // the gradient matrix [wgrad | bgrad], rows x cols (wgrad laid out as wgrad_offset says for taps), goes to GR as
+  // rows x ld4(cols), or transposed as cols x ld4(rows) by gather_t_kernel
+  int rows = 0, cols = 0, taps = 0;
+  bool transposed = false;
+  size_t gr = 0, t1 = 0, t2 = 0;   // floats of the scratch matrices GR, T1, T2
+  int ones = 0;                    // length of the ones vector its product reads under the inverse method
+  Scratch w{};
+  // the product of stages (1) to (4) (M = N = K = 0: none); the last one writes P and carries the peer stores.  A
+  // product with splits > 1 keeps its partial tiles in the slab of the product of stage slab_of[k] of this item.
+  GroupedGemm stage[4] = {};
+  int slab_of[4] = {0, 1, 2, 3};
+  bool tied = false; TiedScaleDev tied_scale{};   // stage (1)'s product is divided by tied_scale_kernel
+};
+
+static GroupedGemm product(const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M,
+                           int N, int K, int splits = 1) {
+  GroupedGemm g{};
+  g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.D = D; g.ldd = ldd; g.M = M; g.N = N; g.K = K; g.alpha = 1.f;
+  g.epi = EPI_NONE; g.splits = splits;
+  return g;
 }
 
-static void precond_layout(const kfac_precond_item* items, int count, PrecondLayout& L) {
+// the product divided by (dg[m] * da[n] + damping) in its epilogue
+static GroupedGemm div_outer(GroupedGemm g, const float* dg, const float* da, float damping) {
+  g.epi = EPI_DIV_OUTER; g.dg = dg; g.da = da; g.damping = damping;
+  return g;
+}
+
+#define PLAN_CHECK(cond, what) \
+  do { if (!p.err && !(cond)) fail(KFAC_ERR_BAD_ARG, "bad argument: " what " (" #cond ")"); } while (0)
+
+// The plan of one item under `method`.  The sizes and the products do not depend on whether the item passes its
+// checks, so that a call is sized the same way before and after they run.
+static ItemPlan plan_item(const kfac_precond_item& it, int method, float damping, const Scratch& w) {
+  ItemPlan p;
+  p.w = w;
+  auto fail = [&](int rc, const char* msg) { if (!p.err) { p.rc = rc; p.err = msg; } };
+  PLAN_CHECK(it.kind == KFAC_ITEM_DENSE || it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_G ||
+                 it.kind == KFAC_ITEM_TIED || it.kind == KFAC_ITEM_DIAG_A, "precond item kind");
+  PLAN_CHECK(it.n_peers >= 0 && it.n_peers <= 7 && (it.n_peers == 0 || it.peer_P), "precond peers");
+  const bool eigen = method == KFAC_EIGEN;
+  GroupedGemm* st = p.stage;
+  if (it.kind == KFAC_ITEM_DENSE) {
+    PLAN_CHECK(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= it.a, "precond item");
+    if (eigen ? !(it.qa && it.qg && it.qaT && it.qgT && (it.dgda || (it.da && it.dg))) : !(it.a_inv && it.g_inv))
+      fail(KFAC_ERR_NOT_READY, eigen ? "precondition: eigendecompositions for both A and G have not been computed"
+                                     : "precondition: A and G have not been inverted");
+    PLAN_CHECK(it.ldqa >= it.a && it.ldqg >= it.g, "second-order leading dims");
+    PLAN_CHECK(it.wgrad_taps >= 0 && (it.wgrad_taps == 0 || (it.a - (it.bgrad ? 1 : 0)) % it.wgrad_taps == 0),
+               "precond item wgrad_taps");
+    const int g = it.g, a = it.a;
+    p.rows = g; p.cols = a; p.taps = it.wgrad_taps;
+    p.gr = (size_t)g * ld4(a); p.t1 = (size_t)a * ld4(g); p.t2 = (size_t)g * ld4(a);
+    // (1) T^T[a', r] = sum_k (QaT | Ainv)[a', k] grad[r, k]                                  (a x g, K = a)
+    st[0] = product(eigen ? it.qaT : it.a_inv, it.ldqa, w.gr, ld4(a), w.t1, ld4(g), a, g, a, chain_splits(a));
+    if (eigen) {
+      // (2) V2[g', a'] = (sum_k QgT[g', k] T^T[a', k]) * dgda[g', a'], or / (dg[g'] da[a'] + damping)   (g x a, K = g)
+      st[1] = product(it.qgT, it.ldqg, w.t1, ld4(g), w.t2, ld4(a), g, a, g);
+      if (it.dgda) { st[1].epi = EPI_MUL; st[1].E = it.dgda; st[1].lde = it.ld_dgda; }
+      else st[1] = div_outer(st[1], it.dg, it.da, damping);
+      // (3) U^T[c, g'] = sum_k Qa[c, k] V2[g', k]                                  (a x g, K = a, stage (1)'s slab)
+      st[2] = product(it.qa, it.ldqa, w.t2, ld4(a), w.t1, ld4(g), a, g, a, chain_splits(a));
+      p.slab_of[2] = 0;
+    }
+    // (4) P[r, c] = sum_k (Qg | Ginv)[r, k] U^T[c, k]                                       (g x a, K = g)
+    st[3] = product(eigen ? it.qg : it.g_inv, it.ldqg, w.t1, ld4(g), it.P, it.ldp, g, a, g);
+  } else {
+    DiagItem D;
+    const char* not_ready;
+    switch (it.kind) {
+      case KFAC_ITEM_EMBEDDING:
+      case KFAC_ITEM_DIAG_A:
+        D = DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg, nullptr, 0.f};
+        not_ready = is_diag_a(it) ? "precondition: the second-order data of a diagonal-A layer has not been computed"
+                                  : "precondition: the second-order data of an embedding layer has not been computed";
+        break;
+      case KFAC_ITEM_TIED:
+        D = DiagItem{it.a, it.g, it.qg, it.qgT, nullptr, it.da, it.dg, it.ldqg, it.dh, it.tied_damping};
+        not_ready = "precondition: the second-order data of a tied embedding / head pair has not been computed";
+        break;
+      default:                          // KFAC_ITEM_DIAG_G, or a kind the first check rejects
+        D = DiagItem{it.g, it.a, it.qa, it.qaT, it.a_inv, it.dg, it.da, it.ldqa, nullptr, 0.f};
+        not_ready = "precondition: the second-order data of a diagonal-G layer has not been computed";
+    }
+    PLAN_CHECK(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= (is_diag_a(it) ? D.rows : D.n) &&
+                   D.ldq >= D.n && (it.kind == KFAC_ITEM_DIAG_G || is_diag_a(it) || !it.bgrad),
+               "precond diagonal item");
+    PLAN_CHECK(it.kind != KFAC_ITEM_TIED || it.tied_damping > 0.f, "precond tied item damping");
+    const bool tied = it.kind == KFAC_ITEM_TIED;
+    if (!(D.vrow && (tied ? (D.q && D.qT && D.vcol && D.vrow2) : eigen ? (D.q && D.qT && D.vcol) : D.inv != nullptr)))
+      fail(KFAC_ERR_NOT_READY, not_ready);
+    const int ldn = ld4(D.n);
+    p.transposed = is_diag_a(it);
+    p.rows = p.transposed ? D.n : D.rows; p.cols = p.transposed ? D.rows : D.n;
+    p.gr = p.t1 = (size_t)D.rows * ldn;
+    p.ones = tied ? 0 : D.n;
+    if (tied || eigen) {
+      // (1) T[v, j] = (sum_k grad[v, k] Q[k, j]) / (vrow[v] vcol[j] + damping), the division of a tied item by
+      // tied_scale_kernel                                                                      (rows x n, K = n)
+      st[0] = product(w.gr, ldn, D.qT, D.ldq, w.t1, ldn, D.rows, D.n, D.n);
+      if (!tied) st[0] = div_outer(st[0], D.vrow, D.vcol, damping);
+      else { p.tied = true; p.tied_scale = TiedScaleDev{w.t1, D.vrow, D.vrow2, D.vcol, D.damping, D.n, ldn, 0}; }
+    }
+    if (is_diag_a(it)) {
+      // (4) P[r, c] = sum_k Qg[r, k] T[c, k], or (sum_k Ginv[r, k] grad^T[c, k]) / (a[c] + damping)   (g x a, K = g)
+      st[3] = eigen ? product(D.q, D.ldq, w.t1, ldn, it.P, it.ldp, D.n, D.rows, D.n)
+                    : div_outer(product(D.inv, D.ldq, w.gr, ldn, it.P, it.ldp, D.n, D.rows, D.n), w.ones, D.vrow,
+                                damping);
+    } else {
+      // (4) P[v, c] = sum_k T[v, k] Q[c, k], or (sum_k grad[v, k] Inv[c, k]) / (vrow[v] + damping)  (rows x n, K = n)
+      st[3] = eigen || tied ? product(w.t1, ldn, D.q, D.ldq, it.P, it.ldp, D.rows, D.n, D.n)
+                            : div_outer(product(w.gr, ldn, D.inv, D.ldq, it.P, it.ldp, D.rows, D.n, D.n), D.vrow,
+                                        w.ones, damping);
+    }
+  }
+  // the last product splits where it has the plain epilogue and P is at its padded width
+  if (st[3].epi == EPI_NONE && it.ldp == ld4(st[3].N)) st[3].splits = chain_splits(st[3].K);
+  if (!p.err) {
+    // fused compute + broadcast: the same P goes to the peers, from the tile epilogue or from the split's reduce pass
+    st[3].npeer = it.n_peers;
+    for (int q = 0; q < it.n_peers; ++q) st[3].peerD[q] = it.peer_P[q];
+  }
+  return p;
+}
+
+#undef PLAN_CHECK
+
+// workspace: [GatherDev table][TiedScaleDev table][grouped-GEMM tables][ones vector][per item: GR, T1, T2][slabs]
+struct PrecondLayout { size_t off_gather, off_tied, off_gemm, off_ones, total; int ones_n; };
+
+// Plans every item and lays out the workspace from the plans; with a base, the plans address that workspace.
+static PrecondLayout plan_items(const kfac_precond_item* items, int count, int method, float damping, char* base,
+                                std::vector<ItemPlan>& plans) {
+  PrecondLayout L{};
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
+  auto at = [&](size_t o) { return base ? (float*)(base + o) : nullptr; };
+  plans.resize(count);
+  for (int i = 0; i < count; ++i) plans[i] = plan_item(items[i], method, damping, Scratch{});
   L.off_gather = take(sizeof(GatherDev) * (size_t)std::max(1, count));
   L.off_tied = take(sizeof(TiedScaleDev) * (size_t)std::max(1, count));
   L.off_gemm = take(grouped_gemm_ws_bytes(count));
-  L.ones_n = 0;
-  for (int i = 0; i < count; ++i)
-    if (is_diag(items[i]) && items[i].kind != KFAC_ITEM_TIED) L.ones_n = std::max(L.ones_n, diag_view(items[i]).n);
+  for (const ItemPlan& p : plans) L.ones_n = std::max(L.ones_n, p.ones);
   L.off_ones = L.ones_n ? take((size_t)L.ones_n * sizeof(float)) : off;
-  L.off_tiles = off;
-  L.gr.resize(count); L.t1.resize(count); L.t2.resize(count);
-  L.slab_a.assign(count, 0); L.slab_g.assign(count, 0); L.splits_a.assign(count, 1); L.splits_g.assign(count, 1);
-  for (int i = 0; i < count; ++i) {
-    const size_t a = items[i].a, g = items[i].g;
-    if (is_diag(items[i])) {
-      const DiagItem D = diag_view(items[i]);
-      L.gr[i] = take((size_t)D.rows * ld4(D.n) * sizeof(float));
-      L.t1[i] = take((size_t)D.rows * ld4(D.n) * sizeof(float));
-      L.t2[i] = 0;
-      continue;
-    }
-    L.gr[i] = take(g * ld4((int)a) * sizeof(float));
-    L.t1[i] = take(a * ld4((int)g) * sizeof(float));
-    L.t2[i] = take(g * ld4((int)a) * sizeof(float));
+  std::vector<Scratch> w(count);
+  for (int i = 0; i < count; ++i) {   // a braced list is evaluated in order: GR, T1, T2
+    const ItemPlan& p = plans[i];
+    w[i] = Scratch{at(take(p.gr * sizeof(float))), at(take(p.t1 * sizeof(float))), at(take(p.t2 * sizeof(float))),
+                   at(L.off_ones)};
   }
-  L.off_slab = off;
   // long reductions (K > 1024) are split into chains of <= 512: the tensor-core accumulator truncates, short
   // chains keep the 3xTF32 result at fp32 accuracy; the partial tiles go to slabs and are added in a fixed order
   // (deterministic: every replica that preconditions a layer locally must get the same bits).  The layout does not
   // depend on n_peers: a fused broadcast runs the same split, its peers get the reduced sums.
-  for (int i = 0; i < count; ++i) {
-    const size_t a = items[i].a, g = items[i].g;
-    if (is_diag(items[i])) {
-      // only the plain product with Q^T (K = n) can split; the products with an epilogue run unsplit, like stage (2)
-      const DiagItem D = diag_view(items[i]);
-      if (D.n > 1024) {
-        // P is rows x ld4(n), or n x ld4(rows) for a diagonal-A item
-        const size_t p_elems = is_diag_a(items[i]) ? (size_t)D.n * ld4(D.rows) : (size_t)D.rows * ld4(D.n);
-        L.splits_g[i] = ceil_div(D.n, 512);
-        L.slab_g[i] = take((size_t)L.splits_g[i] * p_elems * sizeof(float));
-      }
-      continue;
+  std::vector<std::array<float*, 4>> slab(count);
+  for (int i = 0; i < count; ++i)
+    for (int k = 0; k < 4; ++k) {
+      const GroupedGemm& g = plans[i].stage[k];
+      if (g.splits > 1 && plans[i].slab_of[k] == k) slab[i][k] = at(take((size_t)g.splits * g.M * g.ldd * sizeof(float)));
     }
-    if (a > 1024) { L.splits_a[i] = ceil_div(a, 512); L.slab_a[i] = take((size_t)L.splits_a[i] * a * ld4((int)g) * sizeof(float)); }
-    if (g > 1024) { L.splits_g[i] = ceil_div(g, 512); L.slab_g[i] = take((size_t)L.splits_g[i] * g * ld4((int)a) * sizeof(float)); }
-  }
   L.total = off;
+  if (!base) return L;
+  for (int i = 0; i < count; ++i) {
+    ItemPlan& p = plans[i] = plan_item(items[i], method, damping, w[i]);
+    for (int k = 0; k < 4; ++k) {
+      GroupedGemm& g = p.stage[k];
+      if (g.splits > 1) { g.slab = slab[i][p.slab_of[k]]; g.slab_stride = (int64_t)g.M * g.ldd; }
+    }
+  }
+  return L;
 }
 
 // T[v][j] /= (f[v] + t) + (h[v] + t) mu[j] for every tied item, one launch: the division of a tied item's first product,
@@ -349,9 +464,10 @@ __global__ void fill_ones_kernel(float* out, int n) {
 
 extern "C" size_t kfac_precondition_workspace_bytes(const kfac_precond_item* items, int count) {
   if (count <= 0) return 0;
-  PrecondLayout L;
-  precond_layout(items, count, L);
-  return L.total;
+  // enough for either method (the eigen method's plans split the most)
+  std::vector<ItemPlan> plans;
+  return std::max(plan_items(items, count, KFAC_EIGEN, 0.f, nullptr, plans).total,
+                  plan_items(items, count, KFAC_INVERSE, 0.f, nullptr, plans).total);
 }
 
 extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int method, float damping,
@@ -359,187 +475,67 @@ extern "C" int kfac_precondition(const kfac_precond_item* items, int count, int 
   KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "items");
   KFAC_CHECK_ARG(method == KFAC_EIGEN || method == KFAC_INVERSE, "method");
   if (count == 0) return KFAC_OK;
-  PrecondLayout L;
-  precond_layout(items, count, L);
+  std::vector<ItemPlan> plans;
+  char* base = (char*)ws;
+  const PrecondLayout L = plan_items(items, count, method, damping, base, plans);
   if (!ws || ws_bytes < L.total) {
     set_error("precondition: workspace too small (%zu < %zu)", ws_bytes, L.total);
     return KFAC_ERR_WORKSPACE;
   }
+  for (const ItemPlan& p : plans)
+    if (p.rc) { set_error("%s", p.err); return p.rc; }
   cudaStream_t s = (cudaStream_t)stream;
-  char* base = (char*)ws;
-  auto F = [&](size_t off) { return (float*)(base + off); };
-  // stage 0: grad matrices [wgrad | bgrad] of all layers, one launch
+  // stage 0: the gradient matrices of all items, one launch (the transposed ones have no elements in it)
   std::vector<GatherDev> gat(count);
   long long total = 0;
   for (int i = 0; i < count; ++i) {
     const kfac_precond_item& it = items[i];
-    KFAC_CHECK_ARG(it.kind == KFAC_ITEM_DENSE || it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_G ||
-                   it.kind == KFAC_ITEM_TIED || it.kind == KFAC_ITEM_DIAG_A, "precond item kind");
-    KFAC_CHECK_ARG(it.n_peers >= 0 && it.n_peers <= 7 && (it.n_peers == 0 || it.peer_P), "precond peers");
-    if (is_diag(it)) {
-      const DiagItem D = diag_view(it);
-      KFAC_CHECK_ARG(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= (is_diag_a(it) ? D.rows : D.n) &&
-                     D.ldq >= D.n && (it.kind == KFAC_ITEM_DIAG_G || is_diag_a(it) || !it.bgrad),
-                     "precond diagonal item");
-      KFAC_CHECK_ARG(it.kind != KFAC_ITEM_TIED || it.tied_damping > 0.f, "precond tied item damping");
-      const bool ready = D.vrow && (it.kind == KFAC_ITEM_TIED ? (D.q && D.qT && D.vcol && D.vrow2)
-                                    : method == KFAC_EIGEN ? (D.q && D.qT && D.vcol) : D.inv != nullptr);
-      if (!ready) {
-        set_error(it.kind == KFAC_ITEM_EMBEDDING
-                      ? "precondition: the second-order data of an embedding layer has not been computed"
-                  : it.kind == KFAC_ITEM_TIED
-                      ? "precondition: the second-order data of a tied embedding / head pair has not been computed"
-                  : it.kind == KFAC_ITEM_DIAG_A
-                      ? "precondition: the second-order data of a diagonal-A layer has not been computed"
-                      : "precondition: the second-order data of a diagonal-G layer has not been computed");
-        return KFAC_ERR_NOT_READY;
-      }
-      if (is_diag_a(it)) {              // grad^T, by gather_t_kernel below: no elements in the gather of the others
-        gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, 0, 0, 1, F(L.gr[i]), total, 0};
-        continue;
-      }
-      // [wgrad | bgrad] as a (rows, n) layer: an embedding's V x d weight gradient, or a diagonal-G layer's own
-      gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, D.rows, D.n, ld4(D.n), F(L.gr[i]), total, 0};
-      total += (long long)D.rows * ld4(D.n);
-      continue;
-    }
-    KFAC_CHECK_ARG(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= it.a, "precond item");
-    if (method == KFAC_EIGEN) {
-      if (!(it.qa && it.qg && it.qaT && it.qgT && (it.dgda || (it.da && it.dg)))) {
-        set_error("precondition: eigendecompositions for both A and G have not been computed");
-        return KFAC_ERR_NOT_READY;
-      }
-    } else if (!(it.a_inv && it.g_inv)) {
-      set_error("precondition: A and G have not been inverted");
-      return KFAC_ERR_NOT_READY;
-    }
-    KFAC_CHECK_ARG(it.ldqa >= it.a && it.ldqg >= it.g, "second-order leading dims");
-    KFAC_CHECK_ARG(it.wgrad_taps >= 0 && (it.wgrad_taps == 0 || (it.a - (it.bgrad ? 1 : 0)) % it.wgrad_taps == 0),
-                   "precond item wgrad_taps");
-    gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, it.g, it.a, ld4(it.a), F(L.gr[i]), total, it.wgrad_taps};
-    total += (long long)it.g * ld4(it.a);
+    const ItemPlan& p = plans[i];
+    if (p.transposed) { gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, 0, 0, 1, p.w.gr, total, 0}; continue; }
+    gat[i] = GatherDev{it.wgrad, it.bgrad, it.grad_dtype, p.rows, p.cols, ld4(p.cols), p.w.gr, total, p.taps};
+    total += (long long)p.rows * ld4(p.cols);
   }
   KFAC_CUDA(cudaMemcpyAsync(base + L.off_gather, gat.data(), sizeof(GatherDev) * count, cudaMemcpyHostToDevice, s));
   gather_all_kernel<<<grid_for(total), 256, 0, s>>>((const GatherDev*)(base + L.off_gather), count, total);
   KFAC_LAUNCH_CHECK();
   for (int i = 0; i < count; ++i) {
     const kfac_precond_item& it = items[i];
-    if (!is_diag_a(it)) continue;
+    if (!plans[i].transposed) continue;
     KFAC_CHECK_ARG(ceil_div(it.a, 32) <= 65535, "precond diagonal-A item: a");
     const dim3 grid((unsigned)ceil_div(ld4(it.g), 32), (unsigned)ceil_div(it.a, 32));
-    gather_t_kernel<<<grid, dim3(32, 8), 0, s>>>(it.wgrad, it.bgrad, it.grad_dtype, it.g, it.a, F(L.gr[i]), ld4(it.g));
+    gather_t_kernel<<<grid, dim3(32, 8), 0, s>>>(it.wgrad, it.bgrad, it.grad_dtype, it.g, it.a, plans[i].w.gr, ld4(it.g));
     KFAC_LAUNCH_CHECK();
   }
-  const float* ones = F(L.off_ones);
   if (L.ones_n && method == KFAC_INVERSE) {
-    fill_ones_kernel<<<grid_for(L.ones_n), 256, 0, s>>>(F(L.off_ones), L.ones_n);
+    fill_ones_kernel<<<grid_for(L.ones_n), 256, 0, s>>>((float*)(base + L.off_ones), L.ones_n);
     KFAC_LAUNCH_CHECK();
   }
-
+  // stage k of all items is one grouped launch (none where no item has a product in it)
   std::vector<GroupedGemm> st(count);
-  auto run = [&]() { return launch_grouped_gemm(st.data(), count, base + L.off_gemm, grouped_gemm_ws_bytes(count), s); };
-  auto plain = [&](int i, const float* A, int64_t lda, const float* B, int64_t ldb, float* D, int64_t ldd, int M, int N, int K) {
-    GroupedGemm g{};
-    g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.D = D; g.ldd = ldd; g.M = M; g.N = N; g.K = K; g.alpha = 1.f;
-    g.epi = EPI_NONE; g.splits = 1;
-    st[i] = g;
-  };
-  auto none = [&](int i) { st[i] = GroupedGemm{}; };   // M = N = K = 0: the item has no problem in this stage
-  // 1 / (vrow[v] * col[j] + damping) on the rows of a diagonal item's product: col = vcol (eigen) or ones (inverse)
-  auto div_rows = [&](int i, const DiagItem& D, const float* col) {
-    st[i].epi = EPI_DIV_OUTER; st[i].dg = D.vrow; st[i].da = col; st[i].damping = damping;
+  auto run = [&](int k) {
+    for (int i = 0; i < count; ++i) st[i] = plans[i].stage[k];
+    return launch_grouped_gemm(st.data(), count, base + L.off_gemm, grouped_gemm_ws_bytes(count), s);
   };
   int rc;
-  // the four (two) GEMMs of every layer form a chain; stage k of all layers is one grouped launch.  A diagonal
-  // item runs its first product in stage (1) (eigen) and its last in stage (4).
-  for (int i = 0; i < count; ++i) {     // (1) T^T[a', r] = sum_k (QaT | Ainv)[a', k] grad[r, k]          (a x g, K = a)
-    const kfac_precond_item& it = items[i];
-    const int g = it.g, a = it.a;
-    if (is_diag(it)) {                  // (1d) T[v, j] = (sum_k grad[v, k] Q[k, j]) / (vrow[v] vcol[j] + damping)   (rows x n, K = n)
-      const DiagItem D = diag_view(it);
-      if (it.kind == KFAC_ITEM_TIED) {  // (1t) T[v, j] = sum_k grad[v, k] M[k, j], divided by tied_scale_kernel below
-        plain(i, F(L.gr[i]), ld4(D.n), D.qT, D.ldq, F(L.t1[i]), ld4(D.n), D.rows, D.n, D.n);
-      } else if (method == KFAC_EIGEN) {
-        plain(i, F(L.gr[i]), ld4(D.n), D.qT, D.ldq, F(L.t1[i]), ld4(D.n), D.rows, D.n, D.n);
-        div_rows(i, D, D.vcol);
-      } else {
-        none(i);
-      }
-      continue;
-    }
-    plain(i, method == KFAC_EIGEN ? it.qaT : it.a_inv, it.ldqa, F(L.gr[i]), ld4(a), F(L.t1[i]), ld4(g), a, g, a);
-    if (L.splits_a[i] > 1) { st[i].splits = L.splits_a[i]; st[i].slab = F(L.slab_a[i]); st[i].slab_stride = (int64_t)a * ld4(g); }
+  if ((rc = run(0))) return rc;
+  // the tied items' division, elementwise over all of them in one launch
+  std::vector<TiedScaleDev> tied;
+  long long tied_total = 0;
+  for (const ItemPlan& p : plans) {
+    if (!p.tied) continue;
+    tied.push_back(p.tied_scale);
+    tied.back().elem0 = tied_total;
+    tied_total += (long long)p.stage[0].M * p.stage[0].ldd;
   }
-  if ((rc = run())) return rc;
-  {                                     // (1t') the tied items' division, elementwise over all of them in one launch
-    std::vector<TiedScaleDev> tied;
-    long long tied_total = 0;
-    for (int i = 0; i < count; ++i) {
-      if (items[i].kind != KFAC_ITEM_TIED) continue;
-      const DiagItem D = diag_view(items[i]);
-      tied.push_back(TiedScaleDev{F(L.t1[i]), D.vrow, D.vrow2, D.vcol, D.damping, D.n, ld4(D.n), tied_total});
-      tied_total += (long long)D.rows * ld4(D.n);
-    }
-    if (!tied.empty()) {
-      KFAC_CUDA(cudaMemcpyAsync(base + L.off_tied, tied.data(), sizeof(TiedScaleDev) * tied.size(),
-                                cudaMemcpyHostToDevice, s));
-      tied_scale_kernel<<<grid_for(tied_total), 256, 0, s>>>((const TiedScaleDev*)(base + L.off_tied), (int)tied.size(),
-                                                             tied_total);
-      KFAC_LAUNCH_CHECK();
-    }
+  if (!tied.empty()) {
+    KFAC_CUDA(cudaMemcpyAsync(base + L.off_tied, tied.data(), sizeof(TiedScaleDev) * tied.size(), cudaMemcpyHostToDevice, s));
+    tied_scale_kernel<<<grid_for(tied_total), 256, 0, s>>>((const TiedScaleDev*)(base + L.off_tied), (int)tied.size(),
+                                                           tied_total);
+    KFAC_LAUNCH_CHECK();
   }
-  if (method == KFAC_EIGEN) {
-    for (int i = 0; i < count; ++i) {   // (2) V2[g', a'] = (sum_k QgT[g', k] T^T[a', k]) * dgda[g', a']     (g x a, K = g)
-      const kfac_precond_item& it = items[i];
-      const int g = it.g, a = it.a;
-      if (is_diag(it)) { none(i); continue; }
-      plain(i, it.qgT, it.ldqg, F(L.t1[i]), ld4(g), F(L.t2[i]), ld4(a), g, a, g);
-      if (it.dgda) { st[i].epi = EPI_MUL; st[i].E = it.dgda; st[i].lde = it.ld_dgda; }
-      else { st[i].epi = EPI_DIV_OUTER; st[i].dg = it.dg; st[i].da = it.da; st[i].damping = damping; }
-    }
-    if ((rc = run())) return rc;
-    for (int i = 0; i < count; ++i) {   // (3) U^T[c, g'] = sum_k Qa[c, k] V2[g', k]                         (a x g, K = a)
-      const kfac_precond_item& it = items[i];
-      const int g = it.g, a = it.a;
-      if (is_diag(it)) { none(i); continue; }
-      plain(i, it.qa, it.ldqa, F(L.t2[i]), ld4(a), F(L.t1[i]), ld4(g), a, g, a);
-      if (L.splits_a[i] > 1) { st[i].splits = L.splits_a[i]; st[i].slab = F(L.slab_a[i]); st[i].slab_stride = (int64_t)a * ld4(g); }
-    }
-    if ((rc = run())) return rc;
-  }
-  for (int i = 0; i < count; ++i) {     // (4) P[r, c] = sum_k (Qg | Ginv)[r, k] U^T[c, k]                  (g x a, K = g)
-    const kfac_precond_item& it = items[i];
-    const int g = it.g, a = it.a;
-    int64_t p_rows = g, p_ld = ld4(a);
-    if (is_diag_a(it)) {
-      const DiagItem D = diag_view(it);
-      if (method == KFAC_EIGEN) {       // (4a) P[r, c] = sum_k Qg[r, k] T[c, k]  (g x a, K = g)
-        plain(i, D.q, D.ldq, F(L.t1[i]), ld4(D.n), it.P, it.ldp, D.n, D.rows, D.n);
-      } else {                          // (4a) P[r, c] = (sum_k Ginv[r, k] grad^T[c, k]) / (a[c] + damping)  (g x a, K = g)
-        plain(i, D.inv, D.ldq, F(L.gr[i]), ld4(D.n), it.P, it.ldp, D.n, D.rows, D.n);
-        st[i].epi = EPI_DIV_OUTER; st[i].dg = ones; st[i].da = D.vrow; st[i].damping = damping;
-      }
-      p_rows = D.n; p_ld = ld4(D.rows);
-    } else if (is_diag(it)) {
-      const DiagItem D = diag_view(it);
-      if (method == KFAC_EIGEN || it.kind == KFAC_ITEM_TIED) {   // (4d) P[v, c] = sum_k T[v, k] Q[c, k]  (rows x n, K = n)
-        plain(i, F(L.t1[i]), ld4(D.n), D.q, D.ldq, it.P, it.ldp, D.rows, D.n, D.n);
-      } else {                          // (4d) P[v, c] = (sum_k grad[v, k] Inv[c, k]) / (vrow[v] + damping)  (rows x n, K = n)
-        plain(i, F(L.gr[i]), ld4(D.n), D.inv, D.ldq, it.P, it.ldp, D.rows, D.n, D.n);
-        div_rows(i, D, ones);
-      }
-      p_rows = D.rows; p_ld = ld4(D.n);
-    } else {
-      plain(i, method == KFAC_EIGEN ? it.qg : it.g_inv, it.ldqg, F(L.t1[i]), ld4(g), it.P, it.ldp, g, a, g);
-    }
-    if (L.splits_g[i] > 1 && it.ldp == p_ld && st[i].epi == EPI_NONE) {
-      st[i].splits = L.splits_g[i]; st[i].slab = F(L.slab_g[i]); st[i].slab_stride = p_rows * p_ld;
-    }
-    // fused compute + broadcast: the same P goes to the peers, from the tile epilogue or from the split's reduce pass
-    st[i].npeer = it.n_peers;
-    for (int q = 0; q < it.n_peers; ++q) st[i].peerD[q] = it.peer_P[q];
-  }
-  return run();
+  for (int k = 1; k < 4; ++k)
+    if ((rc = run(k))) return rc;
+  return KFAC_OK;
 }
 
 extern "C" size_t kfac_grad_workspace_bytes(int count) {

@@ -69,8 +69,6 @@ __global__ void transpose_tied_kernel(const TiedDev* items) {
   }
 }
 
-int splits_for(int K) { return K > 1024 ? ceil_div(K, 512) : 1; }
-
 // workspace: [grouped-GEMM tables][TiedDev table][per item: X (d x ld), Y (d x ld), slab (splits x d x ld)]
 struct TiedLayout {
   size_t off_gemm, off_dev, total;
@@ -87,7 +85,7 @@ void tied_layout(const kfac_tied_item* items, int count, TiedLayout& L) {
     const size_t mat = (size_t)items[i].d * items[i].ld * sizeof(float);
     L.x[i] = take(mat);
     L.y[i] = take(mat);
-    if (splits_for(items[i].d) > 1) L.slab[i] = take(splits_for(items[i].d) * mat);
+    if (chain_splits(items[i].d) > 1) L.slab[i] = take(chain_splits(items[i].d) * mat);
   }
   L.total = off;
 }
@@ -96,7 +94,7 @@ GroupedGemm product(const float* A, const float* B, float* D, int d, int ld, flo
   GroupedGemm g{};
   g.A = A; g.lda = ld; g.B = B; g.ldb = ld; g.D = D; g.ldd = ld; g.M = d; g.N = d; g.K = d; g.alpha = 1.f;
   g.epi = EPI_NONE; g.splits = 1;
-  if (splits_for(d) > 1) { g.splits = splits_for(d); g.slab = slab; g.slab_stride = (int64_t)d * ld; }
+  if (chain_splits(d) > 1) { g.splits = chain_splits(d); g.slab = slab; g.slab_stride = (int64_t)d * ld; }
   return g;
 }
 

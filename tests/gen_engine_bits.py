@@ -2,7 +2,7 @@
 
 Needs one H100.  Every case runs a seeded set of engine calls and hashes the exact output bits (SHA-256 of the
 float32 arrays), so a change to the engine's schedule, staging or register use can be checked to leave every bit
-of every output where it was:
+of every output where it was.  Each case's kernel launches (kfac_launch_count) are recorded beside its digest:
 
     python tests/gen_engine_bits.py [OUT.json]        # default: tests/golden/engine_bits.json
 
@@ -222,6 +222,99 @@ def case_precondition():
     return _digest(*outs)
 
 
+def _precond_item(gen, keep, kind, g, a, bias=False, epi='dadg', taps=0, ldp_pad=0):
+    """One kfac_precondition item of any kind, with every second-order operand filled (seeded), so that both methods
+    can run on it.  g and a are the item's fields: for an embedding or tied item g = d and a = V.  Returns the item
+    and its P (rows x ldp, ldp = ld4 of P's columns + ldp_pad)."""
+    ld4 = _cabi.ld4
+
+    def mat(n):                                       # n x ld4(n), zero padding columns
+        m = torch.zeros(n, ld4(n), device=_dev())
+        m[:, :n] = _randn(gen, n, n) / n ** 0.5
+        return m
+
+    def vec(n):
+        return _randn(gen, n).abs() + 0.1
+
+    it = _cabi.PrecondItem()
+    it.kind, it.g, it.a, it.grad_dtype, it.wgrad_taps = kind, g, a, 0, taps
+    transposed_rows = kind in (_cabi.KFAC_ITEM_EMBEDDING, _cabi.KFAC_ITEM_TIED)   # wgrad is (a, g) = (V, d)
+    rows, cols = (a, g) if transposed_rows else (g, a)
+    hb = 1 if bias else 0
+    w = _randn(gen, (cols - hb) // taps, rows, taps) if taps else _randn(gen, rows, cols - hb)
+    b = _randn(gen, rows) if bias else None
+    it.wgrad, it.bgrad = w.data_ptr(), (b.data_ptr() if bias else None)
+    keep.extend([w, b])
+    fields = {}
+    if kind in (_cabi.KFAC_ITEM_DENSE, _cabi.KFAC_ITEM_DIAG_G):
+        fields.update(qa=mat(a), qaT=mat(a), a_inv=mat(a), da=vec(a))
+        it.ldqa = ld4(a)
+    if kind in (_cabi.KFAC_ITEM_DENSE, _cabi.KFAC_ITEM_EMBEDDING, _cabi.KFAC_ITEM_TIED, _cabi.KFAC_ITEM_DIAG_A):
+        fields.update(qg=mat(g), qgT=mat(g), g_inv=mat(g), dg=vec(g))
+        it.ldqg = ld4(g)
+    if kind != _cabi.KFAC_ITEM_DENSE and 'da' not in fields:
+        fields['da'] = vec(a)
+    if kind == _cabi.KFAC_ITEM_DIAG_G:
+        fields['dg'] = vec(g)
+    if kind == _cabi.KFAC_ITEM_DENSE and epi == 'dgda':
+        fields['dgda'] = _randn(gen, g, ld4(a)).abs() + 0.1
+        it.ld_dgda = ld4(a)
+    if kind == _cabi.KFAC_ITEM_TIED:
+        fields['dh'] = vec(a)
+        it.tied_damping = 0.25
+    for name, t in fields.items():
+        setattr(it, name, t.data_ptr())
+        keep.append(t)
+    it.ldp = ld4(cols) + ldp_pad
+    P = torch.zeros(rows, it.ldp, device=_dev())
+    it.P = P.data_ptr()
+    return it, P
+
+
+def case_precondition_kinds(method, specs):
+    """One kfac_precondition call over the items of `specs` ((kind, g, a, options) each) with the given method."""
+    lib = _cabi.load()
+    gen = torch.Generator().manual_seed(11)
+    keep, outs = [], []
+    items = (_cabi.PrecondItem * len(specs))()
+    for i, (kind, g, a, opts) in enumerate(specs):
+        items[i], P = _precond_item(gen, keep, kind, g, a, **opts)
+        outs.append(P)
+    need = lib.kfac_precondition_workspace_bytes(items, len(specs))
+    ws = torch.zeros(need, dtype=torch.uint8, device=_dev())
+    rc = lib.kfac_precondition(items, len(specs), method, 3e-3, ws.data_ptr(), need, _stream())
+    assert rc == 0, lib.kfac_last_error()
+    return _digest(*outs)
+
+
+DENSE, EMB, DIAG_G, TIED, DIAG_A = (_cabi.KFAC_ITEM_DENSE, _cabi.KFAC_ITEM_EMBEDDING, _cabi.KFAC_ITEM_DIAG_G,
+                                    _cabi.KFAC_ITEM_TIED, _cabi.KFAC_ITEM_DIAG_A)
+EIGEN, INVERSE = _cabi.KFAC_EIGEN, _cabi.KFAC_INVERSE
+# every item kind and method; a > 1024 splits stages (1) and (3), g > 1024 (n > 1024 for a diagonal item) stage (4)
+PRECOND_CASES = {
+    'dense_dgda': (EIGEN, [(DENSE, 300, 1501, dict(bias=True, epi='dgda')), (DENSE, 1500, 300, dict(epi='dgda')),
+                           (DENSE, 96, 130, dict(bias=True, epi='dgda'))]),
+    'dense_dadg': (EIGEN, [(DENSE, 300, 1501, dict(bias=True)), (DENSE, 1500, 300, {}), (DENSE, 96, 130, {})]),
+    'dense_inverse': (INVERSE, [(DENSE, 300, 1501, dict(bias=True)), (DENSE, 1500, 300, {}), (DENSE, 96, 130, {})]),
+    'conv_transpose_eigen': (EIGEN, [(DENSE, 96, 40 * 9 + 1, dict(bias=True, taps=9))]),
+    'conv_transpose_inverse': (INVERSE, [(DENSE, 1100, 24 * 27, dict(taps=27))]),
+    'embedding_eigen': (EIGEN, [(EMB, 1000, 3000, {}), (EMB, 1100, 2000, {})]),
+    'embedding_inverse': (INVERSE, [(EMB, 1000, 3000, {}), (EMB, 1100, 2000, {})]),
+    'diag_g_eigen': (EIGEN, [(DIAG_G, 3000, 1000, dict(bias=True)), (DIAG_G, 2000, 1101, dict(bias=True))]),
+    'diag_g_inverse': (INVERSE, [(DIAG_G, 3000, 1000, dict(bias=True)), (DIAG_G, 2000, 1101, dict(bias=True))]),
+    'diag_a_eigen': (EIGEN, [(DIAG_A, 1100, 3001, dict(bias=True)), (DIAG_A, 500, 2000, {})]),
+    'diag_a_inverse': (INVERSE, [(DIAG_A, 1100, 3001, dict(bias=True)), (DIAG_A, 500, 2000, {})]),
+    'tied_eigen': (EIGEN, [(TIED, 1100, 3000, {}), (TIED, 200, 1500, {})]),
+    'mixed_eigen': (EIGEN, [(DENSE, 1100, 1200, dict(bias=True)), (EMB, 1100, 2000, {}),
+                            (DIAG_G, 1500, 1030, dict(bias=True)), (TIED, 300, 1000, {}), (DIAG_A, 1050, 2001, dict(bias=True)),
+                            (DENSE, 64, 40 * 4, dict(taps=4))]),
+    'mixed_inverse': (INVERSE, [(DENSE, 1100, 1200, dict(bias=True)), (EMB, 1100, 2000, {}),
+                                (DIAG_G, 1500, 1030, dict(bias=True)), (TIED, 300, 1000, {}),
+                                (DIAG_A, 1050, 2001, dict(bias=True)), (DENSE, 64, 40 * 4, dict(taps=4))]),
+    'ldp_padded': (EIGEN, [(DENSE, 1500, 300, dict(ldp_pad=8)), (EMB, 1100, 2000, dict(ldp_pad=4))]),
+}
+
+
 CASES = {
     'gemm_tn_tc_4096': lambda: case_gemm_tn_tc(4096, 4096, 4096),
     'gemm_tn_tc_odd_1000x777x1234': lambda: case_gemm_tn_tc(1000, 777, 1234),
@@ -232,18 +325,28 @@ CASES = {
     'factor_syrk_one_split': lambda: case_factor_syrk(False),
     'eigh_r50': case_eigh_r50,
     'precondition_eigen': case_precondition,
+    **{f'precondition_{name}': (lambda m=m, s=s: case_precondition_kinds(m, s)) for name, (m, s) in PRECOND_CASES.items()},
 }
+
+
+def run(name):
+    """(digest, native kernel launches) of one case"""
+    lib = _cabi.load()
+    before = lib.kfac_launch_count()
+    digest = CASES[name]()
+    return digest, lib.kfac_launch_count() - before
 
 
 def main():
     out = sys.argv[1] if len(sys.argv) > 1 else GOLDEN
-    res = {}
-    for name, fn in CASES.items():
-        res[name] = fn()
-        print(name, res[name], flush=True)
+    res, launches = {}, {}
+    for name in CASES:
+        res[name], launches[name] = run(name)
+        print(name, res[name], launches[name], flush=True)
     os.makedirs(os.path.dirname(os.path.abspath(out)), exist_ok=True)
     with open(out, 'w') as f:
-        json.dump({'device': torch.cuda.get_device_name(0), 'digests': res}, f, indent=1, sort_keys=True)
+        json.dump({'device': torch.cuda.get_device_name(0), 'digests': res, 'launches': launches}, f, indent=1,
+                  sort_keys=True)
         f.write('\n')
     print('wrote', out)
 
