@@ -358,6 +358,33 @@ int kfac_dgda(const float* dg, const float* da, int g, int a, float damping,
 int kfac_inverse_from_eigh(const float* Q, int ldq, const float* d, int n,
                            float damping, float* inv, int ld_inv, void* ws,
                            size_t ws_bytes, void* stream);
+/* pi-adjusted (factored Tikhonov) damping (Martens & Grosse 2015, sec. 6.3; an extension beyond the reference,
+ * opt-in): the damping lambda of the Kronecker product A (x) G is split between the factors by their trace norms,
+ *     pi = sqrt((tr A / a) / (tr G / g)),    s = sqrt(lambda),    gamma_A = s * pi,    gamma_G = s / pi,
+ * so that (A + gamma_A I) (x) (G + gamma_G I) does not depend on how the scale of the product is split between A and G.
+ * kfac_pi: pi of every item, one launch per 768 items (one block each).  A factor is dense (ld >= its dimension; its
+ * diagonal is read) or a vector (ld = 0: a diagonal factor, its own diagonal).  Both traces are summed in fp64 in a
+ * fixed order (no atomics: repeat calls give the same bits), pi is rounded once to fp32, and it is 1 where a mean
+ * trace is not a positive finite number (or pi does not round to a positive finite float).  No host sync, no
+ * workspace. */
+typedef struct kfac_pi_item {
+  const float* A;  /* a x a (ld = lda), or a floats (lda = 0) */
+  const float* G;  /* g x g (ld = ldg), or g floats (ldg = 0) */
+  float* pi;       /* out: one float */
+  int a, g;
+  int lda, ldg;
+} kfac_pi_item;
+int kfac_pi(const kfac_pi_item* items, int count, void* stream);
+/* kfac_dgda with pi: out[i,j] = 1 / ((dg[i] + gamma_G) * (da[j] + gamma_A)), gamma_A = s * *pi, gamma_G = s / *pi
+ * (fp32, each rounded on its own); s on the host, pi a DEVICE float. */
+int kfac_dgda_pi(const float* dg, const float* da, int g, int a, float s, const float* pi,
+                 float* out, int ld_out, void* stream);
+/* kfac_inverse_from_eigh with the damping gamma of one factor: side +1 (A) gamma = s * *pi, side -1 (G)
+ * gamma = s / *pi; inv = Q diag(1 / (d + gamma)) Q^T with the same workspace, products and bits as
+ * kfac_inverse_from_eigh with damping = gamma. */
+int kfac_inverse_from_eigh_pi(const float* Q, int ldq, const float* d, int n, float s,
+                              const float* pi, int side, float* inv, int ld_inv, void* ws,
+                              size_t ws_bytes, void* stream);
 /* dst (cols x rows, ld_dst) = src^T (src rows x cols, ld_src): gives a rank that
  * received an eigenbasis by broadcast the K-major copy the GEMM engine wants */
 int kfac_transpose(const float* src, int ld_src, float* dst, int ld_dst, int rows,
@@ -404,7 +431,16 @@ int kfac_transpose(const float* src, int ld_src, float* dst, int ld_dst, int row
  * is the EPI_DIV_OUTER epilogue of the first product), the last one formed transposed so that P is
  * g x a.  The two (one) GEMMs join the grouped launches; the last one is split into chains of at
  * most 512 for g > 1024 (eigen), and its peer stores give the bits of the local P.  The other
- * items' results do not depend on diagonal-A items. */
+ * items' results do not depend on diagonal-A items.
+ * pi-adjusted damping (pi != NULL, a DEVICE float from kfac_pi; every kind but KFAC_ITEM_TIED, which rejects it with
+ * KFAC_ERR_BAD_ARG): with s = sqrtf(damping), gamma_A = s * *pi and gamma_G = s / *pi, every division by
+ * (u x v + damping) above, u and v the eigenvalues (or diagonals) of the two factors, becomes a division by
+ * (u + gamma_u) x (v + gamma_v) (the EPI_DIV_FACTORED epilogue), and each one-sided division of the INVERSE method
+ * takes the gamma of its diagonal factor.  So
+ *   dense EIGEN (no dgda):  P = Qg [(Qg^T grad Qa) / ((dg + gamma_G) x (da + gamma_A))] Qa^T
+ *   embedding EIGEN:        P = [(wgrad Qg) / ((da + gamma_A) x (dg + gamma_G))] Qg^T
+ *   diagonal-G INVERSE:     P = diag(1 / (dg + gamma_G)) grad Ainv,   and likewise for the other kinds.
+ * dgda, a_inv and g_inv are used as given (kfac_dgda_pi and kfac_inverse_from_eigh_pi form them with pi). */
 enum kfac_item_kind {
   KFAC_ITEM_DENSE = 0, KFAC_ITEM_EMBEDDING = 1, KFAC_ITEM_DIAG_G = 2, KFAC_ITEM_TIED = 3, KFAC_ITEM_DIAG_A = 4
 };
@@ -443,6 +479,9 @@ typedef struct kfac_precond_item {
    * (g, a - has_bias); T > 0 = a transposed convolution's (C_in, g, T) weight gradient, whose
    * grad-matrix element (r, ci * T + t) lies at wgrad[(ci * g + r) * T + t].  P stays (g, a). */
   int wgrad_taps;
+  /* pi-adjusted damping: a DEVICE float (kfac_pi) or NULL (the initialisers written before this field) for the
+   * damping above, with its bits */
+  const float* pi;
 } kfac_precond_item;
 size_t kfac_precondition_workspace_bytes(const kfac_precond_item* items, int count);
 int kfac_precondition(const kfac_precond_item* items, int count, int method,

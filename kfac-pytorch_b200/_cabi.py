@@ -60,7 +60,13 @@ class PrecondItem(C.Structure):
                 ('ldqa', c_int), ('ldqg', c_int), ('ld_dgda', c_int),
                 ('P', c_void_p), ('ldp', c_int),
                 ('peer_P', C.POINTER(c_void_p)), ('n_peers', c_int), ('kind', c_int),
-                ('dh', c_void_p), ('tied_damping', c_float), ('wgrad_taps', c_int)]
+                ('dh', c_void_p), ('tied_damping', c_float), ('wgrad_taps', c_int), ('pi', c_void_p)]
+
+
+class PiItem(C.Structure):
+    """kfac_pi_item: the factors of one layer (ld 0: a vector factor) and its pi slot."""
+    _fields_ = [('A', c_void_p), ('G', c_void_p), ('pi', c_void_p), ('a', c_int), ('g', c_int), ('lda', c_int),
+                ('ldg', c_int)]
 
 
 class TiedItem(C.Structure):
@@ -156,6 +162,10 @@ SIGNATURES = {
     'kfac_eigh_status': (c_int, [c_void_p, c_void_p, c_void_p]),
     'kfac_dgda': (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_int, c_void_p]),
     'kfac_inverse_from_eigh': (c_int, [c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
+    'kfac_pi': (c_int, [C.POINTER(PiItem), c_int, c_void_p]),
+    'kfac_dgda_pi': (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p]),
+    'kfac_inverse_from_eigh_pi': (c_int, [c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_int, c_void_p, c_int,
+                                          c_void_p, c_size_t, c_void_p]),
     'kfac_transpose': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     'kfac_precondition_workspace_bytes': (c_size_t, [C.POINTER(PrecondItem), c_int]),
     'kfac_precondition': (c_int, [C.POINTER(PrecondItem), c_int, c_int, c_float, c_void_p, c_size_t, c_void_p]),

@@ -230,8 +230,20 @@ def second_order_layout(layer: KFACLayer) -> Layout:
         item = dict(kind=_cabi.KFAC_ITEM_DENSE, ldqa=ld4(a), ldqg=ld4(g), ld_dgda=ld4(a))
         if layer.module.wgrad_taps:     # a transposed convolution's (C_in, g, T) weight gradient
             item['wgrad_taps'] = layer.module.wgrad_taps
+    if layer.pi_damping:
+        # pi-adjusted damping: every rank forms pi of every layer from the all-reduced factors at each inverse step;
+        # the damped dgda and inverses read it, and so does the precondition
+        entries += (E('pi', (1,), 'all'),)
+        needs = set(needs) | {'pi'}
+        post = tuple((holder, op, keys + ('pi',)) for holder, op, keys in post)
     fields = tuple((e.key.lstrip('_'), e.key) for e in entries if e.shipped or e.holder in ('grad', 'all'))
     return Layout(entries, factors, snapshots, decompositions, post, frozenset(needs), unready, fields, item, eigen)
+
+
+def pi_s(damping: float) -> float:
+    """s = sqrt(damping) of pi-adjusted damping, as kfac_precondition forms it: the fp32 square root of the fp32 damping
+    (the square root in fp64 of a float, rounded to a float, is the correctly rounded fp32 square root)."""
+    return C.c_float(math.sqrt(C.c_float(damping).value)).value
 
 
 def _holds(holder: str, name: str, assignment: WorkAssignment, rank: int) -> bool:
@@ -1167,21 +1179,45 @@ class BaseKFACPreconditioner:
             self._eig_slots = list(range(len(batches))) + ([2] if snapshots else []) + ([3] if tied else [])
             self._eig_event.record()
             self._eig_pending = True
+        # pi of the layers with pi-adjusted damping, from the factors just decomposed: every rank forms it for every
+        # such layer from its copy of the all-reduced factors, in one launch and with the same bits, so it needs no
+        # collective; it is kept until the next inverse step
+        pi_layers = [l for l in self._layouts if l.pi_damping]
+        if pi_layers:
+            items = (_cabi.PiItem * len(pi_layers))()
+            for i, l in enumerate(pi_layers):
+                items[i] = _cabi.PiItem(l._a_view.data_ptr(), l._g_view.data_ptr(), l._inv['pi'].data_ptr(), l.a_dim,
+                                        l.g_dim, 0 if l.diag_a else l.a_dim, 0 if l.diag_g else l.g_dim)
+                l._inv_ready.add('pi')
+            _cabi.check(lib.kfac_pi(items, len(pi_layers), stream), 'kfac_pi')
+        s = pi_s(damping)
         for layer, op, keys in post:
             I = layer._inv
             if op == 'dgda':
-                dg, da, dgda = keys
-                _cabi.check(lib.kfac_dgda(I[dg].data_ptr(), I[da].data_ptr(), layer.g_dim, layer.a_dim, damping,
-                                          I[dgda].data_ptr(), _cabi.ld4(layer.a_dim), stream), 'kfac_dgda')
+                dg, da, dgda, *pi = keys
+                if pi:
+                    _cabi.check(lib.kfac_dgda_pi(I[dg].data_ptr(), I[da].data_ptr(), layer.g_dim, layer.a_dim, s,
+                                                 I[pi[0]].data_ptr(), I[dgda].data_ptr(), _cabi.ld4(layer.a_dim),
+                                                 stream), 'kfac_dgda_pi')
+                else:
+                    _cabi.check(lib.kfac_dgda(I[dg].data_ptr(), I[da].data_ptr(), layer.g_dim, layer.a_dim, damping,
+                                              I[dgda].data_ptr(), _cabi.ld4(layer.a_dim), stream), 'kfac_dgda')
             elif op == 'inverse':
-                q, d, inv = keys
+                q, d, inv, *pi = keys
                 n = I[q].shape[0]
                 ld = _cabi.ld4(n)
                 need = n * ld * 4
                 ws = self._gemm_scratch.get(need, self._device)
-                _cabi.check(lib.kfac_inverse_from_eigh(I[q].data_ptr(), ld, I[d].data_ptr(), n, damping,
-                                                       I[inv].data_ptr(), ld, ws.data_ptr(), need, stream),
-                            'kfac_inverse_from_eigh')
+                if pi:
+                    # gamma_A = s pi for A's inverse, gamma_G = s / pi for G's
+                    _cabi.check(lib.kfac_inverse_from_eigh_pi(I[q].data_ptr(), ld, I[d].data_ptr(), n, s,
+                                                              I[pi[0]].data_ptr(), 1 if inv == 'a_inv' else -1,
+                                                              I[inv].data_ptr(), ld, ws.data_ptr(), need, stream),
+                                'kfac_inverse_from_eigh_pi')
+                else:
+                    _cabi.check(lib.kfac_inverse_from_eigh(I[q].data_ptr(), ld, I[d].data_ptr(), n, damping,
+                                                           I[inv].data_ptr(), ld, ws.data_ptr(), need, stream),
+                                'kfac_inverse_from_eigh')
         # C2: one broadcast per (source, gradient-worker group)
         bcast = self._assignment.broadcast_inverses()
         for seg in self._inv_segments:

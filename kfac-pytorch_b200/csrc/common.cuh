@@ -186,7 +186,21 @@ __device__ __forceinline__ void store_from_float(void* p, int dtype, int64_t i, 
 }
 
 // ---------------------------------------------------------------- SIMT GEMM
-enum GemmEpilogue { EPI_NONE = 0, EPI_MUL = 1, EPI_DIV_OUTER = 2, EPI_SQUARE = 3 };   // EPI_SQUARE: store x^2
+// EPI_SQUARE: store x^2.  EPI_DIV_FACTORED: x / ((dg[m] + gamma_m) (da[n] + gamma_n)), the factored (pi-adjusted)
+// Tikhonov damping, with damping = s and gamma_m = pi_gamma(s, *pi, pi_side_m), gamma_n likewise
+enum GemmEpilogue { EPI_NONE = 0, EPI_MUL = 1, EPI_DIV_OUTER = 2, EPI_SQUARE = 3, EPI_DIV_FACTORED = 4 };
+
+// The damping of one Kronecker factor under pi-adjusted damping: side +1 (the A factor) s * pi, side -1 (the G
+// factor) s / pi, side 0 (no factor: a vector of ones) 0.  Rounded on its own (never fused into the add that follows),
+// so that it is the fp32 gamma the caller would form.
+__device__ __forceinline__ float pi_gamma(float s, float pi, int side) {
+  return side > 0 ? __fmul_rn(s, pi) : side < 0 ? __fdiv_rn(s, pi) : 0.f;
+}
+__device__ __forceinline__ float div_factored(float x, float dm, float dn, float s, const float* pi, int side_m,
+                                              int side_n) {
+  const float p = *pi;
+  return x / (__fmul_rn(__fadd_rn(dm, pi_gamma(s, p, side_m)), __fadd_rn(dn, pi_gamma(s, p, side_n))));
+}
 
 struct GemmArgs {
   const float* A; int64_t sa_m, sa_k, sa_b;   // A(m,k) = A[b*sa_b + m*sa_m + k*sa_k]
@@ -199,7 +213,8 @@ struct GemmArgs {
   float alpha, beta;
   int epi;
   const float* E; int64_t lde;   // EPI_MUL: C *= E[m*lde+n]
-  const float* dg; const float* da; float damping;  // EPI_DIV_OUTER
+  const float* dg; const float* da; float damping;  // EPI_DIV_OUTER; EPI_DIV_FACTORED (damping = s)
+  const float* pi; int pi_side_m, pi_side_n;        // EPI_DIV_FACTORED
 };
 
 int launch_gemm(const GemmArgs& g, cudaStream_t stream);
@@ -220,6 +235,7 @@ struct TcGemmArgs {
   int splits;                      // <= 0: automatic
   float alpha;
   int epi; const float* E; int64_t lde; const float* dg; const float* da; float damping;
+  const float* pi; int pi_side_m, pi_side_n;   // EPI_DIV_FACTORED
   float* peerD[7]; int npeer;      // fused broadcast: the epilogue also stores the tile into these peer copies of D
 };
 bool tc_gemm_supported(const TcGemmArgs& a);

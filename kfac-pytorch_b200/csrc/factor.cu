@@ -6,6 +6,9 @@
 // are read in their native NCHW / (rows, features) layout.
 #include "common.cuh"
 
+#include <cfloat>
+#include <string.h>
+
 #include <algorithm>
 #include <type_traits>
 
@@ -552,6 +555,57 @@ __global__ void dgda_kernel(const float* dg, const float* da, int g, int a, floa
   }
 }
 
+// out[i][j] = 1 / ((dg[i] + gamma_G) (da[j] + gamma_A)), gamma_A = s pi, gamma_G = s / pi; zero in the padding columns
+__global__ void dgda_pi_kernel(const float* dg, const float* da, int g, int a, float s, const float* pi, float* out,
+                               int ldo) {
+  const float p = *pi, gam_a = pi_gamma(s, p, 1), gam_g = pi_gamma(s, p, -1);
+  const int64_t total = (int64_t)g * ldo;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (int64_t)gridDim.x * blockDim.x) {
+    const int j = (int)(idx % ldo);
+    out[idx] = j < a ? 1.f / __fmul_rn(__fadd_rn(dg[idx / ldo], gam_g), __fadd_rn(da[j], gam_a)) : 0.f;
+  }
+}
+
+// pi of up to PI_BATCH items, one block each: the traces of A and G summed in fp64 (a fixed assignment of the diagonal
+// entries to the threads and a fixed reduction tree, so the same factors give the same bits), then
+// pi = sqrt((tr A / a) / (tr G / g)) rounded once to fp32, or 1 where a mean or pi is not a positive finite number
+constexpr int PI_BATCH = 768;
+struct PiBatch { kfac_pi_item it[PI_BATCH]; };
+static_assert(sizeof(PiBatch) <= 32000, "kernel parameter space");
+
+__device__ double block_sum(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double t = 0.0;
+  for (int k = 0; k < (int)(blockDim.x >> 5); ++k) t += red[k];
+  __syncthreads();
+  return t;
+}
+
+__device__ double trace_of(const float* F, int n, int ld, double* red) {
+  const int64_t step = (int64_t)ld + 1;   // ld 0: a vector, its own diagonal
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) acc += (double)F[i * step];
+  return block_sum(acc, red);
+}
+
+__global__ void __launch_bounds__(256) pi_kernel(const __grid_constant__ PiBatch b) {
+  __shared__ double red[8];
+  const kfac_pi_item& it = b.it[blockIdx.x];
+  const double ma = trace_of(it.A, it.a, it.lda, red) / it.a;
+  const double mg = trace_of(it.G, it.g, it.ldg, red) / it.g;
+  if (threadIdx.x != 0) return;
+  float pi = 1.f;
+  if (ma > 0.0 && ma <= DBL_MAX && mg > 0.0 && mg <= DBL_MAX) {
+    const float p = (float)sqrt(ma / mg);
+    if (p > 0.f && p <= FLT_MAX) pi = p;
+  }
+  *it.pi = pi;
+}
+
 __global__ void triu_pack_kernel(const float* F, int n, float* packed) {
   const int64_t total = (int64_t)n * n;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -1070,6 +1124,31 @@ extern "C" int kfac_dgda(const float* dg, const float* da, int g, int a, float d
   KFAC_CHECK_ARG(dg && da && out && g > 0 && a > 0 && ld_out >= a, "dgda args");
   dgda_kernel<<<grid_for((int64_t)g * ld_out), 256, 0, (cudaStream_t)stream>>>(dg, da, g, a, damping, out, ld_out);
   KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
+extern "C" int kfac_dgda_pi(const float* dg, const float* da, int g, int a, float s, const float* pi, float* out,
+                            int ld_out, void* stream) {
+  KFAC_CHECK_ARG(dg && da && pi && out && g > 0 && a > 0 && ld_out >= a, "dgda_pi args");
+  dgda_pi_kernel<<<grid_for((int64_t)g * ld_out), 256, 0, (cudaStream_t)stream>>>(dg, da, g, a, s, pi, out, ld_out);
+  KFAC_LAUNCH_CHECK();
+  return KFAC_OK;
+}
+
+extern "C" int kfac_pi(const kfac_pi_item* items, int count, void* stream) {
+  KFAC_CHECK_ARG(count >= 0 && (items || count == 0), "pi args");
+  for (int i = 0; i < count; ++i) {
+    const kfac_pi_item& it = items[i];
+    KFAC_CHECK_ARG(it.A && it.G && it.pi && it.a > 0 && it.g > 0 && (it.lda == 0 || it.lda >= it.a) &&
+                       (it.ldg == 0 || it.ldg >= it.g), "pi item");
+  }
+  for (int i0 = 0; i0 < count; i0 += PI_BATCH) {
+    const int n = std::min(PI_BATCH, count - i0);
+    PiBatch b;
+    memcpy(b.it, items + i0, sizeof(kfac_pi_item) * n);
+    pi_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(b);
+    KFAC_LAUNCH_CHECK();
+  }
   return KFAC_OK;
 }
 

@@ -27,6 +27,7 @@ struct alignas(128) GProb {
   int work0;                       // first work item of this problem
   float alpha;
   int epi; const float* E; int64_t lde; const float* dg; const float* da; float damping;
+  const float* pi; int pi_side_m, pi_side_n;
   int64_t slab_stride;             // != 0: D is the slab base, split sp stores to D + sp * slab_stride
   int mode;                        // 0 store, 1 read-modify-write accumulate, 2 atomicAdd
   const int* krange;               // device-side {first, end} k-block of the reduction (mode 2), or null
@@ -35,6 +36,9 @@ struct alignas(128) GProb {
 
 struct GroupedParams { const GProb* probs; int nprobs; };
 
+// FACTORED: the instantiation that also takes EPI_DIV_FACTORED, launched only for a list with such a problem, so that
+// the epilogue of every other launch stays as compact as it was
+template <bool FACTORED>
 struct GroupedPolicy {
   using Params = GroupedParams;
   struct Item { const GProb* pr; int m0, n0, kb0, kb1, sp, idx; };
@@ -72,6 +76,7 @@ struct GroupedPolicy {
   struct Out {
     float* D; int64_t ldd; int M, N, m0, n0;
     float alpha; int epi; const float* E; int64_t lde; const float* dg; const float* da; float damping;
+    const float* pi; int pi_side_m, pi_side_n;
     int mode, npeer; const GProb* pr;
   };
   __device__ static Out out(const Params&, const Item& it) {
@@ -79,6 +84,7 @@ struct GroupedPolicy {
     Out o;
     o.D = p.D + (int64_t)it.sp * p.slab_stride; o.ldd = p.ldd; o.M = p.M; o.N = p.N; o.m0 = it.m0; o.n0 = it.n0;
     o.alpha = p.alpha; o.epi = p.epi; o.E = p.E; o.lde = p.lde; o.dg = p.dg; o.da = p.da; o.damping = p.damping;
+    o.pi = p.pi; o.pi_side_m = p.pi_side_m; o.pi_side_n = p.pi_side_n;
     o.mode = p.mode; o.npeer = p.npeer; o.pr = it.pr;
     return o;
   }
@@ -93,6 +99,8 @@ struct GroupedPolicy {
         if (p.epi == EPI_MUL) x *= p.E[(int64_t)m * p.lde + nb + j];
         else if (p.epi == EPI_DIV_OUTER) x = x / (p.dg[m] * p.da[nb + j] + p.damping);
         else if (p.epi == EPI_SQUARE) x = x * x;
+        else if (FACTORED && p.epi == EPI_DIV_FACTORED)
+          x = div_factored(x, p.dg[m], p.da[nb + j], p.damping, p.pi, p.pi_side_m, p.pi_side_n);
       }
       v[j] = x;
     }
@@ -172,8 +180,10 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
   }
   static bool attr = false;
   if (!attr) {
-    KFAC_CUDA(cudaFuncSetAttribute(tc::pipeline_kernel<GroupedPolicy>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)tc::PSMEM));
+    KFAC_CUDA(cudaFuncSetAttribute(tc::pipeline_kernel<GroupedPolicy<false>>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::PSMEM));
+    KFAC_CUDA(cudaFuncSetAttribute(tc::pipeline_kernel<GroupedPolicy<true>>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::PSMEM));
     attr = true;
   }
   // the arguments of every problem are checked (and every tensor map encoded) before anything is launched: a
@@ -206,6 +216,7 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
     if ((rc = make_tmap_3d(&p.tmB, g.B, (uint64_t)g.K, (uint64_t)g.N, 1, (uint64_t)g.ldb * 4, (uint64_t)g.ldb * 4 * g.N, GBM))) return rc;
     p.M = g.M; p.N = g.N; p.K = g.K; p.ldd = g.ldd; p.alpha = g.alpha;
     p.epi = g.epi; p.E = g.E; p.lde = g.lde; p.dg = g.dg; p.da = g.da; p.damping = g.damping;
+    p.pi = g.pi; p.pi_side_m = g.pi_side_m; p.pi_side_n = g.pi_side_n;
     p.tiles_n = ceil_div(g.N, GBN);
     const int tiles = ceil_div(g.M, GBM) * p.tiles_n;
     p.kb_total = ceil_div(g.K, GBK);
@@ -239,6 +250,7 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
     a.A = g.A; a.sa_m = g.lda; a.sa_k = 1; a.B = g.B; a.sb_k = 1; a.sb_n = g.ldb;
     a.C = g.D; a.ldc = g.ldd; a.M = g.M; a.N = g.N; a.K = g.K; a.batch = 1; a.splitk = 1;
     a.alpha = g.alpha; a.beta = g.mode == 0 ? 0.f : 1.f; a.epi = g.epi; a.E = g.E; a.lde = g.lde; a.dg = g.dg; a.da = g.da; a.damping = g.damping;
+    a.pi = g.pi; a.pi_side_m = g.pi_side_m; a.pi_side_n = g.pi_side_n;
     int rc = launch_gemm(a, s);
     if (rc) return rc;
     if (g.npeer > 0) {
@@ -256,7 +268,9 @@ int launch_grouped_gemm(const GroupedGemm* probs, int count, void* ws, size_t ws
   GroupedParams gp{d_tab, (int)tab.size()};
   const int sms = max_ctas > 0 ? std::min(max_ctas, tc_num_sms()) : tc_num_sms();
   const int grid = std::min(work, sms);
-  tc::pipeline_kernel<GroupedPolicy><<<grid, tc::PTHREADS, tc::PSMEM, s>>>(gp, work);
+  const bool factored = std::any_of(tab.begin(), tab.end(), [](const GProb& p) { return p.epi == EPI_DIV_FACTORED; });
+  if (factored) tc::pipeline_kernel<GroupedPolicy<true>><<<grid, tc::PTHREADS, tc::PSMEM, s>>>(gp, work);
+  else tc::pipeline_kernel<GroupedPolicy<false>><<<grid, tc::PTHREADS, tc::PSMEM, s>>>(gp, work);
   KFAC_LAUNCH_CHECK();
   if (!red.empty()) {
     if ((rc = send_table(stage, d_red, red.data(), sizeof(RProb) * red.size(), s))) return rc;

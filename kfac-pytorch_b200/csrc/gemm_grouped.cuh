@@ -11,6 +11,7 @@ struct GroupedGemm {
   int M, N, K;
   float alpha;
   int epi; const float* E; int64_t lde; const float* dg; const float* da; float damping;   // GemmEpilogue
+  const float* pi; int pi_side_m, pi_side_n;                                                 // EPI_DIV_FACTORED
   float* peerD[7]; int npeer;      // fused broadcast (mode 0, npeer <= 7): D is also stored into these peer copies, by
                                    // the tile epilogue, or by the reduce pass of a slab split (the same bits as D)
   int splits;                      // > 1: split-K -- deterministic through `slab` (plain epilogue), or mode 2

@@ -7,6 +7,8 @@ namespace kfac {
 
 constexpr int BM = 64, BN = 64, BK = 16;
 
+// FACTORED: the instantiation for EPI_DIV_FACTORED, kept apart so that the other epilogues keep their registers
+template <bool FACTORED>
 __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
   __shared__ __align__(16) float As[BK][BM + 4];
   __shared__ __align__(16) float Bs[BK][BN + 4];
@@ -74,6 +76,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
       if (g.epi == EPI_MUL) v *= g.E[(int64_t)m * g.lde + n];
       else if (g.epi == EPI_DIV_OUTER) v = v / (g.dg[m] * g.da[n] + g.damping);
       else if (g.epi == EPI_SQUARE) v = v * v;
+      else if (FACTORED) v = div_factored(v, g.dg[m], g.da[n], g.damping, g.pi, g.pi_side_m, g.pi_side_n);
       float* c = &C[(int64_t)m * g.ldc + n];
       if (g.atomic) atomicAdd(c, v);
       else *c = (g.beta == 0.f) ? v : (v + g.beta * (*c));
@@ -99,7 +102,8 @@ int launch_gemm(const GemmArgs& g0, cudaStream_t stream) {
     set_error("launch_gemm: grid too large (%u,%u,%u)", grid.x, grid.y, grid.z);
     return KFAC_ERR_BAD_ARG;
   }
-  gemm_simt_kernel<<<grid, 256, 0, stream>>>(g);
+  if (g.epi == EPI_DIV_FACTORED) gemm_simt_kernel<true><<<grid, 256, 0, stream>>>(g);
+  else gemm_simt_kernel<false><<<grid, 256, 0, stream>>>(g);
   KFAC_LAUNCH_CHECK();
   return KFAC_OK;
 }

@@ -23,10 +23,13 @@ struct TcParams {
   int tiles_m, tiles_n, splits, upper_only, atomic, accum;
   float alpha;
   int epi; const float* E; int64_t lde; const float* dg; const float* da; float damping;
+  const float* pi; int pi_side_m, pi_side_n;
   float* peerD[7]; int npeer;
   int64_t slab_stride;             // != 0: split sp writes to D + sp * slab_stride (plain stores, no atomics)
 };
 
+// FACTORED: the instantiation that also takes EPI_DIV_FACTORED (as in the grouped engine)
+template <bool FACTORED>
 struct GemmPolicy {
   using Params = TcParams;
   struct Item { int m0, n0, kb0, kb1, diag, sp; };
@@ -70,6 +73,8 @@ struct GemmPolicy {
       if (nb + j < p.N) {
         if (p.epi == EPI_MUL) x *= p.E[(int64_t)m * p.lde + nb + j];
         else if (p.epi == EPI_DIV_OUTER) x = x / (p.dg[m] * p.da[nb + j] + p.damping);
+        else if (FACTORED && p.epi == EPI_DIV_FACTORED)
+          x = div_factored(x, p.dg[m], p.da[nb + j], p.damping, p.pi, p.pi_side_m, p.pi_side_n);
       }
       v[j] = x;
     }
@@ -179,7 +184,9 @@ int launch_tc_gemm(const TcGemmArgs& a, cudaStream_t stream) {
     int dev = 0;
     KFAC_CUDA(cudaGetDevice(&dev));
     KFAC_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-    KFAC_CUDA(cudaFuncSetAttribute(tc::pipeline_kernel<GemmPolicy>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    KFAC_CUDA(cudaFuncSetAttribute(tc::pipeline_kernel<GemmPolicy<false>>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)tc::PSMEM));
+    KFAC_CUDA(cudaFuncSetAttribute(tc::pipeline_kernel<GemmPolicy<true>>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    (int)tc::PSMEM));
     attr = true;
   }
@@ -193,6 +200,7 @@ int launch_tc_gemm(const TcGemmArgs& a, cudaStream_t stream) {
   p.upper_only = a.upper_only; p.atomic = a.atomic; p.alpha = a.alpha; p.accum = a.accumulate;
   if (a.accumulate && (a.atomic || a.npeer > 0 || a.splits > 1)) { set_error("tc_gemm: accumulate needs the plain single-split epilogue"); return KFAC_ERR_BAD_ARG; }
   p.epi = a.epi; p.E = a.E; p.lde = a.lde; p.dg = a.dg; p.da = a.da; p.damping = a.damping;
+  p.pi = a.pi; p.pi_side_m = a.pi_side_m; p.pi_side_n = a.pi_side_n;
   p.npeer = a.npeer;
   for (int q = 0; q < a.npeer && q < 7; ++q) p.peerD[q] = a.peerD[q];
   if (a.npeer > 0 && (a.atomic || a.upper_only)) { set_error("tc_gemm: peer stores need the plain-store epilogue"); return KFAC_ERR_BAD_ARG; }
@@ -210,7 +218,8 @@ int launch_tc_gemm(const TcGemmArgs& a, cudaStream_t stream) {
   if (a.slab) { p.D = a.slab; p.slab_stride = a.slab_stride; }
   const int total = ntiles * splits;
   const int grid = std::min(total, num_sms);
-  tc::pipeline_kernel<GemmPolicy><<<grid, tc::PTHREADS, tc::PSMEM, stream>>>(p, total);
+  if (p.epi == EPI_DIV_FACTORED) tc::pipeline_kernel<GemmPolicy<true>><<<grid, tc::PTHREADS, tc::PSMEM, stream>>>(p, total);
+  else tc::pipeline_kernel<GemmPolicy<false>><<<grid, tc::PTHREADS, tc::PSMEM, stream>>>(p, total);
   KFAC_LAUNCH_CHECK();
   return KFAC_OK;
 }

@@ -4,6 +4,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <vector>
 
 #include "common.cuh"
@@ -138,8 +139,10 @@ __global__ void __launch_bounds__(256) update_all_kernel(const GradDev* items, i
   }
 }
 
-// out[i][j] = Q[i][j] / (d[j] + damping), zero in the padding columns
-__global__ void scale_cols_kernel(const float* Q, int ldq, const float* d, int n, float damping, float* out) {
+// out[i][j] = Q[i][j] / (d[j] + damping), zero in the padding columns; with pi, damping is pi_gamma(damping, *pi, side)
+__global__ void scale_cols_kernel(const float* Q, int ldq, const float* d, int n, float damping, const float* pi,
+                                  int side, float* out) {
+  if (pi) damping = pi_gamma(damping, *pi, side);
   const int64_t total = (int64_t)n * ldq;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (int64_t)gridDim.x * blockDim.x) {
@@ -218,8 +221,9 @@ using namespace kfac;
 
 static inline int ld4(int x) { return (x + 3) & ~3; }
 
-extern "C" int kfac_inverse_from_eigh(const float* Q, int ldq, const float* d, int n, float damping,
-                                      float* inv, int ld_inv, void* ws, size_t ws_bytes, void* stream) {
+// inv = Q diag(1 / (d + gamma)) Q^T with gamma = damping, or pi_gamma(damping, *pi, side) with pi
+static int inverse_from_eigh(const float* Q, int ldq, const float* d, int n, float damping, const float* pi, int side,
+                             float* inv, int ld_inv, void* ws, size_t ws_bytes, void* stream) {
   KFAC_CHECK_ARG(Q && d && inv && n > 0 && ldq >= n && ld_inv >= n, "inverse args");
   const size_t need = (size_t)n * ldq * sizeof(float);
   if (!ws || ws_bytes < need) {
@@ -228,10 +232,21 @@ extern "C" int kfac_inverse_from_eigh(const float* Q, int ldq, const float* d, i
   }
   cudaStream_t s = (cudaStream_t)stream;
   float* T = (float*)ws;
-  scale_cols_kernel<<<grid_for((int64_t)n * ldq), 256, 0, s>>>(Q, ldq, d, n, damping, T);
+  scale_cols_kernel<<<grid_for((int64_t)n * ldq), 256, 0, s>>>(Q, ldq, d, n, damping, pi, side, T);
   KFAC_LAUNCH_CHECK();
   // inv[i][j] = sum_k T[i][k] Q[j][k]; the same bits in every call (for n > 1024 the chains of gemm_tn)
   return gemm_tn(T, ldq, Q, ldq, inv, ld_inv, n, n, n, Epi{}, s);
+}
+
+extern "C" int kfac_inverse_from_eigh(const float* Q, int ldq, const float* d, int n, float damping,
+                                      float* inv, int ld_inv, void* ws, size_t ws_bytes, void* stream) {
+  return inverse_from_eigh(Q, ldq, d, n, damping, nullptr, 0, inv, ld_inv, ws, ws_bytes, stream);
+}
+
+extern "C" int kfac_inverse_from_eigh_pi(const float* Q, int ldq, const float* d, int n, float s, const float* pi,
+                                         int side, float* inv, int ld_inv, void* ws, size_t ws_bytes, void* stream) {
+  KFAC_CHECK_ARG(pi && (side == 1 || side == -1), "inverse_pi args");
+  return inverse_from_eigh(Q, ldq, d, n, s, pi, side, inv, ld_inv, ws, ws_bytes, stream);
 }
 
 extern "C" int kfac_transpose(const float* src, int ld_src, float* dst, int ld_dst, int rows, int cols,
@@ -263,6 +278,7 @@ struct DiagItem {
   int ldq;
   const float* vrow2;
   float damping;
+  int side_row;   // the factor of vrow under pi-adjusted damping: +1 A, -1 G (vcol is the other one)
 };
 
 static bool is_diag_a(const kfac_precond_item& it) { return it.kind == KFAC_ITEM_DIAG_A; }
@@ -300,6 +316,13 @@ static GroupedGemm div_outer(GroupedGemm g, const float* dg, const float* da, fl
   return g;
 }
 
+// the product divided by (dm[m] + gamma_m) (dn[n] + gamma_n) in its epilogue, gamma_m = pi_gamma(s, *pi, side_m)
+static GroupedGemm div_factored(GroupedGemm g, const float* dm, const float* dn, const float* pi, float s, int side_m,
+                                int side_n) {
+  g.epi = EPI_DIV_FACTORED; g.dg = dm; g.da = dn; g.pi = pi; g.damping = s; g.pi_side_m = side_m; g.pi_side_n = side_n;
+  return g;
+}
+
 #define PLAN_CHECK(cond, what) \
   do { if (!p.err && !(cond)) fail(KFAC_ERR_BAD_ARG, "bad argument: " what " (" #cond ")"); } while (0)
 
@@ -312,7 +335,14 @@ static ItemPlan plan_item(const kfac_precond_item& it, int method, float damping
   PLAN_CHECK(it.kind == KFAC_ITEM_DENSE || it.kind == KFAC_ITEM_EMBEDDING || it.kind == KFAC_ITEM_DIAG_G ||
                  it.kind == KFAC_ITEM_TIED || it.kind == KFAC_ITEM_DIAG_A, "precond item kind");
   PLAN_CHECK(it.n_peers >= 0 && it.n_peers <= 7 && (it.n_peers == 0 || it.peer_P), "precond peers");
+  PLAN_CHECK(!it.pi || it.kind != KFAC_ITEM_TIED, "precond tied item pi");
   const bool eigen = method == KFAC_EIGEN;
+  // the division of an item's eigenvalues (or diagonal factor): by (u v + damping), or with pi by the factored
+  // (u + gamma_u)(v + gamma_v) with s = sqrt(damping); side 0 is a vector of ones, which takes no damping
+  const float s = std::sqrt(damping);
+  auto divide = [&](GroupedGemm g, const float* u, const float* v, int side_u, int side_v) {
+    return it.pi ? div_factored(g, u, v, it.pi, s, side_u, side_v) : div_outer(g, u, v, damping);
+  };
   GroupedGemm* st = p.stage;
   if (it.kind == KFAC_ITEM_DENSE) {
     PLAN_CHECK(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= it.a, "precond item");
@@ -331,7 +361,7 @@ static ItemPlan plan_item(const kfac_precond_item& it, int method, float damping
       // (2) V2[g', a'] = (sum_k QgT[g', k] T^T[a', k]) * dgda[g', a'], or / (dg[g'] da[a'] + damping)   (g x a, K = g)
       st[1] = product(it.qgT, it.ldqg, w.t1, ld4(g), w.t2, ld4(a), g, a, g);
       if (it.dgda) { st[1].epi = EPI_MUL; st[1].E = it.dgda; st[1].lde = it.ld_dgda; }
-      else st[1] = div_outer(st[1], it.dg, it.da, damping);
+      else st[1] = divide(st[1], it.dg, it.da, -1, 1);
       // (3) U^T[c, g'] = sum_k Qa[c, k] V2[g', k]                                  (a x g, K = a, stage (1)'s slab)
       st[2] = product(it.qa, it.ldqa, w.t2, ld4(a), w.t1, ld4(g), a, g, a, chain_splits(a));
       p.slab_of[2] = 0;
@@ -344,16 +374,16 @@ static ItemPlan plan_item(const kfac_precond_item& it, int method, float damping
     switch (it.kind) {
       case KFAC_ITEM_EMBEDDING:
       case KFAC_ITEM_DIAG_A:
-        D = DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg, nullptr, 0.f};
+        D = DiagItem{it.a, it.g, it.qg, it.qgT, it.g_inv, it.da, it.dg, it.ldqg, nullptr, 0.f, 1};
         not_ready = is_diag_a(it) ? "precondition: the second-order data of a diagonal-A layer has not been computed"
                                   : "precondition: the second-order data of an embedding layer has not been computed";
         break;
       case KFAC_ITEM_TIED:
-        D = DiagItem{it.a, it.g, it.qg, it.qgT, nullptr, it.da, it.dg, it.ldqg, it.dh, it.tied_damping};
+        D = DiagItem{it.a, it.g, it.qg, it.qgT, nullptr, it.da, it.dg, it.ldqg, it.dh, it.tied_damping, 1};
         not_ready = "precondition: the second-order data of a tied embedding / head pair has not been computed";
         break;
       default:                          // KFAC_ITEM_DIAG_G, or a kind the first check rejects
-        D = DiagItem{it.g, it.a, it.qa, it.qaT, it.a_inv, it.dg, it.da, it.ldqa, nullptr, 0.f};
+        D = DiagItem{it.g, it.a, it.qa, it.qaT, it.a_inv, it.dg, it.da, it.ldqa, nullptr, 0.f, -1};
         not_ready = "precondition: the second-order data of a diagonal-G layer has not been computed";
     }
     PLAN_CHECK(it.wgrad && it.P && it.g > 0 && it.a > 0 && it.ldp >= (is_diag_a(it) ? D.rows : D.n) &&
@@ -372,19 +402,19 @@ static ItemPlan plan_item(const kfac_precond_item& it, int method, float damping
       // (1) T[v, j] = (sum_k grad[v, k] Q[k, j]) / (vrow[v] vcol[j] + damping), the division of a tied item by
       // tied_scale_kernel                                                                      (rows x n, K = n)
       st[0] = product(w.gr, ldn, D.qT, D.ldq, w.t1, ldn, D.rows, D.n, D.n);
-      if (!tied) st[0] = div_outer(st[0], D.vrow, D.vcol, damping);
+      if (!tied) st[0] = divide(st[0], D.vrow, D.vcol, D.side_row, -D.side_row);
       else { p.tied = true; p.tied_scale = TiedScaleDev{w.t1, D.vrow, D.vrow2, D.vcol, D.damping, D.n, ldn, 0}; }
     }
     if (is_diag_a(it)) {
       // (4) P[r, c] = sum_k Qg[r, k] T[c, k], or (sum_k Ginv[r, k] grad^T[c, k]) / (a[c] + damping)   (g x a, K = g)
       st[3] = eigen ? product(D.q, D.ldq, w.t1, ldn, it.P, it.ldp, D.n, D.rows, D.n)
-                    : div_outer(product(D.inv, D.ldq, w.gr, ldn, it.P, it.ldp, D.n, D.rows, D.n), w.ones, D.vrow,
-                                damping);
+                    : divide(product(D.inv, D.ldq, w.gr, ldn, it.P, it.ldp, D.n, D.rows, D.n), w.ones, D.vrow, 0,
+                             D.side_row);
     } else {
       // (4) P[v, c] = sum_k T[v, k] Q[c, k], or (sum_k grad[v, k] Inv[c, k]) / (vrow[v] + damping)  (rows x n, K = n)
       st[3] = eigen || tied ? product(w.t1, ldn, D.q, D.ldq, it.P, it.ldp, D.rows, D.n, D.n)
-                            : div_outer(product(w.gr, ldn, D.inv, D.ldq, it.P, it.ldp, D.rows, D.n, D.n), D.vrow,
-                                        w.ones, damping);
+                            : divide(product(w.gr, ldn, D.inv, D.ldq, it.P, it.ldp, D.rows, D.n, D.n), D.vrow,
+                                     w.ones, D.side_row, 0);
     }
   }
   // the last product splits where it has the plain epilogue and P is at its padded width

@@ -1097,6 +1097,8 @@ class KFACLayer:
         # factors
         self.tied_head: KFACLayer | None = None
         self.tied_embedding: KFACLayer | None = None
+        # pi-adjusted damping (set by the preconditioner): the damping is split between A and G by their trace norms
+        self.pi_damping = False
         self.index = -1
         # arena views (bound by the preconditioner)
         self._a_view = self._g_view = None

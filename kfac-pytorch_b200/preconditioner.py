@@ -119,6 +119,21 @@ def _tie_pairs(layers: dict[torch.nn.Module, tuple[str, KFACLayer]], compute_met
     # a weight shared by two Linears (with or without an embedding) stays refused by the checks that follow
 
 
+def _enable_pi_damping(layers: dict[torch.nn.Module, tuple[str, KFACLayer]], compute_method: ComputeMethod) -> None:
+    """Turn on pi-adjusted damping for every registered layer of the work assignment (normalization layers keep their
+    damping), refusing the layers it does not cover."""
+    for name, l in layers.values():
+        if compute_method == ComputeMethod.EKFAC:
+            raise ValueError(f'pi_damping does not support compute_method=EKFAC (layer "{name}"), which damps its '
+                             'measured second moments directly; add the layers to skip_layers or set pi_damping=False')
+        if l.tied_head is not None:
+            head = next(n for n, hl in layers.values() if hl is l.tied_head)
+            raise ValueError(f'pi_damping does not support the tied embedding / head pair "{name}" / "{head}"; add one '
+                             'of the two layers to skip_layers or set pi_damping=False')
+    for _, l in layers.values():
+        l.pi_damping = True
+
+
 class KFACPreconditioner(BaseKFACPreconditioner):
     """K-FAC gradient preconditioner with KAISA placement on H100 (sm_90a).
 
@@ -280,6 +295,25 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     ValueError naming the layer and `skip_layers`: EKFAC, a match on an embedding, a normalization layer, an attention
     projection, a recurrent sub-layer or a transposed convolution, a layer matched by `diagonal_g_layers` too, a G
     above 8192, and a weight shared with another registered module.
+
+    `pi_damping=True` splits the damping between the two Kronecker factors of every registered layer by their trace
+    norms (factored Tikhonov damping with the trace-norm pi, Martens & Grosse 2015, sec. 6.3; `compute_pi_tracenorm` in
+    TF K-FAC, pi-adjusted damping in KFAC-JAX).  A (x) G equals cA (x) G/c for any c > 0, and how a layer's statistics
+    split the scale between A and G differs a lot between layer kinds (a conv layer's 1/S, an embedding's token
+    frequencies, a loss that is a mean over tokens).  With
+        pi = sqrt((tr A / a_dim) / (tr G / g_dim)),    s = sqrt(damping),    gamma_A = s pi,    gamma_G = s / pi
+    (pi = 1 where a mean trace is not a positive finite number; a diagonal factor's trace is the sum of its vector) the
+    layer is preconditioned by (A + gamma_A I) (x) (G + gamma_G I), which does not depend on that split:
+        eigen:   P = Qg [(Qg^T grad Qa) / ((dg + gamma_G) x (da + gamma_A))] Qa^T
+        inverse: P = (G + gamma_G I)^-1 grad (A + gamma_A I)^-1
+    and the same formulas for embeddings, diagonal-G and diagonal-A layers.  This is the Tikhonov damping of the
+    product, so each factor receives sqrt(damping): the inverse method's damping changes meaning relative to
+    `pi_damping=False`.  pi is formed at every inverse step (and by `load_state_dict(compute_inverses=True)`) from the
+    factors that step decomposes, by every rank for every layer, and kept until the next inverse step; it needs no
+    collective and is not part of `state_dict()`.  The damping of the inverse step forms dgda and the inverses, the
+    damping of the step that preconditions divides by the eigenvalues without `compute_eigenvalue_outer_product` and
+    by the diagonal factors.  Normalization layers keep their blocks damped by `damping`.  Refused with a ValueError
+    naming the layer: EKFAC (which damps its measured S directly) and tied embedding / head pairs.
     """
 
     def __init__(
@@ -317,7 +351,10 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         precondition_group_norms: bool = False,
         precondition_recurrent: bool = False,
         diagonal_a_layers: list[str] | None = None,
+        pi_damping: bool = False,
     ) -> None:
+        if not isinstance(pi_damping, bool):
+            raise ValueError(f'pi_damping must be a bool, got {pi_damping!r}')
         if allreduce_bucket_cap_mb < 0:
             raise ValueError('allreduce_bucket_cap_mb must be >= 0')
         if kfac_approx not in ('expand', 'reduce'):
@@ -412,6 +449,8 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         norm_layers = {m: v for m, v in kfac_layers.items() if v[1].norm}
         kfac_layers = {m: v for m, v in kfac_layers.items() if not v[1].norm}
         _check_diagonal_layers(kfac_layers, compute_method, tied_embeddings=precondition_tied_embeddings)
+        if pi_damping:
+            _enable_pi_damping(kfac_layers, compute_method)
         for name, kfac_layer in list(kfac_layers.values()) + list(norm_layers.values()):
             logger.log(loglevel, f'Registered name="{name}": {repr(kfac_layer)}')
 
@@ -449,6 +488,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'precondition_group_norms': precondition_group_norms,
             'precondition_recurrent': precondition_recurrent,
             'diagonal_a_layers': diagonal_a_layers,
+            'pi_damping': pi_damping,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
