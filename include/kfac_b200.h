@@ -197,6 +197,31 @@ enum kfac_index_dtype { KFAC_I32 = 3, KFAC_I64 = 4 };
 size_t kfac_factor_embedding_workspace_bytes(int V);
 int kfac_factor_embedding(const void* idx, int index_dtype, int64_t N, int V, float alpha,
                           float* acc, void* ws, size_t ws_bytes, void* stream);
+/* Embedding bags (nn.EmbeddingBag, opt-in): bag b of B pools its entries into the row c_b of a
+ * Linear layer on R^V,
+ *   KFAC_BAG_SUM:  c_bv = sum_{i in b, t_i = v} w_i      (w_i = weights[i], or 1)
+ *   KFAC_BAG_MEAN: c_bv = n_bv / L_b                     (c_b = 0 for an empty bag)
+ * where entries equal to padding_idx (>= 0; -1 for none) are left out and L_b counts the others.
+ * kfac_factor_embedding_bag keeps the diagonal of (1/B) C^T C:  acc[v] += alpha * sum_b c_bv^2
+ * (alpha = 1/B).  Bags of one index give the bits of kfac_factor_embedding on the same indices.
+ * idx: N int32 / int64 indices in [0, V) (index_dtype), trusted like kfac_factor_embedding's.
+ *   offsets != NULL: idx is 1-D and bag b is [offsets[b], offsets[b + 1]), the last bag ending
+ *     at N.  Only the first B offsets are read (include_last_offset's extra entry is not: as in
+ *     torch, the last bag ends at N).  offsets has index_dtype, is non-decreasing, starts at 0
+ *     and is read on the device.
+ *   offsets == NULL: idx is (B, N / B) row-major, one bag per row.
+ * weights: NULL, or N per-sample weights of weight_dtype (KFAC_F32/F16/BF16), KFAC_BAG_SUM only.
+ * c_bv is formed in fp64 (weights summed in entry order), squared and summed over the bags in bag
+ * order in fp64, rounded once to fp32 as s_v, then acc[v] = fl(acc[v] + fl(alpha * s_v)).  The
+ * (token, bag) pairs are grouped by a stable radix sort on the token (CUB): no floating-point
+ * atomics, the same bits on every run, no host sync.  ws: kfac_factor_embedding_bag_workspace_bytes
+ * (N, B, V) bytes (N < 2^31). */
+enum kfac_bag_mode { KFAC_BAG_SUM = 0, KFAC_BAG_MEAN = 1 };
+size_t kfac_factor_embedding_bag_workspace_bytes(int64_t N, int64_t B, int V);
+int kfac_factor_embedding_bag(const void* idx, const void* offsets, int index_dtype, int64_t N,
+                              int64_t B, int64_t padding_idx, int mode,
+                              const void* weights, int weight_dtype, int V, float alpha,
+                              float* acc, void* ws, size_t ws_bytes, void* stream);
 /* EMA of diagonal factors (vectors of d = V floats), the schedule of kfac_factor_ema on the
  * diagonal and with the same rounding (the bits kfac_factor_ema gives on diag(batch)):
  *   factor = alpha*(first ? 1 : factor) + (1-alpha)*inv_count*batch;   batch = 0

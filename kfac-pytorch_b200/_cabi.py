@@ -27,6 +27,7 @@ KFAC_ITEM_DENSE, KFAC_ITEM_EMBEDDING, KFAC_ITEM_DIAG_G, KFAC_ITEM_TIED, KFAC_ITE
 
 DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 INDEX_DTYPE_CODE = {torch.int32: 3, torch.int64: 4}
+KFAC_BAG_SUM, KFAC_BAG_MEAN = 0, 1
 
 
 class ConvGeometry(C.Structure):
@@ -136,6 +137,9 @@ SIGNATURES = {
     'kfac_factor_embedding_workspace_bytes': (c_size_t, [c_int]),
     'kfac_factor_embedding': (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_void_p, c_void_p, c_size_t,
                                       c_void_p]),
+    'kfac_factor_embedding_bag_workspace_bytes': (c_size_t, [c_int64, c_int64, c_int]),
+    'kfac_factor_embedding_bag': (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_int64, c_int, c_void_p, c_int,
+                                          c_int, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     'kfac_factor_ema_diag': (c_int, [C.POINTER(EmaItem), c_int, c_float, c_void_p]),
     'kfac_factor_ema_diag_guarded_workspace_bytes': (c_size_t, [c_int]),
     'kfac_factor_ema_diag_guarded': (c_int, [C.POINTER(EmaItem), c_int, c_float, C.POINTER(c_void_p), c_void_p,

@@ -993,13 +993,14 @@ class BaseKFACPreconditioner:
         flags = None
         # diagonal factors (an embedding's or a diagonal-A layer's A, a diagonal-G layer's G) take the EMA of vectors.
         # A window of token counts is finite whatever the loss scale and is never guarded; a diagonal A of activations
-        # and a diagonal G are guarded like every dense A and G.  The blocks of a normalization layer (G side) are
+        # or of an embedding bag's pooled rows (per-sample weights are forward values) and a diagonal G are guarded like
+        # every dense A and G.  The blocks of a normalization layer (G side) are
         # element-wise too and take the same path
         def vec(l, w):
             return l.diag_side == w or l.norm
 
         def guard(l, w):
-            return self._guard_factors and (w == 'g' or not l.embedding)
+            return self._guard_factors and (w == 'g' or not l.module.counts_a)
         split = {alpha: ([(l, w) for l, w in todo if vec(l, w) and not guard(l, w)],
                          [(l, w) for l, w in todo if vec(l, w) and guard(l, w)],
                          [(l, w) for l, w in todo if not vec(l, w)])

@@ -6,7 +6,7 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 ARCH="-gencode arch=compute_90a,code=sm_90a"
 FLAGS="$ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC"
 OBJS=""
-for f in api gemm_simt gemm_tc gemm_grouped factor eigh sytrd stedc eigh_direct precond ekfac norm reduce tied recurrent $EXTRA_SRCS; do
+for f in api gemm_simt gemm_tc gemm_grouped factor eigh sytrd stedc eigh_direct precond ekfac norm reduce tied recurrent embedding_bag $EXTRA_SRCS; do
   if [ ! -f $f.o ] || [ $f.cu -nt $f.o ] || [ common.cuh -nt $f.o ] || [ tc_common.cuh -nt $f.o ] || [ tc_pipeline.cuh -nt $f.o ] || [ ../../include/kfac_b200.h -nt $f.o ] || [ eigh_direct.cuh -nt $f.o ] || [ gemm_grouped.cuh -nt $f.o ] || [ build.sh -nt $f.o ]; then
     echo "nvcc $f.cu"
     $NVCC $FLAGS ${PTXAS_V:+-Xptxas -v} -c $f.cu -o $f.o

@@ -41,7 +41,8 @@ class ModuleHelper:
 
     diagonal_a = False      # True: A is kept as a vector (embeddings; Linear and convolutions in diagonal_a_layers)
     diagonal_g = False      # True: G is approximated by its diagonal and kept as a vector (diagonal_g_layers)
-    embedding = False       # True: an nn.Embedding (its diagonal A is exact, its input indices, P is (V, d))
+    embedding = False       # True: an nn.Embedding or EmbeddingBag (a diagonal A, its input indices, P is (V, d))
+    counts_a = False        # True: A counts the input indices, so it is finite whatever the forward values
     norm = False            # True: exact per-channel Fisher blocks instead of two factors (precondition_norms)
     call_kwargs = False     # True: the A hook passes every call's arguments to bind_call (output_size)
     # 0: the weight gradient is the row-major (g, a - has_bias) gradient matrix; T > 0: it is (C_in, g, T), a transposed
@@ -608,6 +609,7 @@ class EmbeddingModuleHelper(LinearModuleHelper):
 
     diagonal_a = True
     embedding = True
+    counts_a = True
 
     @property
     def a_factor_shape(self):
@@ -638,6 +640,71 @@ class EmbeddingModuleHelper(LinearModuleHelper):
         _cabi.check(lib.kfac_factor_embedding(x.data_ptr(), code, n, V, 1.0 / n, acc.data_ptr(),
                                               _workspace(scratch, need, x.device), need, _cabi.stream_ptr()),
                     'kfac_factor_embedding')
+
+
+class EmbeddingBagModuleHelper(EmbeddingModuleHelper):
+    """torch.nn.EmbeddingBag with mode 'sum' or 'mean' (an extension beyond the reference, opt-in through
+    `precondition_embedding_bags`).
+
+    Bag b pools its entries into the row c_b in R^V of a Linear layer, output_b = W^T c_b and weight.grad = C^T g:
+    c_bv = sum of the per-sample weights (or 1) of its entries equal to v ('sum'), or n_bv / L_b ('mean', L_b the
+    bag's non-padding entries; an empty bag is a zero row), `padding_idx` entries left out.  A = (1/B) C^T C is V x V
+    and not diagonal once a bag holds two distinct tokens; its diagonal (1/B) sum_b c_bv^2 is kept, a vector of V
+    floats, exact for bags of one index (where it is nn.Embedding's A).  Every bag, empty or not, is one row (N = B),
+    also under K-FAC-reduce.  G is formed from the rows of the (B, d) output gradient like a Linear layer's.  The
+    gradient and P use the weight's layout (V x d).  The call's `offsets` and `per_sample_weights` reach the A
+    statistic through bind_call."""
+
+    call_kwargs = True
+    counts_a = False
+
+    def __init__(self, module: torch.nn.Module):
+        super().__init__(module)
+        self._call: tuple[torch.Tensor | None, torch.Tensor | None] = (None, None)
+
+    def bind_call(self, args: tuple, kwargs: dict) -> None:
+        """Take the offsets and per-sample weights of a forward call, positional or keyword."""
+        offsets = args[1] if len(args) > 1 else kwargs.get('offsets')
+        weights = args[2] if len(args) > 2 else kwargs.get('per_sample_weights')
+        self._call = (offsets, weights)
+
+    def accumulate_a(self, x, acc, scratch):
+        """acc += the diagonal of the pooled rows' C^T C / B for the call bind_call saw."""
+        offsets, weights = self._call
+        self._call = (None, None)
+        m = self.module
+        x = _detached(x)
+        if x.dim() == 2:
+            B, offsets = x.size(0), None
+        elif x.dim() == 1 and offsets is not None:
+            offsets = _detached(offsets)
+            B = offsets.numel() - int(m.include_last_offset)
+            if offsets.dtype != x.dtype:        # torch promotes mixed index and offset dtypes to int64
+                x, offsets = x.long(), offsets.long()
+            offsets = _dense(offsets)
+        else:
+            raise ValueError(f'EmbeddingBag: input of shape {tuple(x.shape)} (1-D input needs offsets)')
+        try:
+            code = _cabi.INDEX_DTYPE_CODE[x.dtype]
+        except KeyError:
+            raise ValueError(f'unsupported embedding bag index dtype {x.dtype}') from None
+        x = _dense(x)
+        n = x.numel()
+        if n == 0 or B <= 0:
+            return
+        wcode = 0
+        if weights is not None:
+            weights = _dense(cast_for_factor(_detached(weights), None))
+            wcode = _dtype_code(weights)
+        V = m.num_embeddings
+        mode = {'sum': _cabi.KFAC_BAG_SUM, 'mean': _cabi.KFAC_BAG_MEAN}[m.mode]
+        lib = _cabi.load()
+        need = lib.kfac_factor_embedding_bag_workspace_bytes(n, B, V)
+        _cabi.check(lib.kfac_factor_embedding_bag(x.data_ptr(), offsets.data_ptr() if offsets is not None else None,
+                                                  code, n, B, -1 if m.padding_idx is None else m.padding_idx, mode,
+                                                  weights.data_ptr() if weights is not None else None, wcode, V,
+                                                  1.0 / B, acc.data_ptr(), _workspace(scratch, need, x.device), need,
+                                                  _cabi.stream_ptr()), 'kfac_factor_embedding_bag')
 
 
 class DiagonalGLinearModuleHelper(LinearModuleHelper):
@@ -1020,6 +1087,7 @@ CONV2D_TYPES: tuple[type, ...] = (torch.nn.Conv2d,)
 CONV_ND_TYPES: tuple[type, ...] = (torch.nn.Conv1d, torch.nn.Conv3d)
 CONV_TRANSPOSE_TYPES: tuple[type, ...] = (torch.nn.ConvTranspose1d, torch.nn.ConvTranspose2d, torch.nn.ConvTranspose3d)
 EMBEDDING_TYPES: tuple[type, ...] = (torch.nn.Embedding,)
+EMBEDDING_BAG_TYPES: tuple[type, ...] = (torch.nn.EmbeddingBag,)
 # SyncBatchNorm (global statistics) and BatchNorm3d are in neither tuple; GroupNorm and InstanceNorm* are registered
 # through their own keyword (precondition_group_norms)
 NORM_TYPES: tuple[type, ...] = (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d, torch.nn.LayerNorm, torch.nn.RMSNorm)
@@ -1032,11 +1100,12 @@ RECURRENT_TYPES: tuple[type, ...] = (torch.nn.RNN, torch.nn.LSTM, torch.nn.GRU)
 def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
                       diagonal_g: bool = False, norms: bool = False, reduce: bool = False,
                       conv_nd: bool = False, conv_transpose: bool = False,
-                      group_norms: bool = False, diagonal_a: bool = False) -> ModuleHelper | None:
+                      group_norms: bool = False, diagonal_a: bool = False,
+                      embedding_bags: bool = False) -> ModuleHelper | None:
     """reduce: K-FAC-reduce statistics for Linear (dense and diagonal-G), Conv2d and (with conv_nd) Conv1d / Conv3d
-    and (with conv_transpose) ConvTranspose1d / 2d / 3d layers; embeddings and normalization layers keep their own
-    statistics.  diagonal_a: a diagonal A for a Linear, Conv2d or (with conv_nd) Conv1d / Conv3d layer; the other
-    kinds ignore it (register_modules refuses them)."""
+    and (with conv_transpose) ConvTranspose1d / 2d / 3d layers; embeddings, embedding bags and normalization layers keep
+    their own statistics.  diagonal_a: a diagonal A for a Linear, Conv2d or (with conv_nd) Conv1d / Conv3d layer; the
+    other kinds ignore it (register_modules refuses them)."""
     if isinstance(module, LINEAR_TYPES):
         if diagonal_g:
             return DiagonalGLinearModuleHelper(module, reduce=reduce)
@@ -1049,6 +1118,8 @@ def get_module_helper(module: torch.nn.Module, embeddings: bool = False,
         return ConvTransposeModuleHelper(module, reduce=reduce)
     if embeddings and isinstance(module, EMBEDDING_TYPES):
         return EmbeddingModuleHelper(module)
+    if embedding_bags and isinstance(module, EMBEDDING_BAG_TYPES):
+        return EmbeddingBagModuleHelper(module)
     if norms and isinstance(module, NORM_TYPES) and getattr(module, 'weight', None) is not None:
         return NormModuleHelper(module)      # affine=False / elementwise_affine=False: nothing to precondition
     if group_norms and isinstance(module, GROUP_NORM_TYPES) and getattr(module, 'weight', None) is not None:
@@ -1085,7 +1156,7 @@ class KFACLayer:
         self.g_dim = module.g_factor_shape[0]
         # A is a vector of a_dim floats (embeddings, diagonal_a_layers)
         self.diag_a = module.diagonal_a
-        # an nn.Embedding: its input is indices, and P has the weight's layout (a x g) instead of (g x a)
+        # an nn.Embedding or EmbeddingBag: its input is indices, and P has the weight's layout (a x g), not (g x a)
         self.embedding = module.embedding
         # G is a vector of g_dim floats (diagonal_g_layers); P keeps the dense layout (g x a)
         self.diag_g = module.diagonal_g
@@ -1263,7 +1334,7 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
                      kfac_approx: str = 'expand', precondition_attention: bool = False,
                      precondition_conv_nd: bool = False, precondition_conv_transpose: bool = False,
                      precondition_group_norms: bool = False, precondition_recurrent: bool = False,
-                     diagonal_a_layers: list[str] | None = None,
+                     diagonal_a_layers: list[str] | None = None, precondition_embedding_bags: bool = False,
                      **layer_kwargs: Any) -> dict[torch.nn.Module, tuple[str, KFACLayer]]:
     """Leaf-module discovery with regex skip on name and class name
     (kfac/layers/register.py:57-95).  precondition_embeddings: also register torch.nn.Embedding
@@ -1284,7 +1355,8 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
     RecurrentSubLayerHelper (not in the reference).  diagonal_a_layers: regexes on name and class name; a registered
     torch.nn.Linear, Conv2d or (precondition_conv_nd) Conv1d / Conv3d that matches keeps a diagonal A and may have an A
     above the eigensolver's limit (not in the reference); any other registered module that matches, a match of
-    diagonal_g_layers too and a G above the limit are errors.  `layer.index` counts the other layers and the
+    diagonal_g_layers too and a G above the limit are errors.  precondition_embedding_bags: also register
+    torch.nn.EmbeddingBag modules (not in the reference).  `layer.index` counts the other layers and the
     normalization layers separately."""
     diagonal_g_layers = diagonal_g_layers or []
     diagonal_a_layers = diagonal_a_layers or []
@@ -1320,7 +1392,8 @@ def register_modules(model: torch.nn.Module, skip_layers: list[str], preconditio
         helper = get_module_helper(module, embeddings=precondition_embeddings, diagonal_g=diag_g,
                                    norms=precondition_norms, reduce=kfac_approx == 'reduce',
                                    conv_nd=precondition_conv_nd, conv_transpose=precondition_conv_transpose,
-                                   group_norms=precondition_group_norms, diagonal_a=diag_a and not diag_g)
+                                   group_norms=precondition_group_norms, diagonal_a=diag_a and not diag_g,
+                                   embedding_bags=precondition_embedding_bags)
         if helper is None:
             continue
         if diag_g and not helper.diagonal_g:

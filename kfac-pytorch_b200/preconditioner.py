@@ -66,16 +66,21 @@ def _check_diagonal_layers(layers: dict[torch.nn.Module, tuple[str, KFACLayer]],
     if tied_embeddings:
         _tie_pairs(layers, compute_method)
     for module, name, l in diag:
-        kind, keyword = (('embedding', 'precondition_embeddings') if l.embedding
+        bag = isinstance(module, torch.nn.EmbeddingBag)
+        kind, keyword = (('embedding bag', 'precondition_embedding_bags') if bag
+                         else ('embedding', 'precondition_embeddings') if l.embedding
                          else ('layer', 'diagonal_a_layers') if l.diag_a else ('layer', 'diagonal_g_layers'))
         if compute_method == ComputeMethod.EKFAC:
             raise ValueError(f'{keyword} does not support compute_method=EKFAC ({kind} "{name}"); '
                              f'add the {kind}s to skip_layers')
+        if bag and module.mode == 'max':
+            raise ValueError(f'embedding bag "{name}" has mode=\'max\': each output column reads a different row, so '
+                             'it is not a Kronecker-factored layer (add it to skip_layers)')
         if l.embedding and module.sparse:
-            raise ValueError(f'embedding "{name}" has sparse=True: K-FAC needs a dense weight gradient '
+            raise ValueError(f'{kind} "{name}" has sparse=True: K-FAC needs a dense weight gradient '
                              '(add it to skip_layers or use sparse=False)')
         if l.embedding and module.scale_grad_by_freq:
-            raise ValueError(f'embedding "{name}" has scale_grad_by_freq=True: its weight gradient is then not the '
+            raise ValueError(f'{kind} "{name}" has scale_grad_by_freq=True: its weight gradient is then not the '
                              'one the K-FAC factors model (add it to skip_layers)')
         for other, (other_name, _) in layers.items():
             if l.tied_head is not None or l.tied_embedding is not None:
@@ -89,7 +94,7 @@ def _tie_pairs(layers: dict[torch.nn.Module, tuple[str, KFACLayer]], compute_met
     """Form the tied pairs of precondition_tied_embeddings: a registered embedding and the one other registered module
     that owns its weight, which must be a bias-less torch.nn.Linear matched by diagonal_g_layers."""
     for module, (name, l) in layers.items():
-        if not l.embedding:
+        if not l.embedding or isinstance(module, torch.nn.EmbeddingBag):    # a bag never forms a pair
             continue
         owners = [(other, other_name, ol) for other, (other_name, ol) in layers.items()
                   if other is not module and any(p is module.weight for p in other.parameters())]
@@ -143,7 +148,8 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     `accumulation_steps=1` and, for integer schedules, `inv_update_steps` a multiple of
     `factor_update_steps`; `compute_eigenvalue_outer_product` is ignored with it.
 
-    `precondition_embeddings=True` also registers leaf `torch.nn.Embedding` modules (not `EmbeddingBag`), which
+    `precondition_embeddings=True` also registers leaf `torch.nn.Embedding` modules (`EmbeddingBag` has its own
+    keyword, `precondition_embedding_bags`), which
     the reference leaves to the first-order optimizer.  Their A factor is diagonal (the token frequencies) and
     kept as a vector; see `kfac_b200.layers.EmbeddingModuleHelper`.  The embedding's P is always formed from the
     eigenvalue vectors (`compute_eigenvalue_outer_product` does not apply to it, so no V x d matrix is stored),
@@ -314,6 +320,21 @@ class KFACPreconditioner(BaseKFACPreconditioner):
     damping of the step that preconditions divides by the eigenvalues without `compute_eigenvalue_outer_product` and
     by the diagonal factors.  Normalization layers keep their blocks damped by `damping`.  Refused with a ValueError
     naming the layer: EKFAC (which damps its measured S directly) and tied embedding / head pairs.
+
+    `precondition_embedding_bags=True` also registers leaf `torch.nn.EmbeddingBag` modules whose weight requires grad
+    (the bag-of-tokens text classifier, fastText-style n-gram models, the sparse-feature tables of DLRM-style
+    recommenders), independently of `precondition_embeddings`.  A call of B bags is a Linear layer on the pooled rows
+    c_b in R^V (c_bv the sum of the `per_sample_weights`, or 1, of bag b's entries equal to v for mode='sum'; their
+    count over the bag's non-padding entries for mode='mean'; `padding_idx` entries left out), so its A factor
+    (1/B) C^T C is V x V.  The bag keeps its diagonal A_v = (1/B) sum_b c_bv^2, a vector of V floats, exact for bags
+    of one index (where it is `nn.Embedding`'s A); this is a different approximation from the exact Fisher, hence
+    opt-in.  Every bag, empty or not, is one row, also under `kfac_approx='reduce'`.  G comes from the (B, d) output
+    gradient, and P, placement, collectives, `state_dict()` (A as a V-vector) and `memory_usage()` are an embedding's.
+    1-D indices with `offsets` (with or without `include_last_offset`) and 2-D indices are supported.  Under a
+    `grad_scaler` the bag's A takes the guarded EMA like a dense A (per-sample weights are forward values); without
+    one, a non-finite A makes the next `step()` raise.  Refused with a ValueError naming the layer and `skip_layers`:
+    mode='max', `sparse=True`, `scale_grad_by_freq=True`, EKFAC, a `diagonal_g_layers` or `diagonal_a_layers` match
+    and a weight shared with another registered module.
     """
 
     def __init__(
@@ -352,6 +373,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
         precondition_recurrent: bool = False,
         diagonal_a_layers: list[str] | None = None,
         pi_damping: bool = False,
+        precondition_embedding_bags: bool = False,
     ) -> None:
         if not isinstance(pi_damping, bool):
             raise ValueError(f'pi_damping must be a bool, got {pi_damping!r}')
@@ -442,7 +464,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             precondition_conv_transpose=precondition_conv_transpose,
             precondition_group_norms=precondition_group_norms,
             precondition_recurrent=precondition_recurrent, diagonal_a_layers=diagonal_a_layers,
-            method=compute_method,
+            precondition_embedding_bags=precondition_embedding_bags, method=compute_method,
             prediv_eigenvalues=compute_eigenvalue_outer_product, grad_scaler=grad_scaler,
             factor_dtype=factor_dtype, inv_dtype=inv_dtype, symmetry_aware=symmetry_aware)
         # normalization layers are preconditioned locally on every rank: the placement never sees them
@@ -489,6 +511,7 @@ class KFACPreconditioner(BaseKFACPreconditioner):
             'precondition_recurrent': precondition_recurrent,
             'diagonal_a_layers': diagonal_a_layers,
             'pi_damping': pi_damping,
+            'precondition_embedding_bags': precondition_embedding_bags,
         }
         super().__init__(
             kfac_layers, norm_layers=norm_layers, factor_update_steps=factor_update_steps,
